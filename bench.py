@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- ESKF frames/s and residuals/s of the FAST-LIVO measurement + iterated-ESKF hot
-path on B200 (BASELINE.json metric), with the reference-equivalent CPU path timed beside it.
+path on H100 (BASELINE.json metric), with the reference-equivalent CPU path timed beside it.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload C2] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload C2] [--impl reference] [--dump-outputs DIR]
 
 A *step* is one frame: one full LIO update (all passes, kNN on the rematch passes) followed by
 one full VIO update (ComputeJ: 3 pyramid levels) whose prior is the LIO posterior, on one
@@ -49,7 +49,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler:
@@ -144,6 +144,19 @@ class ClockSampler:
                 "reasons": sorted(self.reasons), "source": self.mode}
 
 
+def dump_outputs(d, x, lrep, vrep, has_vio):
+    """--dump-outputs DIR: what the caller of the timed path receives after its last step -- the posterior state
+    (rot, pos, vel, bg, ba, grav), its 18x18 covariance and the LIO / VIO reports -- as float64 .npy files."""
+    os.makedirs(d, exist_ok=True)
+    out = {"state": x.vector(), "cov": x.P,
+           "lio_report": [lrep.passes, lrep.knn_passes, lrep.n_eff_last, lrep.res_mean_last, lrep.rows_total,
+                          lrep.converged_last, lrep.status]}
+    if has_vio:
+        out["vio_report"] = [*vrep.passes, *vrep.last_error, vrep.rows_total, vrep.skipped_last, vrep.cov_updated, vrep.status]
+    for k, v in out.items():
+        np.save(os.path.join(d, k + ".npy"), np.asarray(v, np.float64))
+
+
 def pass_counts(cfg):
     """Fixed pass schedule with early stop disabled (SURVEY.md §8d / Appendix A): K LIO passes with
     kNN on the first and the last, K VIO passes on each of 3 levels."""
@@ -177,7 +190,8 @@ def cpu_frame_runner(po, frame, nthreads, tree="build"):
             vrep = vio.update(vprm, x, x.copy())
             rows += vrep.rows_total
         return x, rows
-    kind = "reference kNN (ikd_Tree.cpp via oracle/_ref) + line-cited C++ port of the rest" if tree else "port (brute-force kNN)"
+    kind = "reference kNN (ikd_Tree.cpp via oracle/_ref) + line-cited C++ port of the rest" if tree else \
+        "port (brute-force kNN: the reference's ikd-Tree was not built, the reference tree was not available to build())"
     return run, kind
 
 
@@ -433,29 +447,13 @@ class Rig:
         return fams
 
 
-def traffic_table():
-    """dram__bytes_read+write per launch of the persistent kernels from this round's ncu --set full captures
-    (profiles/r02_traffic.json, regenerated by profiles/make_traffic.py whenever a kernel changes)."""
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p):
-            with open(p) as f:
-                return json.load(f), name
-    return {}, None
-
-
 def roofline_of(fams, hbm, peak_src, workload, note):
     dom = max((f for f in fams if f["algorithmic_bytes"] > 0), key=lambda f: f["share_of_frame"], default=None)
     if dom is None:
         return None
-    tj, tname = traffic_table()
-    key = dom["kernel"].split(" ")[0]
-    traffic = (tj.get(workload) or {}).get(key) if isinstance(tj.get(workload), dict) else (tj.get(key) if workload == "C2" else None)
     return {"bound": "hbm", "kernel": dom["kernel"], "achieved": dom["achieved_gbs"], "peak": hbm, "unit": "GB/s",
-            "frac": dom["achieved_gbs"] / hbm, "traffic": traffic,
-            "traffic_source": f"ncu --set full capture of this code, profiles/{tname}" if traffic else None,
-            "peak_source": peak_src, "avg_launch_us": dom["avg_us"], "algorithmic_bytes_per_launch": dom["algorithmic_bytes"],
-            "note": note}
+            "frac": dom["achieved_gbs"] / hbm, "peak_source": peak_src, "avg_launch_us": dom["avg_us"],
+            "algorithmic_bytes_per_launch": dom["algorithmic_bytes"], "note": note}
 
 
 def measure_other_workload(flb, torch, name, local, dev, stream, flush, hbm, peak_src, po, steps=10):
@@ -664,14 +662,18 @@ def main():
     ap.add_argument("--quick", action="store_true", help="profiling aid: skip the e2e / profile / cpu_baseline legs")
     ap.add_argument("--no-others", action="store_true", help="skip the other_workloads (C3, C4) and batched legs")
     ap.add_argument("--cell-size", type=float, default=0.0, help="experiment: kNN grid cell size (default 2 x the map pitch)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the timed path returned in its last step (state, covariance, reports) as DIR/<name>.npy")
     ap.add_argument("--cpu-one-frame", default=None, help=argparse.SUPPRESS)      # child process of measure_other_workload
     ap.add_argument("--cpu-baseline-child", default=None, help=argparse.SUPPRESS)  # child process of the cpu_baseline leg
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.warmup < 3:
         args.warmup = 3
     if args.impl == "reference":
-        if args.steps > 30:
-            args.steps = 30           # bounded sample: the CPU arm needs ~0.1-1 s per frame
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes what the GPU path computed; it does not apply to --impl reference")
         return run_reference(args)
 
     if args.cpu_one_frame:
@@ -730,6 +732,8 @@ def main():
     total_ms, launches, t_wall = rig.time_resident(args.steps)
     clocks = sampler.stop() if sampler else None
     fps = args.steps / (total_ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *h.state_download(), has_vio)
 
     trace = rig.pass_trace() if world == 1 else None
     if args.quick:

@@ -1,6 +1,6 @@
-"""fastlivo_b200 -- B200-native FAST-LIVO measurement / iterated-ESKF hot path.
+"""fastlivo_b200 -- H100-native FAST-LIVO measurement / iterated-ESKF hot path.
 
-The product is ``libfastlivo_b200.so`` (hand-written sm_100a CUDA behind the C ABI of
+The product is ``libfastlivo_b200.so`` (hand-written sm_90a CUDA behind the C ABI of
 ``include/fastlivo_b200.h``).  This Python package is only the thin ctypes binding the
 tests and ``bench.py`` drive it through, plus the synthetic-frame generator.  The
 directory name contains a hyphen, so import it through ``fastlivo_loader.load()`` at

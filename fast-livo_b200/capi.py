@@ -182,7 +182,7 @@ def lib_path() -> str:
 
 
 def build(force: bool = False) -> str:
-    """Compile libfastlivo_b200.so for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile libfastlivo_b200.so for sm_90a (nvcc cross-compiles without a GPU)."""
     srcs = [os.path.join(_HERE, "csrc", f) for f in os.listdir(os.path.join(_HERE, "csrc"))]
     srcs.append(os.path.join(_HERE, "..", "include", "fastlivo_b200.h"))
     stale = (not os.path.exists(_SO)) or os.path.getmtime(_SO) < max(os.path.getmtime(s) for s in srcs)

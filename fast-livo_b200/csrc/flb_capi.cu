@@ -1,4 +1,4 @@
-// flb_capi.cu -- the C ABI of include/fastlivo_b200.h over the sm_100a kernels.
+// flb_capi.cu -- the C ABI of include/fastlivo_b200.h over the sm_90a kernels.
 // Host side is plain C++ (no Eigen / PCL / torch); the handle owns device memory, three streams (updates; image + patch
 // copies; scan copy + ordering -- every input has two device sets, so an upload never waits for the update that is
 // running: DESIGN.md section 4.8), CUDA events and an optional NCCL communicator (dlopen'ed lazily).
@@ -614,8 +614,8 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
             }
         }
         {
-            // L2 prefetch of the map (points + cell table) at kernel start: on by default (C2, 5.3 MB: first pass 36.1 -> 34.0 us,
-            // +1.2 % frames/s; C3, 27 MB: 250 -> 239 us); FLB_PREFETCH=0/1 overrides
+            // L2 prefetch of the map (points + cell table) at kernel start: on by default above 1 MB (H100, FLB_PREFETCH=0 vs 1,
+            // device-resident frames/s: C2 (5.3 MB) 5505 -> 5557, C3 (27 MB) 1502 -> 1515, C4 2557 -> 2568); FLB_PREFETCH=0/1 overrides
             const size_t bytes = (size_t)h->M * 16 + ((size_t)h->ncell + 1) * 4;
             static const int env = [] { const char* e = getenv("FLB_PREFETCH"); return e ? atoi(e) : -1; }();
             a.prefetch = env >= 0 ? env : (bytes > (1u << 20) ? 1 : 0);
@@ -1612,8 +1612,8 @@ int flb_scan_upload(flb_handle* h, const float* body_xyz, int N, int stride) {
         if (!direct) FLB_CUDA(h, h->st_scan.mark(ss));
         // Morton order in the body frame (cell = twice the map grid's cell): spatially coherent warps at any pose
         const float inv_cell = 0.5f / (float)h->cfg.cell_size;
-        // One-block ordering vs keys + device-wide radix sort + gather (identical order).  Measured on an idle GPU
-        // (profiles/scan_upload_probe.py, copy included): 8 k points 45 vs 76 us, 16 k 78 vs 82, 24 k 116 vs 89 -- but the
+        // One-block ordering vs keys + device-wide radix sort + gather (identical order).  Measured on an idle H100
+        // (profiles/scan_upload_probe.py, copy included): 8 k points 42 vs 77 us, 16 k 100 vs 89, 24 k 129 vs 99 -- but the
         // one-block kernel runs on the SM the persistent kernels leave free, so when an update is still running on
         // `stream` (a pipelined caller) it costs nothing, while the device-wide kernels would queue behind the update.
         // So: one block up to 16 896 points always, up to 25 600 when `stream` is busy; FLB_BLOCK_SORT=0 / 2 or

@@ -1,4 +1,4 @@
-// flb_device.cuh -- per-thread device math of the FAST-LIVO hot path (sm_100a).
+// flb_device.cuh -- per-thread device math of the FAST-LIVO hot path (sm_90a).
 //
 // Everything here is a pure function of its arguments, compiled with
 // -fmad=false so that every float/double expression rounds exactly as written

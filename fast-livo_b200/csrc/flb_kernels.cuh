@@ -1,4 +1,4 @@
-// flb_kernels.cuh -- __global__ kernels of the FAST-LIVO hot path for sm_100a.
+// flb_kernels.cuh -- __global__ kernels of the FAST-LIVO hot path for sm_90a.
 //
 // Kernel families (SURVEY.md §8):
 //   * LIO pass  : per-point world transform + exact 5-NN over the device map grid + float32 QR
@@ -573,7 +573,8 @@ __global__ void k_scan_gather(const float* __restrict__ xyz, int N, const int* _
 
 // State in / result out as ONE launch each, reading / writing the page-locked host buffer directly (mapped memory):
 // k_state_install replaces a host-to-device copy + a device-to-device copy (state pair + its saved copy),
-// k_pack_result four small device-to-host copies -- on a 200 us frame every queued operation is 2-3 us of stream time.
+// k_pack_result four small device-to-host copies -- on a frame of a few hundred us every queued operation is a visible
+// share of stream time.
 __global__ void __launch_bounds__(256) k_state_install(const double* __restrict__ host_pair, State18* __restrict__ states) {
     constexpr int n = (int)(2 * sizeof(State18) / sizeof(double));
     double* d0 = reinterpret_cast<double*>(&states[0]);
@@ -597,7 +598,7 @@ __global__ void __launch_bounds__(256) k_pack_result(const State18* __restrict__
 
 // The whole upload ordering (keys, stable sort, gather, flag reset) in ONE block, for scans of up to BLOCK * ITEMS
 // points: the per-frame persistent kernels leave one SM free (flb_capi.cu, `pers_cap`), and this kernel -- launched on
-// the handle's scan stream -- orders frame k+1's scan on that SM while frame k's VIO update still runs on the other 147.
+// the handle's scan stream -- orders frame k+1's scan on that SM while frame k's VIO update still runs on the others.
 // Same keys and same tie order (stable, by input index) as k_scan_keys + the device-wide radix sort + k_scan_gather.
 // Layout: item j of thread t is input index t * ITEMS + j ("blocked"; ITEMS odd so that the shared-memory transpose
 // below is conflict-free); the sort's last pass leaves the output "striped" (position j * BLOCK + t), so the 16-byte
@@ -1036,7 +1037,7 @@ __device__ __forceinline__ void vio_patch_error(const VioArgs& a, int i, const d
 
 // `defer` (persistent kernel, last patch of this warp in the pass): the per-patch error chain is NOT run here; the caller
 // runs vio_patch_error after its block has arrived at the pass barrier -- the chain (64 dependent steps by one lane,
-// ~1.3 us) feeds only the leader's error sum, which is off the critical path, while the barrier is on it.  Returns true
+// about a microsecond) feeds only the leader's error sum, which is off the critical path, while the barrier is on it.  Returns true
 // when a chain is pending (`tiny_out` is its argument; s_res must stay untouched until then).
 __device__ __forceinline__ bool vio_patch(const VioArgs& a, const VioPose& pose, int level, int i, const PatchIn& in,
                                           float* s_lat, double* s_res, double& accv, double& n_meas, double& skipped,
@@ -1703,7 +1704,7 @@ struct VioSolveArgs {
 
 constexpr int kErrChunk = 2048;          // staging capacity of the kernel-per-pass finalize kernel (static shared memory)
 // threads of the leader block that gather + sum the per-patch errors: 160 of the persistent kernel's 512 (the other 352 reduce
-// the 146 block partials in ten slices of 15: one round trip), 128 of the finalize kernel's 256
+// the worker blocks' partials in one round trip), 128 of the finalize kernel's 256
 constexpr int kVioDbg = 8 + 4 * 16;   // debug stamps per block (tracing only)
 
 // One VIO leader step (whole block, NT threads), in two halves like the LIO one.  Requires the 24
@@ -1774,7 +1775,7 @@ __device__ __forceinline__ void vio_leader_solve(const VioSolveArgs& s, LeaderSm
         // of kErrSlice (each thread 16 independent loads / unit polls per slice: one L2 round trip per attempt) and hand
         // each slice over through a named barrier (arrive / sync pairs, two ids alternating); lane 0 of the last warp runs
         // the exact sequential float sum (:852) behind them, one FADD latency per patch, 16 addends per step with the next
-        // 16 already fetched from shared memory.  The chain is the longer of the two (2 k patches: 4 us, 10 k: 20 us), so
+        // 16 already fetched from shared memory.  The chain is the longer of the two (one FADD latency per patch), so
         // the gather costs one round trip, not one per slice.  Both are hidden behind the other threads' reduce + solve
         // and -- in the persistent kernel -- behind the next pass, which has already been started on the accept branch.
         constexpr int kStagers = kErrTeam - 32, kPer = 16, kErrSlice = kStagers * kPer;

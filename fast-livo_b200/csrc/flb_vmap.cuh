@@ -1,4 +1,4 @@
-// flb_vmap.cuh -- device-resident visual map (SURVEY.md section 8 rows f2 and f4) for sm_100a.
+// flb_vmap.cuh -- device-resident visual map (SURVEY.md section 8 rows f2 and f4) for sm_90a.
 //
 //   select   LidarSelector::addFromSparseMap (src/lidar_selection.cpp:346-587): scan-voxel set + sparse depth image,
 //            per-grid-cell closest visible map point, depth-continuity test, closest-view observation

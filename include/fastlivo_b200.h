@@ -1,4 +1,4 @@
-/* fastlivo_b200 -- C ABI of the B200-native FAST-LIVO measurement/ESKF hot path.
+/* fastlivo_b200 -- C ABI of the H100-native FAST-LIVO measurement/ESKF hot path.
  *
  * Plain C, plain pointers and sizes, no torch / Eigen / PCL types.  Every entry
  * point cites the reference code it replaces (paths relative to the reference
@@ -443,7 +443,7 @@ int flb_comm_unique_id(void* unique_id_128b);
 int flb_comm_init(flb_handle* h, const void* unique_id_128b, int rank, int world_size);
 int flb_comm_destroy(flb_handle* h);
 
-/* Fused NVLink exchange: the B200-idiomatic alternative to the NCCL path.  Inside the persistent update
+/* Fused NVLink exchange: the NVLink-native alternative to the NCCL path.  Inside the persistent update
  * kernel every rank writes its packed sums (leader block) and its VIO per-patch errors (the worker warp that
  * computed each one) straight into every rank's mailbox over NVLink peer memory as self-validating units
  * {payload, exchange tag} -- one store instruction per unit, no separate flag, no system fence, one NVLink

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE -- NOT PRODUCT CODE.  See flo_oracle.h for the rules on who
 // may load this library.  "parity unpinned": the reference has no tests and its
 // node cannot be built in this image; every function below follows the cited
-// reference lines (paths relative to /root/reference) op for op.
+// reference lines (paths relative to the reference tree, hku-mars/FAST-LIVO @ dcebf84) op for op.
 //
 // Build: oracle/Makefile (g++ -std=c++17 -O3 -fopenmp -ffp-contract=off, no
 // -march=native: mirrors reference CMakeLists.txt:8,39-41; x86-64 baseline has

@@ -16,7 +16,7 @@
  * inverse() and vikit's pinhole model restated from their published algorithms
  * (SURVEY.md Appendix C).
  *
- * All citations are relative to /root/reference.
+ * All citations are relative to the reference tree (hku-mars/FAST-LIVO @ dcebf84).
  */
 #ifndef FLO_ORACLE_H
 #define FLO_ORACLE_H

@@ -4,7 +4,7 @@
  * (reference src/lidar_selection.cpp:150-168; SURVEY.md section 8 row f4): every scan point is projected into the
  * new frame, scored with vikit's Shi-Tomasi corner score and competes for its image-grid cell.
  * vikit (uzh-rpg/rpg_vikit, vikit_common/src/vision.cpp: shiTomasiScore; abstract_camera.h: isInFrame;
- * pinhole_camera.cpp: world2cam) is a third-party dependency absent from /root/reference; its published
+ * pinhole_camera.cpp: world2cam) is a third-party dependency absent from the reference tree; its published
  * algorithm is restated here (SURVEY.md Appendix C).  PARITY STATUS: "parity unpinned".
  */
 #include <cmath>
@@ -73,7 +73,7 @@ extern "C" void flo_visual_candidates(const flo_cam* cam, const double* Rcw, con
  * getpatch (:121-141), addSparseMap's second loop (:171-195), AddPoint (:204-230), addObservation (:913-965)
  * and Point::getCloseViewObs / getFurthestViewObs / addFrameRef / deleteFeatureRef (src/point.cpp).
  *
- * Third-party pieces absent from /root/reference, restated from their published sources (PARITY UNPINNED):
+ * Third-party pieces absent from the reference tree, restated from their published sources (PARITY UNPINNED):
  *   vikit  PinholeCamera::cam2world (pinhole_camera.cpp), AbstractCamera::isInFrame, vk::interpolateMat_8u
  *          (vikit_common/include/vikit/vision.h)
  *   Sophus SE3 (the SVO-era, non-templated version): T * p, inverse(), composition.  Sophus keeps the rotation
@@ -587,7 +587,7 @@ void flo_colorize(const flo_cam* cam, const double* Rcw, const double* Pcw, cons
 }
 
 /* pcl::VoxelGrid<PointT>::applyFilter on x, y, z (PCL 1.8+, filters/include/pcl/filters/impl/voxel_grid.hpp; third-party,
- * absent from /root/reference, restated): leaf index from the cloud minimum, points of a leaf summed in float and divided by
+ * absent from the reference tree, restated): leaf index from the cloud minimum, points of a leaf summed in float and divided by
  * the count, output in ascending leaf index.  PCL orders (leaf idx, point) pairs with std::sort on the leaf idx alone, so
  * the order INSIDE a leaf -- and with it the last bits of the float sum -- is unspecified; this restatement uses the input
  * order (a stable sort), which is one of the orders PCL can produce.  Returns the number of leaves. */

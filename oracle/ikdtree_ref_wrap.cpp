@@ -3,7 +3,7 @@
 // file builds (oracle/_ref/libikdtree_ref.so).
 //
 // Thin C-ABI wrapper around the reference's OWN k-d tree
-// (/root/reference/include/ikd-Tree/ikd_Tree.{h,cpp}, compiled unmodified from
+// (the reference's include/ikd-Tree/ikd_Tree.{h,cpp}, compiled unmodified from
 // where it lies through oracle/shim/, see oracle/Makefile).  It exposes exactly
 // the two calls the hot path makes:
 //   KD_TREE::Build          (reference src/laserMapping.cpp:1411-1419)

@@ -205,13 +205,24 @@ KNN_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void
 
 
 def build(force: bool = False) -> None:
-    """Compile the checker (and, when /root/reference is present, the reference ikd-Tree)."""
+    """Compile the checker and, whenever the reference tree is available, the reference ikd-Tree (see reference_dir)."""
     need = force or not os.path.exists(_LIB) or \
         os.path.getmtime(_LIB) < max(os.path.getmtime(os.path.join(_HERE, f)) for f in ("flo_oracle.cpp", "flo_ikfom.cpp", "flo_imu.cpp", "flo_vmap.cpp", "flo_oracle.h"))
     if need:
         subprocess.check_call(["make", "-s", "-C", _HERE, "liboracle.so"])
-    if os.path.isdir("/root/reference/include/ikd-Tree") and (force or not os.path.exists(_REF)):
-        subprocess.check_call(["make", "-s", "-C", _HERE, "ref"])
+    ref = reference_dir()
+    if ref and (force or not os.path.exists(_REF)):
+        subprocess.check_call(["make", "-s", "-C", _HERE, "ref", f"REF={ref}"])
+
+
+def reference_dir():
+    """The FAST-LIVO checkout the reference ikd-Tree is compiled from: $FASTLIVO_REFERENCE, else a checkout named
+    `reference` next to this repository; None when neither holds include/ikd-Tree (or it cannot be read)."""
+    for d in (os.environ.get("FASTLIVO_REFERENCE", ""), os.path.join(os.path.dirname(_HERE), "..", "reference")):
+        if d and os.path.isfile(os.path.join(d, "include", "ikd-Tree", "ikd_Tree.cpp")) \
+                and os.access(os.path.join(d, "include", "ikd-Tree", "ikd_Tree.cpp"), os.R_OK):
+            return os.path.abspath(d)
+    return None
 
 
 _lib = None
@@ -331,7 +342,7 @@ class IkdTreeRef:
     def __init__(self, map_xyz):
         R = ref_lib()
         if R is None:
-            raise RuntimeError("oracle/_ref/libikdtree_ref.so missing (built only where /root/reference exists)")
+            raise RuntimeError("oracle/_ref/libikdtree_ref.so missing (built only where the reference tree is available, see reference_dir)")
         self._R = R
         m = f32(map_xyz)
         # the reference's KD_TREE constructor printf()s "Multi thread started" (ikd_Tree.cpp:170); keep

@@ -1,8 +1,8 @@
-// Microbenchmark: the floor of an exact sequential float sum on sm_100a.
+// Microbenchmark: the floor of an exact sequential float sum on sm_90a.
 //   (a) a pure register chain of dependent FADDs (issue-to-use latency),
 //   (b) the leader's loop: 16 addends per step from shared memory, the next 16 prefetched (flb_kernels.cuh, error team),
 //   (c) the same with 32 addends per step.
-// One thread; cycles from clock64().  Build on the box:  nvcc -O3 -arch=sm_100a -fmad=false -o fadd_chain fadd_chain.cu
+// One thread; cycles from clock64().  Build:  nvcc -O3 -arch=sm_90a -fmad=false -o fadd_chain fadd_chain.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

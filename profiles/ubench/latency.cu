@@ -1,5 +1,5 @@
 // Dependent-issue latency of a few SASS instructions on the device this runs on (profiling aid).
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -fmad=false -o latency latency.cu
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -fmad=false -o latency latency.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

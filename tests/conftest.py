@@ -12,7 +12,7 @@ import fastlivo_loader  # noqa: E402
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 @pytest.fixture(scope="session")

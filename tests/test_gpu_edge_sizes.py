@@ -16,7 +16,7 @@ def handle(flb, request):
     h.close()
 
 
-@pytest.mark.parametrize("n", [1, 2, 5, 31, 32, 33, 64, 147, 148, 149, 1175, 1176, 1177, 1185])
+@pytest.mark.parametrize("n", [1, 2, 5, 31, 32, 33, 64, 131, 132, 133, 147, 148, 149, 1047, 1048, 1049, 1175, 1176, 1177, 1185])
 def test_lio_update_small_scans(flb, po, frames, handle, n):
     f = dict(frames("T1"))
     rng = np.random.default_rng(n)

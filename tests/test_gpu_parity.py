@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 from conftest import bits
+from golden_util import assert_digest, lattice_fixture, load_ref_golden
 
 pytestmark = pytest.mark.gpu
 
@@ -49,19 +50,16 @@ def test_knn_bit_exact(flb, po, frames, handle, name):
 
 
 def test_knn_vs_reference_ikdtree(flb, po, frames, handle):
-    """Same neighbours as the reference's own KD_TREE::Nearest_Search (oracle/_ref)."""
-    if po.ref_lib() is None:
-        pytest.skip("oracle/_ref/libikdtree_ref.so not built")
+    """Same neighbours as the reference's own KD_TREE::Nearest_Search (stored by tests/golden/make_golden_ref.py)."""
     f = frames("T1")
     handle.map_upload(f["map_xyz"])
-    tree = po.IkdTreeRef(f["map_xyz"])
+    g = load_ref_golden()
     rng = np.random.default_rng(17)
     q = (f["map_xyz"][rng.integers(0, len(f["map_xyz"]), 5000)] + rng.normal(0, 0.3, (5000, 3))).astype(np.float32)
-    ri, rd = tree.knn(q)
     gi, gd = handle.knn(q)
-    ok = rd[:, 4] <= 5.0
+    ok = np.unpackbits(g["knn_T1_ok"], count=len(q)).astype(bool)
     assert ok.sum() > 4000
-    assert (gi[ok] == ri[ok]).all() and (bits(gd[ok]) == bits(rd[ok])).all()
+    assert_digest(g, "knn_T1_digest", gi[ok], gd[ok], expected=lambda: po.knn_brute(f["map_xyz"], q[ok]))
 
 
 def test_knn_exact_ties_vs_reference_ikdtree(flb, po, handle):
@@ -71,16 +69,10 @@ def test_knn_exact_ties_vs_reference_ikdtree(flb, po, handle):
     the data (ikd_Tree.h:57-60 only orders the heap).  What IS defined, and asserted: the five distances agree bit
     for bit at every rank, every returned index is a true neighbour at exactly that distance, and the two index
     lists differ only inside groups of exactly tied distances."""
-    if po.ref_lib() is None:
-        pytest.skip("oracle/_ref/libikdtree_ref.so not built")
-    g = np.arange(-8, 9, dtype=np.float32) * 0.25
-    lat = np.stack(np.meshgrid(g, g, g[:5], indexing="ij"), -1).reshape(-1, 3).astype(np.float32)
-    rng = np.random.default_rng(3)
-    lat = lat[rng.permutation(len(lat))]
+    lat, q = lattice_fixture()
     handle.map_upload(lat)
-    tree = po.IkdTreeRef(lat)
-    q = np.concatenate([lat[:400], lat[400:800] + np.float32(0.125), lat[800:1000] + np.array([0.125, 0, 0], np.float32)]).astype(np.float32)
-    ri, rd = tree.knn(q)
+    g = load_ref_golden()
+    ri, rd = g["ties_idx"], g["ties_d2"]
     gi, gd = handle.knn(q)
     assert (bits(gd) == bits(rd)).all()                        # distances: bit-exact at every rank
     tied_queries = 0

@@ -5,6 +5,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from golden_util import assert_digest, load_ref_golden
+
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
@@ -12,18 +14,14 @@ def _p(a):
 
 @pytest.mark.parametrize("name", ["T0", "T1"])
 def test_brute_knn_equals_reference_ikdtree(po, frames, name):
-    """(i) our brute-force float32 kNN == the reference's own KD_TREE::Nearest_Search."""
-    if po.ref_lib() is None:
-        pytest.skip("oracle/_ref not built (no /root/reference on this box and no prebuilt .so)")
+    """(i) our brute-force float32 kNN == the reference's own KD_TREE::Nearest_Search (indices and distance bits,
+    stored by tests/golden/make_golden_ref.py)."""
     f = frames(name)
-    tree = po.IkdTreeRef(f["map_xyz"])
     rng = np.random.default_rng(1)
     q = (f["map_xyz"][rng.integers(0, len(f["map_xyz"]), 3000)] + rng.normal(0, 0.25, (3000, 3))).astype(np.float32)
     bi, bd = po.knn_brute(f["map_xyz"], q)
-    ri, rd = tree.knn(q, nthreads=4)
     assert (np.diff(bd, axis=1) > 0).all(), "fixture has distance ties"
-    assert (bi == ri).all()
-    assert (bd.view(np.uint32) == rd.view(np.uint32)).all()
+    assert_digest(load_ref_golden(), f"brute_{name}_digest", bi, bd)
 
 
 def test_plane_fit_vs_float64_least_squares(po, frames):
