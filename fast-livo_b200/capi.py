@@ -174,7 +174,8 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_vmap_reset", "flb_vmap_select", "flb_vmap_selected", "flb_vmap_grow", "flb_vmap_add_observations", "flb_vmap_counts",
            "flb_vmap_map_value", "flb_vmap_dump", "flb_colorize", "flb_voxel_grid",
            "flb_batch_begin", "flb_batch_set_frame", "flb_batch_state_reset_enqueue", "flb_batch_update_enqueue", "flb_batch_state_download",
-           "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort"]
+           "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
+           "flb_map_grid_info", "flb_debug_set_map_index"]
 
 
 def lib_path() -> str:
@@ -233,6 +234,8 @@ def lib():
         L.flb_vio_errors.argtypes = [vp, vp, C.c_int]
         L.flb_debug_scan_order.argtypes = [vp, vp, C.c_int]
         L.flb_debug_set_scan_sort.argtypes = [vp, C.c_int]
+        L.flb_map_grid_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_int), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.flb_debug_set_map_index.argtypes = [vp, C.c_int]
         L.flb_vio_update_level.argtypes = [vp, C.POINTER(VioParams), C.c_int, C.c_float, C.POINTER(State18), C.POINTER(State18),
                                            C.POINTER(C.c_float), vp, C.POINTER(VioReport)]
         L.flb_batch_begin.argtypes = [vp, C.c_int, C.c_int]
@@ -361,6 +364,12 @@ class Handle:
         self._ck(self.L.flb_map_download(self.h, _p(out), n, C.byref(m)))
         return out
 
+    def map_grid_info(self):
+        """flb_map_grid_info: dict(cell_size, sparse, cells, index_bytes) of the map's kNN cell index."""
+        cs, sp, nc, nb = C.c_double(), C.c_int(), C.c_int64(), C.c_int64()
+        self._ck(self.L.flb_map_grid_info(self.h, C.byref(cs), C.byref(sp), C.byref(nc), C.byref(nb)))
+        return dict(cell_size=cs.value, sparse=sp.value, cells=nc.value, index_bytes=nb.value)
+
     def voxel_grid(self, xyz, leaf):
         """flb_voxel_grid: pcl::VoxelGrid centroids (m, 3) float32."""
         a = np.ascontiguousarray(xyz, np.float32)
@@ -377,6 +386,10 @@ class Handle:
     def debug_set_scan_sort(self, mode):
         """0 automatic, 1 one-block ordering kernel, 2 device-wide sort (test aid)."""
         self._ck(self.L.flb_debug_set_scan_sort(self.h, int(mode)))
+
+    def debug_set_map_index(self, mode):
+        """Cell index of the following map rebuilds: 0 automatic, 1 dense always, 2 sparse always (test aid)."""
+        self._ck(self.L.flb_debug_set_map_index(self.h, int(mode)))
 
     def debug_scan_order(self):
         """Index in the caller's array of the point at each position of the uploaded (ordered) scan (test aid)."""

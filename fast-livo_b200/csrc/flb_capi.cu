@@ -168,6 +168,11 @@ struct flb_handle {
     DevBuf<unsigned char> cub_tmp;
     DevBuf<float4> map_pts, map_pts_alt;       // sorted grid points (double-buffered for the incremental merge)
     DevBuf<int> cell_start, cell_start_alt;
+    // sparse cell index (GridDesc), built by rebuild_grid when flb_debug_set_map_index asks for it
+    bool sparse = false;
+    int map_index_mode = 0;                    // 0 auto, 1 dense always, 2 sparse always (flb_debug_set_map_index)
+    DevBuf<SparseCell> cell_table;             // ncell = occupied cells, grid.nx = slot mask
+    DevBuf<unsigned long long> cell_keys, cell_keys_alt;   // cell key of every sorted point
     DevBuf<float> map_raw_alt;
     DevBuf<unsigned char> dead, ins;
     DevBuf<int> dead_before, merge_counts, bbox_dev;
@@ -218,7 +223,7 @@ struct flb_handle {
     DevBuf<State18> states;      // [0]=x [1]=x_prop [2]=old_state(VIO) [3]=saved x [4]=saved x_prop
     DevBuf<StateIkfom> ik_states;   // [0] = x_/P_, [1] = x_propagated/P_propagated
     DevBuf<IkfomCtrl> ik_ctrl;
-    int occ_ik = 0;
+    int occ_ik = 0, occ_ik_sparse = 0;
     DevBuf<LioCtrl> lio_ctrl;
     DevBuf<VioCtrl> vio_ctrl;
     DevBuf<GridBarrier> barrier; // grid barrier of the persistent kernels
@@ -238,7 +243,7 @@ struct flb_handle {
     int dbg_blocks = 0;
     bool tracing = false;
     int num_sms = 0;
-    int occ_lio = 0, occ_vio = 0;
+    int occ_lio = 0, occ_lio_sparse = 0, occ_vio = 0;
     Staging st_map, st_scan, st_img, st_patch, st_state, st_misc;   // per-kind upload staging
     PinBuf pin_out;              // staging for downloads
     PinBuf pin_res[2];           // flb_state_download_enqueue / _wait: two result slots in flight
@@ -429,10 +434,12 @@ int ensure_common(flb_handle* h) {
         static const int env_reserve = [] { const char* e = getenv("FLB_RESERVE_SM"); return e ? atoi(e) : 1; }();
         h->pers_sms = (env_reserve && h->num_sms > 2) ? h->num_sms - 1 : h->num_sms;
     }
-    FLB_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->occ_lio, k_lio_update_persistent<kLioPersBlock>, kLioPersBlock, 0));
+    FLB_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->occ_lio, k_lio_update_persistent<kLioPersBlock, false>, kLioPersBlock, 0));
+    FLB_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->occ_lio_sparse, k_lio_update_persistent<kLioPersBlock, true>, kLioPersBlock, 0));
     FLB_CUDA(h, h->ik_states.reserve(2));
     FLB_CUDA(h, h->ik_ctrl.reserve(1));
-    FLB_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->occ_ik, k_lio_update_ikfom_persistent<kLioBlock>, kLioBlock, 0));
+    FLB_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->occ_ik, k_lio_update_ikfom_persistent<kLioBlock, false>, kLioBlock, 0));
+    FLB_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->occ_ik_sparse, k_lio_update_ikfom_persistent<kLioBlock, true>, kLioBlock, 0));
     // the VIO leader stages the per-patch errors of a pass in dynamic shared memory (up to kVioErrCapMax floats)
     FLB_CUDA(h, cudaFuncSetAttribute(k_vio_update_persistent<kVioPersBlock>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      kVioErrCapMax * (int)sizeof(float)));
@@ -442,12 +449,20 @@ int ensure_common(flb_handle* h) {
     return FLB_OK;
 }
 
+// the cell index the kNN reads: dense cell_start, or the sparse table (GridDesc)
+const int* cell_index(const flb_handle* h) {
+    return h->sparse ? reinterpret_cast<const int*>(h->cell_table.p) : h->cell_start.p;
+}
+size_t index_bytes(const flb_handle* h) {
+    return h->sparse ? ((size_t)(unsigned)h->grid.nx + 1) * sizeof(SparseCell) : ((size_t)h->ncell + 1) * sizeof(int);
+}
+
 LioArgs make_lio_args(flb_handle* h, const LioParamsDev& prm, bool exports, int width) {
     LioArgs a{};
     a.scan = h->scan.p;
     a.N = h->N;
     a.grid = h->grid;
-    a.cell_start = h->cell_start.p;
+    a.cell_start = cell_index(h);
     a.map_pts = h->map_pts.p;
     a.state = &h->states.p[0];
     a.prm = prm;
@@ -479,8 +494,13 @@ int launch_lio_pass(flb_handle* h, const LioArgs& a, int width, bool knn_family)
     const int nb = lio_nblocks(h);
     if (nb == 0) return FLB_OK;
     LaunchScope ls(h, knn_family ? FAM_LIO_KNN : FAM_LIO_PLAIN);
-    if (width == 6) k_lio_pass<6, kLioBlock><<<nb, kLioBlock, 0, h->stream>>>(a);
-    else k_lio_pass<12, kLioBlock><<<nb, kLioBlock, 0, h->stream>>>(a);
+    if (h->sparse) {
+        if (width == 6) k_lio_pass<6, kLioBlock, true><<<nb, kLioBlock, 0, h->stream>>>(a);
+        else k_lio_pass<12, kLioBlock, true><<<nb, kLioBlock, 0, h->stream>>>(a);
+    } else {
+        if (width == 6) k_lio_pass<6, kLioBlock, false><<<nb, kLioBlock, 0, h->stream>>>(a);
+        else k_lio_pass<12, kLioBlock, false><<<nb, kLioBlock, 0, h->stream>>>(a);
+    }
     FLB_CUDA(h, cudaGetLastError());
     return FLB_OK;
 }
@@ -589,7 +609,7 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
         // one cooperative launch for the whole iterated update; grid = min(needed, co-resident capacity)
         // whole multiples of the SM count (<= co-resident capacity): chunks are dealt round-robin to blocks
         // worker blocks (one per SM, chunks dealt round-robin) + one leader block
-        const int cap = std::min(h->occ_lio * h->num_sms, h->pers_sms);
+        const int cap = std::min((h->sparse ? h->occ_lio_sparse : h->occ_lio) * h->num_sms, h->pers_sms);
         if (cap < 2) return fail(h, FLB_ERR_STATE, "persistent mode needs two co-resident blocks");
         const int workers = std::max(1, std::min((h->N + 31) / 32, cap - 1));
         const int grid = workers + 1;
@@ -606,8 +626,8 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
             if (env_warm) {
                 WarmList& w = a.warm;
                 const size_t n1 = (size_t)std::max(h->N, 1);
-                const void* ptr[] = {h->scan.p, h->map_pts.p, h->cell_start.p, h->plane.p, h->sel.p, h->plane_ok.p, h->partials.p, h->states.p};
-                const size_t len[] = {n1 * 16, (size_t)h->M * 16, ((size_t)h->ncell + 1) * 4, n1 * 16, n1, n1, (size_t)grid * lio_packed(6) * 8,
+                const void* ptr[] = {h->scan.p, h->map_pts.p, cell_index(h), h->plane.p, h->sel.p, h->plane_ok.p, h->partials.p, h->states.p};
+                const size_t len[] = {n1 * 16, (size_t)h->M * 16, index_bytes(h), n1 * 16, n1, n1, (size_t)grid * lio_packed(6) * 8,
                                       5 * sizeof(State18)};
                 w.n = 8;
                 for (int k = 0; k < 8; ++k) { w.p[k] = ptr[k]; w.bytes[k] = len[k]; }
@@ -616,7 +636,7 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
         {
             // L2 prefetch of the map (points + cell table) at kernel start: on by default above 1 MB (H100, FLB_PREFETCH=0 vs 1,
             // device-resident frames/s: C2 (5.3 MB) 5505 -> 5557, C3 (27 MB) 1502 -> 1515, C4 2557 -> 2568); FLB_PREFETCH=0/1 overrides
-            const size_t bytes = (size_t)h->M * 16 + ((size_t)h->ncell + 1) * 4;
+            const size_t bytes = (size_t)h->M * 16 + index_bytes(h);
             static const int env = [] { const char* e = getenv("FLB_PREFETCH"); return e ? atoi(e) : -1; }();
             a.prefetch = env >= 0 ? env : (bytes > (1u << 20) ? 1 : 0);
         }
@@ -632,7 +652,8 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
         { int rce = next_epoch(h, &epoch); if (rce) return rce; }
         void* args[] = {&a, &s, &bar, &pkt, &epoch, &trace, &dbg};
         LaunchScope ls(h, FAM_LIO_KNN);
-        FLB_CUDA(h, cudaLaunchCooperativeKernel((void*)k_lio_update_persistent<kLioPersBlock>, dim3(grid), dim3(kLioPersBlock), args, 0,
+        void* kern = h->sparse ? (void*)k_lio_update_persistent<kLioPersBlock, true> : (void*)k_lio_update_persistent<kLioPersBlock, false>;
+        FLB_CUDA(h, cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(kLioPersBlock), args, 0,
                                                 h->stream));
         h->last_pass_valid = false;
         return FLB_OK;
@@ -934,6 +955,7 @@ int flb_destroy(flb_handle* h) {
     for (auto& ev : h->evs) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
     h->map_raw.release(); h->keys.release(); h->keys_sorted.release(); h->vals.release(); h->vals_sorted.release();
     h->map_comb.release(); h->boxes.release(); h->vkeys.release(); h->vkeys_sorted.release(); h->keep.release(); h->sel_idx.release();
+    h->cell_table.release(); h->cell_keys.release(); h->cell_keys_alt.release();
     h->map_pts_alt.release(); h->cell_start_alt.release(); h->map_raw_alt.release(); h->dead.release(); h->ins.release();
     h->dead_before.release(); h->merge_counts.release(); h->bbox_dev.release();
     h->cub_tmp.release(); h->map_pts.release(); h->cell_start.release(); h->scan.release(); h->sel.release();
@@ -997,6 +1019,73 @@ int flb_host_free(flb_handle* h, void* p) {
 int64_t flb_launch_count(const flb_handle* h) { return h ? h->launches : 0; }
 
 // ---------------------------------------------------------------------------------------
+constexpr int kDenseCellCap = 1 << 25;      // largest dense cell table (cells); beyond it the cell is enlarged
+
+// Hash table of the occupied cells of the sorted key array h->cell_keys[0..M): >= 2x as many slots as cells.
+static int build_sparse_table(flb_handle* h, int M) {
+    FLB_CUDA(h, h->merge_counts.reserve(2));
+    FLB_CUDA(h, cudaMemsetAsync(h->merge_counts.p, 0, sizeof(int), h->stream));
+    const int nb = (M + 255) / 256;
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_sparse_count_cells<<<nb, 256, 0, h->stream>>>(h->cell_keys.p, M, h->merge_counts.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    int occupied = 0;
+    FLB_CUDA(h, cudaMemcpyAsync(&occupied, h->merge_counts.p, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    size_t slots = 16;
+    while (slots < 2 * (size_t)occupied) slots <<= 1;
+    FLB_CUDA(h, h->cell_table.reserve(slots));
+    FLB_CUDA(h, cudaMemsetAsync(h->cell_table.p, 0xff, slots * sizeof(SparseCell), h->stream));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_sparse_insert<<<nb, 256, 0, h->stream>>>(h->cell_keys.p, M, h->cell_table.p, (unsigned)(slots - 1));
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches++;
+    }
+    h->grid.nx = (int)(slots - 1);
+    h->ncell = occupied;
+    return FLB_OK;
+}
+
+// Sparse cell index over h->map_raw[0..M): anchored where the dense grid would be (h->grid_lo), at the configured cell.
+static int rebuild_sparse(flb_handle* h, int M) {
+    GridDesc g{};
+    g.ox = h->grid_lo[0]; g.oy = h->grid_lo[1]; g.oz = h->grid_lo[2];
+    g.cell = (float)h->cfg.cell_size;
+    g.inv_cell = 1.0f / g.cell;
+    g.max_d2 = (float)h->cfg.knn_max_d2;
+    g.max_ring = (int)std::ceil(std::sqrt(h->cfg.knn_max_d2) / h->cfg.cell_size) + 1;
+    FLB_CUDA(h, h->vkeys.reserve(M));
+    FLB_CUDA(h, h->cell_keys.reserve(M));
+    FLB_CUDA(h, h->vals.reserve(M));
+    FLB_CUDA(h, h->vals_sorted.reserve(M));
+    FLB_CUDA(h, h->map_pts.reserve(M));
+    const int nb = (M + 255) / 256;
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_sparse_cell_keys<<<nb, 256, 0, h->stream>>>(h->map_raw.p, M, g, h->vkeys.p, h->vals.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    size_t tmp_bytes = 0;
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, h->vkeys.p, h->cell_keys.p, h->vals.p, h->vals_sorted.p, M, 0, 63,
+                                                h->stream));
+    FLB_CUDA(h, h->cub_tmp.reserve(tmp_bytes));
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, tmp_bytes, h->vkeys.p, h->cell_keys.p, h->vals.p, h->vals_sorted.p, M, 0,
+                                                63, h->stream));
+    h->launches += 4;
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_map_gather<<<nb, 256, 0, h->stream>>>(h->map_raw.p, M, 3, h->vals_sorted.p, h->map_pts.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    h->grid = g;
+    h->sparse = true;
+    h->M = M;
+    return build_sparse_table(h, M);
+}
+
 // Build the sorted uniform kNN grid over h->map_raw[0..M) with the bounding box h->map_lo/hi.
 static int rebuild_grid(flb_handle* h, int M) {
     // the grid covers the map box plus a margin, so that points added next to the map (a moving sensor) fall inside
@@ -1010,12 +1099,21 @@ static int rebuild_grid(flb_handle* h, int M) {
     }
     const float* lo = h->grid_lo;
     const float* hi = h->grid_hi;
-    // grid geometry; enlarge the cell if the dense grid would exceed 2^25 cells (still exact, just slower)
+    // dense table or sparse index.  The automatic choice is the dense table at every extent: measured on H100
+    // (DESIGN.md section 8) the sparse index beats the coarsened dense grid at a 3 km map but not at 1 km, so it is only
+    // taken when flb_debug_set_map_index asks for it (and the box fits the cell keys)
+    if (h->map_index_mode == 2) {
+        double span = 0.0;
+        for (int k = 0; k < 3; ++k) span = std::max(span, (double)(hi[k] - lo[k]) / h->cfg.cell_size);
+        if (span < (double)(kCellKeyBias - 1)) return rebuild_sparse(h, M);
+    }
+    h->sparse = false;
+    // grid geometry; enlarge the cell if the dense grid would exceed kDenseCellCap cells (still exact, just slower)
     double cell = h->cfg.cell_size;
     for (;;) {
         const double nx = std::floor((hi[0] - lo[0]) / cell) + 1, ny = std::floor((hi[1] - lo[1]) / cell) + 1,
                      nz = std::floor((hi[2] - lo[2]) / cell) + 1;
-        if (nx * ny * nz <= (double)(1 << 25)) break;
+        if (nx * ny * nz <= (double)kDenseCellCap) break;
         cell *= 1.26;
     }
     GridDesc g{};
@@ -1167,6 +1265,83 @@ static int bits_for(long long span) {
     return b;
 }
 
+// Incremental Add_Points on the sparse index (always: there is no box to leave).  The steps of the dense incremental path
+// below, on 64-bit cell keys; the hash table is then rebuilt from the merged key array.  Nothing scales with the extent.
+static int map_add_points_sparse(flb_handle* h, const float* st, int n, float ds, const float* lo, const float* hi) {
+    const int M = h->M;
+    const GridDesc g = h->grid;
+    // voxel keys relative to the new points' own box (absolute 21-bit keys if that box needs more than 62 bits)
+    const int bx = (int)std::floor(lo[0] / ds) - 1, by = (int)std::floor(lo[1] / ds) - 1, bz = (int)std::floor(lo[2] / ds) - 1;
+    const int wx = bits_for((long long)std::floor(hi[0] / ds) + 2 - bx), wy = bits_for((long long)std::floor(hi[1] / ds) + 2 - by),
+              wz = bits_for((long long)std::floor(hi[2] / ds) + 2 - bz);
+    const bool rel = wx + wy + wz <= 62;
+    const int vbits = rel ? wx + wy + wz : 63;
+    FLB_CUDA(h, h->map_comb.reserve((size_t)n * 3));
+    FLB_CUDA(h, h->vkeys.reserve(n));
+    FLB_CUDA(h, h->vkeys_sorted.reserve(n));
+    FLB_CUDA(h, h->vals.reserve(n));
+    FLB_CUDA(h, h->vals_sorted.reserve(n));
+    FLB_CUDA(h, h->dead.reserve(M));
+    FLB_CUDA(h, h->ins.reserve(n));
+    FLB_CUDA(h, h->dead_before.reserve((size_t)M + 1));
+    FLB_CUDA(h, h->merge_counts.reserve(2));
+    FLB_CUDA(h, h->map_pts_alt.reserve((size_t)M + n));
+    FLB_CUDA(h, h->map_raw_alt.reserve(((size_t)M + n) * 3));
+    FLB_CUDA(h, h->cell_keys_alt.reserve((size_t)M + n));
+    float* nxyz = h->map_comb.p;
+    FLB_CUDA(h, cudaMemcpyAsync(nxyz, st, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    FLB_CUDA(h, h->st_map.mark(h->stream));
+    FLB_CUDA(h, cudaMemsetAsync(h->dead.p, 0, M, h->stream));
+    FLB_CUDA(h, cudaMemsetAsync(h->ins.p, 0, n, h->stream));
+    const int gn = (n + 255) / 256, gm = (M + 255) / 256;
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        if (rel) k_vox_keys_rel<<<gn, 256, 0, h->stream>>>(nxyz, n, ds, bx, by, bz, wx, wx + wy, h->vkeys.p, h->vals.p);
+        else k_vox_keys<<<gn, 256, 0, h->stream>>>(nxyz, n, ds, h->vkeys.p, h->vals.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    size_t t1 = 0, t2 = 0, t3 = 0;
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t1, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, vbits, h->stream));
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t2, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, 64, h->stream));
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t3, h->dead_before.p, h->dead_before.p, M, h->stream));
+    FLB_CUDA(h, h->cub_tmp.reserve(std::max(t1, std::max(t2, t3))));
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, t1, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, vbits, h->stream));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_vox_resolve_incremental<true><<<gn, 256, 0, h->stream>>>(h->vkeys_sorted.p, h->vals_sorted.p, nxyz, n, ds, g, cell_index(h),
+                                                                   h->map_pts.p, h->dead.p, h->ins.p);
+        // inserted points sorted by cell key (not-inserted ones carry kNoCell: behind every cell); the voxel keys are spent
+        k_insert_keys_sparse<<<gn, 256, 0, h->stream>>>(nxyz, n, h->ins.p, g, h->vkeys.p, h->vals.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, t2, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, 64, h->stream));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_dead_to_int<<<gm, 256, 0, h->stream>>>(h->dead.p, M, h->dead_before.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, t3, h->dead_before.p, h->dead_before.p, M, h->stream));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_merge_counts_sparse<<<1, 32, 0, h->stream>>>(h->dead_before.p, h->dead.p, M, h->vkeys_sorted.p, n, h->merge_counts.p);
+        k_merge_existing_sparse<<<gm, 256, 0, h->stream>>>(h->map_pts.p, h->cell_keys.p, h->dead.p, h->dead_before.p, M, h->vkeys_sorted.p, n,
+                                                            h->map_pts_alt.p, h->map_raw_alt.p, h->cell_keys_alt.p);
+        k_merge_inserts_sparse<<<gn, 256, 0, h->stream>>>(nxyz, h->vkeys_sorted.p, h->vals_sorted.p, h->merge_counts.p, h->cell_keys.p,
+                                                           h->dead_before.p, M, h->map_pts_alt.p, h->map_raw_alt.p, h->cell_keys_alt.p);
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches += 9;
+    }
+    int counts[2] = {0, 0};
+    FLB_CUDA(h, cudaMemcpyAsync(counts, h->merge_counts.p, sizeof(counts), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    std::swap(h->map_pts, h->map_pts_alt);
+    std::swap(h->map_raw, h->map_raw_alt);
+    std::swap(h->cell_keys, h->cell_keys_alt);
+    h->M = M - counts[0] + counts[1];
+    h->last_pass_valid = false;
+    return build_sparse_table(h, h->M);
+}
+
 int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride, float downsample_size) {
     FLB_CHECK_H(h);
     if (h->M <= 0) return fail(h, FLB_ERR_STATE, "flb_map_add_points: no map uploaded");
@@ -1212,11 +1387,20 @@ int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride,
         const float lim = 1.0e6f * downsample_size;
         for (int k = 0; k < 3; ++k)
             if (lo[k] < -lim || hi[k] > lim) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: coordinate / downsample_size exceeds 2^20 voxels");
+        if (h->sparse) {
+            // the sparse index has no box to leave, but every cell needs a key: within 2^20 cells of the anchor
+            const float o[3] = {h->grid.ox, h->grid.oy, h->grid.oz}, lk = (float)kCellKeyBias;
+            for (int k = 0; k < 3; ++k) {
+                const float a = (lo[k] - o[k]) * h->grid.inv_cell, b = (hi[k] - o[k]) * h->grid.inv_cell;
+                if (!(a >= -lk && b < lk)) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: point more than 2^20 cells from the map's anchor");
+            }
+        }
     }
     // the input is valid from here on: only now does the map box take it in
     bool inside = true;
     for (int k = 0; k < 3; ++k) inside = inside && lo[k] >= h->grid_lo[k] && hi[k] <= h->grid_hi[k];
     for (int k = 0; k < 3; ++k) { h->map_lo[k] = std::min(h->map_lo[k], lo[k]); h->map_hi[k] = std::max(h->map_hi[k], hi[k]); }
+    if (h->sparse) return map_add_points_sparse(h, st, n, downsample_size, lo, hi);
     if (!inside) return map_add_points_full(h, st, n, downsample_size);
 
     // ---- incremental path: every new point lies inside the box the grid covers
@@ -1264,7 +1448,7 @@ int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride,
                                                 wx + wy + wz, h->stream));
     {
         LaunchScope ls(h, FAM_OTHER);
-        k_vox_resolve_incremental<<<gn, 256, 0, h->stream>>>(h->vkeys_sorted.p, h->vals_sorted.p, nxyz, n, ds, g, h->cell_start.p, h->map_pts.p,
+        k_vox_resolve_incremental<false><<<gn, 256, 0, h->stream>>>(h->vkeys_sorted.p, h->vals_sorted.p, nxyz, n, ds, g, h->cell_start.p, h->map_pts.p,
                                                               h->dead.p, h->ins.p);
         // inserted points sorted by grid cell (not-inserted ones sort behind every cell)
         k_insert_cells<<<gn, 256, 0, h->stream>>>(nxyz, n, h->ins.p, g, ncell, h->keys.p, h->vals.p);
@@ -1325,6 +1509,16 @@ int flb_map_delete_boxes(flb_handle* h, const float* boxes, int nb) {
 }
 
 int flb_map_size(const flb_handle* h) { return h ? h->M : 0; }
+
+int flb_map_grid_info(flb_handle* h, double* cell_size, int* sparse, int64_t* cells, int64_t* index_bytes_out) {
+    FLB_CHECK_H(h);
+    if (h->M <= 0) return fail(h, FLB_ERR_STATE, "flb_map_grid_info: no map uploaded");
+    if (cell_size) *cell_size = (double)h->grid.cell;
+    if (sparse) *sparse = h->sparse ? 1 : 0;
+    if (cells) *cells = (int64_t)h->ncell;
+    if (index_bytes_out) *index_bytes_out = (int64_t)index_bytes(h);
+    return FLB_OK;
+}
 
 int flb_map_download(flb_handle* h, float* xyz, int capacity, int* M_out) {
     FLB_CHECK_H(h);
@@ -1688,7 +1882,8 @@ int flb_knn(flb_handle* h, const float* q, int nq, int* idx, float* d2) {
     FLB_CUDA(h, cudaMemcpyAsync(dq.p, q, (size_t)nq * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     {
         LaunchScope ls(h, FAM_LIO_KNN);
-        k_knn<<<(nq + 127) / 128, 128, 0, h->stream>>>(h->grid, h->cell_start.p, h->map_pts.p, dq.p, nq, di.p, dd.p);
+        if (h->sparse) k_knn<true><<<(nq + 127) / 128, 128, 0, h->stream>>>(h->grid, cell_index(h), h->map_pts.p, dq.p, nq, di.p, dd.p);
+        else k_knn<false><<<(nq + 127) / 128, 128, 0, h->stream>>>(h->grid, h->cell_start.p, h->map_pts.p, dq.p, nq, di.p, dd.p);
     }
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaMemcpyAsync(idx, di.p, (size_t)nq * kMatch * sizeof(int), cudaMemcpyDeviceToHost, h->stream);
@@ -1980,8 +2175,9 @@ int flb_lio_update_ikfom(flb_handle* h, const flb_ikfom_params* prm, flb_state_i
     s.prm.R = prm->laser_point_cov;
     s.prm.max_iteration = prm->max_iteration;
     std::memcpy(s.prm.limit, prm->limit, sizeof(s.prm.limit));
-    const int cap = std::max(1, h->occ_ik * h->num_sms);
-    const int want = std::min(cap, std::max(h->num_sms, std::min(2, h->occ_ik) * h->num_sms));
+    const int occ_ik = h->sparse ? h->occ_ik_sparse : h->occ_ik;
+    const int cap = std::max(1, occ_ik * h->num_sms);
+    const int want = std::min(cap, std::max(h->num_sms, std::min(2, occ_ik) * h->num_sms));
     const int grid = std::max(1, std::min((h->N + 31) / 32, want));
     FLB_CUDA(h, h->partials.reserve(std::max<size_t>((size_t)grid * lio_packed(12), h->partials.cap)));
     a.partials = h->partials.p;
@@ -1991,7 +2187,8 @@ int flb_lio_update_ikfom(flb_handle* h, const flb_ikfom_params* prm, flb_state_i
     void* args[] = {&a, &s, &bar};
     {
         LaunchScope ls(h, FAM_LIO_KNN);
-        FLB_CUDA(h, cudaLaunchCooperativeKernel((void*)k_lio_update_ikfom_persistent<kLioBlock>, dim3(grid), dim3(kLioBlock), args, 0,
+        void* kern = h->sparse ? (void*)k_lio_update_ikfom_persistent<kLioBlock, true> : (void*)k_lio_update_ikfom_persistent<kLioBlock, false>;
+        FLB_CUDA(h, cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(kLioBlock), args, 0,
                                                 h->stream));
     }
     h->last_pass_valid = false;
@@ -2392,6 +2589,15 @@ int flb_debug_set_scan_sort(flb_handle* h, int mode) {
     return FLB_OK;
 }
 
+// Test aid: cell index of the following map rebuilds (flb_map_upload, flb_map_delete_boxes, an Add_Points that leaves the
+// dense grid's box) -- 0 automatic (the dense table, see rebuild_grid), 1 dense always, 2 sparse always.
+int flb_debug_set_map_index(flb_handle* h, int mode) {
+    FLB_CHECK_H(h);
+    if (mode < 0 || mode > 2) return fail(h, FLB_ERR_INVALID, "flb_debug_set_map_index: mode 0, 1 or 2");
+    h->map_index_mode = mode;
+    return FLB_OK;
+}
+
 // Test aid: the uploaded scan's order -- src_index[i] = index (in the caller's array) of the point at sorted position i.
 int flb_debug_scan_order(flb_handle* h, int* src_index, int capacity) {
     FLB_CHECK_H(h);
@@ -2613,7 +2819,7 @@ int flb_batch_update_enqueue(flb_handle* h, const flb_lio_params* lprm, const fl
         a.scan = b.scan.p + off;
         a.N = b.N[i];
         a.grid = h->grid;
-        a.cell_start = h->cell_start.p;
+        a.cell_start = cell_index(h);
         a.map_pts = h->map_pts.p;
         a.state = b.states.p + (size_t)i * 5;
         a.prm = ld;
@@ -2651,7 +2857,8 @@ int flb_batch_update_enqueue(flb_handle* h, const flb_lio_params* lprm, const fl
         {
             // family tag: with early stop disabled the rematch passes are the first and the last (Appendix A)
             LaunchScope lsx(h, (it == -1 || it == T - 1) ? FAM_LIO_KNN : FAM_LIO_PLAIN);
-            k_lio_pass_batched<6, kLioBlock><<<dim3(nb_lio, B), kLioBlock, 0, h->stream>>>(b.lio_args.p);
+            if (h->sparse) k_lio_pass_batched<6, kLioBlock, true><<<dim3(nb_lio, B), kLioBlock, 0, h->stream>>>(b.lio_args.p);
+            else k_lio_pass_batched<6, kLioBlock, false><<<dim3(nb_lio, B), kLioBlock, 0, h->stream>>>(b.lio_args.p);
             FLB_CUDA(h, cudaGetLastError());
         }
         LaunchScope lsx(h, FAM_SOLVE);

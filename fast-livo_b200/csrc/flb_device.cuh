@@ -323,13 +323,53 @@ FLB_HD void lio_row12(const LioPose& c, const double* pI, const float* pb, const
 }
 
 // ------------------------------------------------------------------ kNN over the uniform grid
+// Two cell indexes over the same sorted point array (points ordered by cell, x fastest, then by insertion):
+//  dense:  cell_start[(z*ny + y)*nx + x] = first point of the cell, one entry per cell of the grid box;
+//  sparse: an open-addressing hash table of the OCCUPIED cells only, entries {key, start, end} (SparseCell), with the
+//          cell key packing (z, y, x) + 2^20 in 21 bits each, x lowest, so that key order is dense cell-id order.
+// Sparse mode keeps the GridDesc layout: nx holds the table's slot mask, ny / nz are unused, and the cell-table pointer
+// points at the SparseCell array.
 struct GridDesc {
     float ox, oy, oz;     // origin (min corner)
     float cell, inv_cell;
-    int nx, ny, nz;       // cells per axis; cell id = (z*ny + y)*nx + x  (x fastest)
+    int nx, ny, nz;       // cells per axis; cell id = (z*ny + y)*nx + x  (x fastest); sparse: nx = slot mask
     float max_d2;         // 5.0
     int max_ring;         // ceil(sqrt(max_d2)/cell) + 1
 };
+
+constexpr int kCellKeyBias = 1 << 20;                     // cells more than 2^20 from the origin have no key
+constexpr unsigned long long kNoCell = ~0ull;             // empty hash slot; sorts behind every real key
+
+struct alignas(16) SparseCell {
+    unsigned long long key;
+    int start, end;                                       // [start, end) in the sorted point array
+};
+
+FLB_HD bool cell_key_ok(int c) { return c >= -kCellKeyBias && c < kCellKeyBias; }
+FLB_HD unsigned long long cell_key(int cx, int cy, int cz) {
+    return ((unsigned long long)(cz + kCellKeyBias) << 42) | ((unsigned long long)(cy + kCellKeyBias) << 21) |
+           (unsigned long long)(cx + kCellKeyBias);
+}
+FLB_HD unsigned cell_hash(unsigned long long key) { return (unsigned)((key * 0x9E3779B97F4A7C15ull) >> 32); }
+
+// [start, end) of one cell (0, 0 when empty or out of key range); linear probing from the hashed slot
+FLB_HD void sparse_find(const SparseCell* __restrict__ table, unsigned mask, int cx, int cy, int cz, int& s, int& e) {
+    s = e = 0;
+    if (!(cell_key_ok(cx) && cell_key_ok(cy) && cell_key_ok(cz))) return;
+    const unsigned long long key = cell_key(cx, cy, cz);
+    for (unsigned h = cell_hash(key) & mask;; h = (h + 1) & mask) {
+#if defined(__CUDA_ARCH__)
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(table + h));
+        const unsigned long long k = ((unsigned long long)v.y << 32) | v.x;
+        if (k == key) { s = (int)v.z; e = (int)v.w; return; }
+#else
+        const SparseCell v = table[h];
+        const unsigned long long k = v.key;
+        if (k == key) { s = v.start; e = v.end; return; }
+#endif
+        if (k == kNoCell) return;
+    }
+}
 
 struct Top5 {
     float d[kMatch];
@@ -378,6 +418,32 @@ struct map_pt { float x, y, z, w; };
 #define FLB_LDG4(ptr) (*(ptr))
 #define FLB_LDGI(ptr) (*(ptr))
 #endif
+
+// Row bounds, the one reader of a cell index: the points of cells [xa, xb] of row (z, y) are one contiguous run of the
+// sorted array; returns its [start, end).  Dense: two table reads (the caller clips to the grid).  Sparse: start of the
+// first occupied cell, end of the last; (0, 0) when none is occupied.
+template <bool SPARSE>
+FLB_HD void grid_row(const GridDesc& g, const int* __restrict__ cells, int z, int y, int xa, int xb, int& s, int& e) {
+    if constexpr (!SPARSE) {
+        const int rowbase = (z * g.ny + y) * g.nx;
+        s = FLB_LDGI(cells + rowbase + xa);
+        e = FLB_LDGI(cells + rowbase + xb + 1);
+    } else {
+        const SparseCell* table = reinterpret_cast<const SparseCell*>(cells);
+        int x = xa, e0 = 0;
+        s = 0;
+        for (; x <= xb; ++x) {
+            sparse_find(table, (unsigned)g.nx, x, y, z, s, e0);
+            if (e0 > s) break;
+        }
+        e = e0;
+        for (int x1 = xb; x1 > x; --x1) {
+            int s1, e1;
+            sparse_find(table, (unsigned)g.nx, x1, y, z, s1, e1);
+            if (e1 > s1) { e = e1; break; }
+        }
+    }
+}
 
 // Walk `nruns` (<= 9) runs of sorted map points whose [start, end) bounds sit in the per-thread scratch (start of run k
 // at rows[k * rstride], end at rows[(9 + k) * rstride]) as ONE candidate sequence, up to four points (independent 16-B
@@ -441,32 +507,60 @@ FLB_HD void knn_walk_runs(const map_pt* __restrict__ pts, const int* rows, int r
 // a surface ends) are nine 3-cell rows; the shell of ring r >= 2 is (2r+1)-cell rows on its z / y faces and single cells
 // at x = cx -+ r elsewhere.  (A query displaced from the surfaces by the prior's error -- the first pass of a frame --
 // needs ring 2 or 3: round 1 walked those shells one run and one dependent round trip at a time.)
+//
+// SPARSE: `cells` is the SparseCell hash table (see GridDesc).  There is no grid box, so nothing is clipped and there is
+// no early exit outside it; rings 0+1 are 27 independent cell probes (a row's run = first to last occupied cell), the
+// shells r >= 2 probe cell by cell.  Runs, their order and the termination bounds are the dense ones, so on a shared
+// cell geometry both indexes return bit-identical results.
+template <bool SPARSE = false>
 FLB_HD void knn5_grid(const GridDesc& g, const int* __restrict__ cell_start, const map_pt* __restrict__ pts,
                       float qx, float qy, float qz, Top5& t, int* rows, int rstride) {
     // rows: per-thread scratch for 18 ints, element k at rows[k * rstride] (shared memory on the device,
     // one column per thread, so a warp's accesses are conflict-free)
     top5_init(t);
     const float fx = (qx - g.ox) * g.inv_cell, fy = (qy - g.oy) * g.inv_cell, fz = (qz - g.oz) * g.inv_cell;
-    // far outside the grid: nothing within sqrt(max_d2)
-    const float lim = (float)(g.max_ring + 2);
-    if (!(fx > -lim && fy > -lim && fz > -lim && fx < (float)g.nx + lim && fy < (float)g.ny + lim &&
-          fz < (float)g.nz + lim))
-        return;
+    if constexpr (SPARSE) {
+        // beyond the key range (+ the rings): no cell there has a key
+        const float lim = (float)(kCellKeyBias + g.max_ring + 2);
+        if (!(fx > -lim && fy > -lim && fz > -lim && fx < lim && fy < lim && fz < lim)) return;
+    } else {
+        // far outside the grid: nothing within sqrt(max_d2)
+        const float lim = (float)(g.max_ring + 2);
+        if (!(fx > -lim && fy > -lim && fz > -lim && fx < (float)g.nx + lim && fy < (float)g.ny + lim &&
+              fz < (float)g.nz + lim))
+            return;
+    }
     const int cx = (int)floorf(fx), cy = (int)floorf(fy), cz = (int)floorf(fz);
     float mx = fminf(fx - (float)cx, (float)(cx + 1) - fx);
     float my = fminf(fy - (float)cy, (float)(cy + 1) - fy);
     float mz = fminf(fz - (float)cz, (float)(cz + 1) - fz);
     const float margin = fmaxf(fminf(mx, fminf(my, mz)) * g.cell - 1e-3f * g.cell, 0.f);
     {
-        // rings 0+1: rows (dz, dy) in {-1,0,1}^2, x-range [cx-1, cx+1] clipped to the grid
-        const int xa = cx - 1 < 0 ? 0 : cx - 1, xb = cx + 1 >= g.nx ? g.nx - 1 : cx + 1;
-        FLB_UNROLL
-        for (int k = 0; k < 9; ++k) {
-            const int z = cz + k / 3 - 1, y = cy + k % 3 - 1;
-            const bool in = (z >= 0 && z < g.nz && y >= 0 && y < g.ny && xa <= xb);
-            const int rowbase = in ? (z * g.ny + y) * g.nx : 0;
-            rows[k * rstride] = in ? FLB_LDGI(cell_start + rowbase + xa) : 0;
-            rows[(9 + k) * rstride] = in ? FLB_LDGI(cell_start + rowbase + xb + 1) : 0;
+        if constexpr (SPARSE) {
+            // rings 0+1: 27 independent probes, then each row's run from its first to its last occupied cell
+            const SparseCell* table = reinterpret_cast<const SparseCell*>(cell_start);
+            int cs[27], ce[27];
+            FLB_UNROLL
+            for (int k = 0; k < 27; ++k)
+                sparse_find(table, (unsigned)g.nx, cx + k % 3 - 1, cy + (k / 3) % 3 - 1, cz + k / 9 - 1, cs[k], ce[k]);
+            FLB_UNROLL
+            for (int k = 0; k < 9; ++k) {
+                const int* s3 = cs + 3 * k;
+                const int* e3 = ce + 3 * k;
+                rows[k * rstride] = e3[0] > s3[0] ? s3[0] : (e3[1] > s3[1] ? s3[1] : s3[2]);
+                rows[(9 + k) * rstride] = e3[2] > s3[2] ? e3[2] : (e3[1] > s3[1] ? e3[1] : e3[0]);
+            }
+        } else {
+            // rings 0+1: rows (dz, dy) in {-1,0,1}^2, x-range [cx-1, cx+1] clipped to the grid
+            const int xa = cx - 1 < 0 ? 0 : cx - 1, xb = cx + 1 >= g.nx ? g.nx - 1 : cx + 1;
+            FLB_UNROLL
+            for (int k = 0; k < 9; ++k) {
+                const int z = cz + k / 3 - 1, y = cy + k % 3 - 1;
+                const bool in = (z >= 0 && z < g.nz && y >= 0 && y < g.ny && xa <= xb);
+                const int rowbase = in ? (z * g.ny + y) * g.nx : 0;
+                rows[k * rstride] = in ? FLB_LDGI(cell_start + rowbase + xa) : 0;
+                rows[(9 + k) * rstride] = in ? FLB_LDGI(cell_start + rowbase + xb + 1) : 0;
+            }
         }
         knn_walk_runs(pts, rows, rstride, 9, qx, qy, qz, t);
         const float bound = g.cell + margin;
@@ -476,28 +570,48 @@ FLB_HD void knn5_grid(const GridDesc& g, const int* __restrict__ cell_start, con
     }
     for (int r = 2; r <= g.max_ring; ++r) {
         const int z0 = cz - r, z1 = cz + r, y0 = cy - r, y1 = cy + r, x0 = cx - r, x1 = cx + r;
-        const int xa = x0 < 0 ? 0 : x0, xb = x1 >= g.nx ? g.nx - 1 : x1;
         int cnt = 0;
-        for (int z = (z0 < 0 ? 0 : z0); z <= (z1 >= g.nz ? g.nz - 1 : z1); ++z) {
-            const bool zface = (z == z0) || (z == z1);
-            for (int y = (y0 < 0 ? 0 : y0); y <= (y1 >= g.ny ? g.ny - 1 : y1); ++y) {
-                const int rowbase = (z * g.ny + y) * g.nx;
-                if (zface || y == y0 || y == y1) {
-                    if (xa <= xb) {
-                        rows[cnt * rstride] = FLB_LDGI(cell_start + rowbase + xa);
-                        rows[(9 + cnt) * rstride] = FLB_LDGI(cell_start + rowbase + xb + 1);
-                        if (++cnt == 9) { knn_walk_runs(pts, rows, rstride, 9, qx, qy, qz, t); cnt = 0; }
+        if constexpr (!SPARSE) {
+            const int xa = x0 < 0 ? 0 : x0, xb = x1 >= g.nx ? g.nx - 1 : x1;
+            for (int z = (z0 < 0 ? 0 : z0); z <= (z1 >= g.nz ? g.nz - 1 : z1); ++z) {
+                const bool zface = (z == z0) || (z == z1);
+                for (int y = (y0 < 0 ? 0 : y0); y <= (y1 >= g.ny ? g.ny - 1 : y1); ++y) {
+                    const int rowbase = (z * g.ny + y) * g.nx;
+                    if (zface || y == y0 || y == y1) {
+                        if (xa <= xb) {
+                            rows[cnt * rstride] = FLB_LDGI(cell_start + rowbase + xa);
+                            rows[(9 + cnt) * rstride] = FLB_LDGI(cell_start + rowbase + xb + 1);
+                            if (++cnt == 9) { knn_walk_runs(pts, rows, rstride, 9, qx, qy, qz, t); cnt = 0; }
+                        }
+                    } else {
+                        if (x0 >= 0 && x0 < g.nx) {
+                            rows[cnt * rstride] = FLB_LDGI(cell_start + rowbase + x0);
+                            rows[(9 + cnt) * rstride] = FLB_LDGI(cell_start + rowbase + x0 + 1);
+                            if (++cnt == 9) { knn_walk_runs(pts, rows, rstride, 9, qx, qy, qz, t); cnt = 0; }
+                        }
+                        if (x1 >= 0 && x1 < g.nx) {
+                            rows[cnt * rstride] = FLB_LDGI(cell_start + rowbase + x1);
+                            rows[(9 + cnt) * rstride] = FLB_LDGI(cell_start + rowbase + x1 + 1);
+                            if (++cnt == 9) { knn_walk_runs(pts, rows, rstride, 9, qx, qy, qz, t); cnt = 0; }
+                        }
                     }
-                } else {
-                    if (x0 >= 0 && x0 < g.nx) {
-                        rows[cnt * rstride] = FLB_LDGI(cell_start + rowbase + x0);
-                        rows[(9 + cnt) * rstride] = FLB_LDGI(cell_start + rowbase + x0 + 1);
-                        if (++cnt == 9) { knn_walk_runs(pts, rows, rstride, 9, qx, qy, qz, t); cnt = 0; }
-                    }
-                    if (x1 >= 0 && x1 < g.nx) {
-                        rows[cnt * rstride] = FLB_LDGI(cell_start + rowbase + x1);
-                        rows[(9 + cnt) * rstride] = FLB_LDGI(cell_start + rowbase + x1 + 1);
-                        if (++cnt == 9) { knn_walk_runs(pts, rows, rstride, 9, qx, qy, qz, t); cnt = 0; }
+                }
+            }
+        } else {
+            // unclipped: z / y faces are (2r+1)-cell rows, elsewhere the cells x0 and x1; empty runs are not queued
+            for (int z = z0; z <= z1; ++z) {
+                const bool zface = (z == z0) || (z == z1);
+                for (int y = y0; y <= y1; ++y) {
+                    const bool full = zface || y == y0 || y == y1;
+                    for (int part = 0; part < (full ? 1 : 2); ++part) {
+                        int s, e;
+                        if (full) grid_row<true>(g, cell_start, z, y, x0, x1, s, e);
+                        else grid_row<true>(g, cell_start, z, y, part ? x1 : x0, part ? x1 : x0, s, e);
+                        if (e > s) {
+                            rows[cnt * rstride] = s;
+                            rows[(9 + cnt) * rstride] = e;
+                            if (++cnt == 9) { knn_walk_runs(pts, rows, rstride, 9, qx, qy, qz, t); cnt = 0; }
+                        }
                     }
                 }
             }

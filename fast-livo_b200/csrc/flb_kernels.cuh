@@ -363,6 +363,13 @@ __global__ void k_vox_keys_rel(const float* __restrict__ xyz, int n, float ds, i
     keys[i] = (unsigned long long)ix | ((unsigned long long)iy << sy) | ((unsigned long long)iz << sz);
     vals[i] = i;
 }
+// sparse: no grid box to clip to (the new points were checked against the key range)
+template <bool SPARSE>
+__device__ __forceinline__ int grid_axis_cell_t(float v, float o, float inv_cell, int n) {
+    if constexpr (SPARSE) return (int)floorf((v - o) * inv_cell);
+    else return grid_axis_cell(v, o, inv_cell, n);
+}
+template <bool SPARSE>
 __global__ void k_vox_resolve_incremental(const unsigned long long* __restrict__ keys, const int* __restrict__ vals,
                                           const float* __restrict__ nxyz, int n, float ds, GridDesc g, const int* __restrict__ cell_start,
                                           const float4* __restrict__ pts, unsigned char* __restrict__ dead,
@@ -382,15 +389,15 @@ __global__ void k_vox_resolve_incremental(const unsigned long long* __restrict__
         mid[a] = (float)((double)mn[a] + (double)(mx[a] - mn[a]) / 2.0);
     }
     // Downsample_Storage = live points in the half-open box (Search_by_range, :1001)
-    const int cx0 = grid_axis_cell(mn[0], g.ox, g.inv_cell, g.nx), cx1 = grid_axis_cell(mx[0], g.ox, g.inv_cell, g.nx);
-    const int cy0 = grid_axis_cell(mn[1], g.oy, g.inv_cell, g.ny), cy1 = grid_axis_cell(mx[1], g.oy, g.inv_cell, g.ny);
-    const int cz0 = grid_axis_cell(mn[2], g.oz, g.inv_cell, g.nz), cz1 = grid_axis_cell(mx[2], g.oz, g.inv_cell, g.nz);
+    const int cx0 = grid_axis_cell_t<SPARSE>(mn[0], g.ox, g.inv_cell, g.nx), cx1 = grid_axis_cell_t<SPARSE>(mx[0], g.ox, g.inv_cell, g.nx);
+    const int cy0 = grid_axis_cell_t<SPARSE>(mn[1], g.oy, g.inv_cell, g.ny), cy1 = grid_axis_cell_t<SPARSE>(mx[1], g.oy, g.inv_cell, g.ny);
+    const int cz0 = grid_axis_cell_t<SPARSE>(mn[2], g.oz, g.inv_cell, g.nz), cz1 = grid_axis_cell_t<SPARSE>(mx[2], g.oz, g.inv_cell, g.nz);
     int c = 0, best = -1;                           // best >= 0: sorted position of an existing point; <= -2: -(j + 2) of a new one
     float best_d = INFINITY;
     for (int z = cz0; z <= cz1; ++z)
         for (int y = cy0; y <= cy1; ++y) {
-            const int row = (z * g.ny + y) * g.nx;
-            const int s0 = cell_start[row + cx0], s1 = cell_start[row + cx1 + 1];
+            int s0, s1;
+            grid_row<SPARSE>(g, cell_start, z, y, cx0, cx1, s0, s1);
             for (int m = s0; m < s1; ++m) {
                 const float4 p = pts[m];
                 if (mn[0] <= p.x && mx[0] > p.x && mn[1] <= p.y && mx[1] > p.y && mn[2] <= p.z && mx[2] > p.z) {
@@ -414,8 +421,8 @@ __global__ void k_vox_resolve_incremental(const unsigned long long* __restrict__
     if (!replaced) return;                          // the single existing point beat every new one: nothing changes
     for (int z = cz0; z <= cz1; ++z)
         for (int y = cy0; y <= cy1; ++y) {
-            const int row = (z * g.ny + y) * g.nx;
-            const int s0 = cell_start[row + cx0], s1 = cell_start[row + cx1 + 1];
+            int s0, s1;
+            grid_row<SPARSE>(g, cell_start, z, y, cx0, cx1, s0, s1);
             for (int m = s0; m < s1; ++m) {
                 const float4 p = pts[m];
                 if (m != best && mn[0] <= p.x && mx[0] > p.x && mn[1] <= p.y && mx[1] > p.y && mn[2] <= p.z && mx[2] > p.z) dead[m] = 1;
@@ -481,6 +488,93 @@ __global__ void k_merge_inserts(const float* __restrict__ nxyz, const unsigned* 
     const int pos = cs_new[cell + 1] - (last - first) + (k - first);     // inserts go behind the cell's surviving points
     const float* q = nxyz + 3 * (size_t)ins_vals_sorted[k];
     pts_new[pos] = make_float4(q[0], q[1], q[2], __int_as_float(pos));
+    raw_new[3 * (size_t)pos] = q[0]; raw_new[3 * (size_t)pos + 1] = q[1]; raw_new[3 * (size_t)pos + 2] = q[2];
+}
+
+// ---- sparse cell index (GridDesc): points sorted by 64-bit cell key, a hash table of the occupied cells
+__device__ __forceinline__ int lower_bound_u64(const unsigned long long* __restrict__ a, int n, unsigned long long v) {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (a[mid] < v) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+__device__ __forceinline__ unsigned long long point_cell_key(float x, float y, float z, const GridDesc& g) {
+    return cell_key((int)floorf((x - g.ox) * g.inv_cell), (int)floorf((y - g.oy) * g.inv_cell), (int)floorf((z - g.oz) * g.inv_cell));
+}
+__global__ void k_sparse_cell_keys(const float* __restrict__ xyz, int M, GridDesc g, unsigned long long* __restrict__ keys,
+                                   int* __restrict__ vals) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= M) return;
+    keys[i] = point_cell_key(xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2], g);
+    vals[i] = i;
+}
+// occupied cells of the sorted key array (one per run head)
+__global__ void k_sparse_count_cells(const unsigned long long* __restrict__ keys, int M, int* __restrict__ count) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool head = i < M && (i == 0 || keys[i - 1] != keys[i]);
+    const unsigned b = __ballot_sync(0xffffffffu, head);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(count, __popc(b));
+}
+// one thread per run head claims a slot by atomicCAS on the key (linear probing, as sparse_find reads it)
+__global__ void k_sparse_insert(const unsigned long long* __restrict__ keys, int M, SparseCell* __restrict__ table, unsigned mask) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= M) return;
+    const unsigned long long k = keys[i];
+    if (i > 0 && keys[i - 1] == k) return;
+    const int end = lower_bound_u64(keys + i, M - i, k + 1) + i;
+    for (unsigned h = cell_hash(k) & mask;; h = (h + 1) & mask) {
+        if (atomicCAS(&table[h].key, kNoCell, k) == kNoCell) {
+            table[h].start = i;
+            table[h].end = end;
+            return;
+        }
+    }
+}
+// Incremental Add_Points on the sparse index: as k_insert_cells / k_merge_* above, with 64-bit cell keys in place of
+// cell ids; the cell bounds come from the old sorted key array instead of a cell table.
+__global__ void k_insert_keys_sparse(const float* __restrict__ nxyz, int n, const unsigned char* __restrict__ ins, GridDesc g,
+                                     unsigned long long* __restrict__ keys, int* __restrict__ vals) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    keys[i] = ins[i] ? point_cell_key(nxyz[3 * (size_t)i], nxyz[3 * (size_t)i + 1], nxyz[3 * (size_t)i + 2], g) : kNoCell;
+    vals[i] = i;
+}
+__global__ void k_merge_counts_sparse(const int* __restrict__ dead_before, const unsigned char* __restrict__ dead, int M,
+                                      const unsigned long long* __restrict__ ins_keys_sorted, int n, int* __restrict__ counts) {
+    if (threadIdx.x == 0 && blockIdx.x == 0) {
+        counts[0] = dead_before[M - 1] + dead[M - 1];
+        counts[1] = lower_bound_u64(ins_keys_sorted, n, kNoCell);
+    }
+}
+__global__ void k_merge_existing_sparse(const float4* __restrict__ pts_old, const unsigned long long* __restrict__ keys_old,
+                                        const unsigned char* __restrict__ dead, const int* __restrict__ dead_before, int M,
+                                        const unsigned long long* __restrict__ ins_keys_sorted, int n, float4* __restrict__ pts_new,
+                                        float* __restrict__ raw_new, unsigned long long* __restrict__ keys_new) {
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= M || dead[m]) return;
+    float4 p = pts_old[m];
+    const unsigned long long key = keys_old[m];
+    const int pos = m - dead_before[m] + lower_bound_u64(ins_keys_sorted, n, key);
+    p.w = __int_as_float(pos);
+    pts_new[pos] = p;
+    keys_new[pos] = key;
+    raw_new[3 * (size_t)pos] = p.x; raw_new[3 * (size_t)pos + 1] = p.y; raw_new[3 * (size_t)pos + 2] = p.z;
+}
+__global__ void k_merge_inserts_sparse(const float* __restrict__ nxyz, const unsigned long long* __restrict__ ins_keys_sorted,
+                                       const int* __restrict__ ins_vals_sorted, const int* __restrict__ counts,
+                                       const unsigned long long* __restrict__ keys_old, const int* __restrict__ dead_before, int M,
+                                       float4* __restrict__ pts_new, float* __restrict__ raw_new, unsigned long long* __restrict__ keys_new) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= counts[1]) return;
+    const unsigned long long key = ins_keys_sorted[k];
+    // behind the cell's surviving points: survivors with key <= this one, then the k inserts sorted before this one
+    const int s = lower_bound_u64(keys_old, M, key + 1);
+    const int pos = s - (s < M ? dead_before[s] : counts[0]) + k;
+    const float* q = nxyz + 3 * (size_t)ins_vals_sorted[k];
+    pts_new[pos] = make_float4(q[0], q[1], q[2], __int_as_float(pos));
+    keys_new[pos] = key;
     raw_new[3 * (size_t)pos] = q[0]; raw_new[3 * (size_t)pos + 1] = q[1]; raw_new[3 * (size_t)pos + 2] = q[2];
 }
 
@@ -650,13 +744,14 @@ __global__ void __launch_bounds__(kScanSortBlock) k_scan_sort_block(const float*
 // ---------------------------------------------------------------------------------------
 // standalone kNN (flb_knn): thread per query
 // ---------------------------------------------------------------------------------------
+template <bool SPARSE>
 __global__ void k_knn(GridDesc g, const int* __restrict__ cell_start, const float4* __restrict__ pts,
                       const float* __restrict__ q, int nq, int* __restrict__ idx, float* __restrict__ d2) {
     __shared__ int s_rows[18][128];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nq) return;
     Top5 t;
-    knn5_grid(g, cell_start, pts, q[3 * (size_t)i], q[3 * (size_t)i + 1], q[3 * (size_t)i + 2], t, &s_rows[0][threadIdx.x], 128);
+    knn5_grid<SPARSE>(g, cell_start, pts, q[3 * (size_t)i], q[3 * (size_t)i + 1], q[3 * (size_t)i + 2], t, &s_rows[0][threadIdx.x], 128);
 #pragma unroll
     for (int j = 0; j < kMatch; ++j) {
         const bool ok = (t.i[j] >= 0) && !(t.d[j] > g.max_d2);
@@ -673,7 +768,7 @@ struct LioArgs {
     const float4* scan;          // N body points in Morton order, w = original index
     int N;
     GridDesc grid;
-    const int* cell_start;
+    const int* cell_start;       // dense cell table, or the sparse SparseCell table (GridDesc)
     const float4* map_pts;
     const State18* state;        // device state (pose read each pass)
     LioParamsDev prm;
@@ -704,7 +799,7 @@ struct LioArgs {
     WarmList warm;               // persistent kernel: pages to touch before the first pass (n = 0: none)
 };
 
-template <int W>
+template <int W, bool SPARSE>
 __device__ __forceinline__ void lio_point(const LioArgs& a, const LioPose& pose, bool rematch, int i, bool& active,
                                           double (&row)[W], double& z, double& absres, int* rows, int rstride) {
     active = false;
@@ -723,7 +818,7 @@ __device__ __forceinline__ void lio_point(const LioArgs& a, const LioPose& pose,
     if (probe) a.probe[0] = global_ns();
     if (rematch) {
         Top5 t;
-        knn5_grid(a.grid, a.cell_start, a.map_pts, pw[0], pw[1], pw[2], t, rows, rstride);
+        knn5_grid<SPARSE>(a.grid, a.cell_start, a.map_pts, pw[0], pw[1], pw[2], t, rows, rstride);
         if (probe) a.probe[1] = global_ns();
         const bool five = t.i[kMatch - 1] >= 0;
         sel = five && !(t.d[kMatch - 1] > a.grid.max_d2);     // src/laserMapping.cpp:1549 (+ :1567 size check)
@@ -838,7 +933,7 @@ __device__ __forceinline__ void lio_accumulate(double (&acc)[lio_packed(W)], con
 }
 
 // kernel-per-pass: one thread per scan point
-template <int W, int BLOCK>
+template <int W, int BLOCK, bool SPARSE>
 __device__ __forceinline__ void lio_pass_body(const LioArgs& a) {
     constexpr int K = lio_packed(W);
     __shared__ LioPose s_pose;
@@ -860,18 +955,18 @@ __device__ __forceinline__ void lio_pass_body(const LioArgs& a) {
     if (i < a.N) {
         bool active;
         double row[W], z, absres;
-        lio_point<W>(a, s_pose, rematch != 0, i, active, row, z, absres, &s_rows[0][threadIdx.x], BLOCK);
+        lio_point<W, SPARSE>(a, s_pose, rematch != 0, i, active, row, z, absres, &s_rows[0][threadIdx.x], BLOCK);
         if (active) lio_accumulate<W>(acc, row, z, absres);
     }
     block_reduce_store<K, BLOCK>(acc, s_acc, a.partials);
 }
-template <int W, int BLOCK>
-__global__ void __launch_bounds__(BLOCK) k_lio_pass(LioArgs a) { lio_pass_body<W, BLOCK>(a); }
+template <int W, int BLOCK, bool SPARSE>
+__global__ void __launch_bounds__(BLOCK) k_lio_pass(LioArgs a) { lio_pass_body<W, BLOCK, SPARSE>(a); }
 
 // Batched frames (SURVEY.md section 7 H2(iv)): blockIdx.y = frame; every frame has its own scan, state, control
 // block and partial sums (args[frame]), all share the map.  The pass of B frames is ONE launch, so the grid is B times
 // larger than a frame's and the kernel runs where its throughput, not its latency, is what is measured.
-template <int W, int BLOCK>
+template <int W, int BLOCK, bool SPARSE>
 __global__ void __launch_bounds__(BLOCK) k_lio_pass_batched(const LioArgs* __restrict__ args) {
     __shared__ LioArgs s_a;
     {
@@ -881,7 +976,7 @@ __global__ void __launch_bounds__(BLOCK) k_lio_pass_batched(const LioArgs* __res
     }
     __syncthreads();
     if ((int)blockIdx.x * BLOCK >= s_a.N) return;
-    lio_pass_body<W, BLOCK>(s_a);
+    lio_pass_body<W, BLOCK, SPARSE>(s_a);
 }
 
 __global__ void __launch_bounds__(32) k_reduce_only(const double* partials, int nblocks, int K, double* out) {
@@ -2292,7 +2387,7 @@ __device__ __forceinline__ bool leader_wait_arrivals(GridBarrier* b, unsigned ta
 // arrivals of each pass, reduces, solves and publishes the pose packet.  Keeping the leader on one SM
 // keeps its code and its constants (prior block, state_propagat, covariance) warm from pass to pass;
 // a last-arriver leader would run the solve on a different, cold SM every pass.
-template <int BLOCK>
+template <int BLOCK, bool SPARSE>
 __global__ void __launch_bounds__(BLOCK, 1) k_lio_update_persistent(LioArgs a, LioSolveArgs s, GridBarrier* bar,
                                                                  unsigned long long* pkt, unsigned epoch,
                                                                  unsigned long long* trace, unsigned long long* dbg) {
@@ -2342,7 +2437,8 @@ __global__ void __launch_bounds__(BLOCK, 1) k_lio_update_persistent(LioArgs a, L
         // would then pay one DRAM latency per dependent step.  Stream the sorted points and the cell table into L2
         // with bulk prefetches (asynchronous: nobody waits for them), 4 KB per instruction.
         const size_t nb_pts = (size_t)a.M * sizeof(float4);
-        const size_t nb_cells = ((size_t)a.grid.nx * a.grid.ny * a.grid.nz + 1) * sizeof(int) / 16 * 16;
+        const size_t nb_cells = SPARSE ? ((size_t)(unsigned)a.grid.nx + 1) * sizeof(SparseCell)
+                                       : ((size_t)a.grid.nx * a.grid.ny * a.grid.nz + 1) * sizeof(int) / 16 * 16;
         const size_t step = 4096, stride = (size_t)nworkers * BLOCK * step;
         for (size_t off = ((size_t)blockIdx.x * BLOCK + tid) * step; off < nb_pts; off += stride)
             asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<const char*>(a.map_pts) + off),
@@ -2383,7 +2479,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_lio_update_persistent(LioArgs a, L
                 if ((tid & 31) < a.chunk && i < a.N) {
                     bool active;
                     double row[6], z, absres;
-                    lio_point<6>(a, s_pose, nearest != 0, i, active, row, z, absres, &s_rows[0][tid], BLOCK);
+                    lio_point<6, SPARSE>(a, s_pose, nearest != 0, i, active, row, z, absres, &s_rows[0][tid], BLOCK);
                     if (active) lio_accumulate<6>(acc, row, z, absres);
                 }
             }
@@ -3114,7 +3210,7 @@ __device__ __forceinline__ void ikfom_make_pose(const StateIkfom* st, LioPose& p
     m3_T(pose.R_LI, pose.RLIt);
 }
 
-template <int BLOCK>
+template <int BLOCK, bool SPARSE>
 __global__ void __launch_bounds__(BLOCK) k_lio_update_ikfom_persistent(LioArgs a, IkfomSolveArgs s, GridBarrier* bar) {
     constexpr int K = lio_packed(12);
     __shared__ LioPose s_pose;
@@ -3136,7 +3232,7 @@ __global__ void __launch_bounds__(BLOCK) k_lio_update_ikfom_persistent(LioArgs a
             if (i < a.N) {
                 bool active;
                 double row[12], z, absres;
-                lio_point<12>(a, s_pose, converge != 0, i, active, row, z, absres, &s_rows[0][tid], BLOCK);   // converge => redo kNN (:994)
+                lio_point<12, SPARSE>(a, s_pose, converge != 0, i, active, row, z, absres, &s_rows[0][tid], BLOCK);   // converge => redo kNN (:994)
                 if (active) lio_accumulate<12>(acc, row, z, absres);
             }
         }

@@ -103,6 +103,12 @@ int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride_
 int flb_map_delete_boxes(flb_handle* h, const float* boxes, int nb);
 int flb_map_size(const flb_handle* h);
 int flb_map_download(flb_handle* h, float* xyz, int capacity_points, int* M_out);
+/* flb_map_grid_info: the kNN cell geometry in use.  The map's cells are indexed by a dense table over the map's box
+ * (plus a margin); where that would need more than 2^25 cells of flb_config.cell_size the cell is enlarged until it
+ * fits (cell_size reports the enlarged cell).  sparse = 1: a sparse hash index of the occupied cells at the configured
+ * cell (flb_debug_set_map_index).  cells: dense table cells, or occupied cells when sparse; index_bytes: device bytes of
+ * the index.  Any output pointer may be NULL. */
+int flb_map_grid_info(flb_handle* h, double* cell_size, int* sparse, int64_t* cells, int64_t* index_bytes);
 
 /* ---- IMU forward propagation + backward undistortion (SURVEY.md section 8 row f3) ----------------------
  * Replaces ImuProcess::UndistortPcl from src/IMU_Processing.cpp:655 on (called by Process2, :811-849, at
@@ -468,6 +474,9 @@ int flb_debug_scan_order(flb_handle* h, int* src_index, int capacity);
 /* flb_debug_set_scan_sort: ordering path of the following flb_scan_upload calls -- 0 automatic (by size and by
  * whether the handle's stream is busy), 1 the one-block kernel (scans of <= 25 600 points), 2 the device-wide sort. */
 int flb_debug_set_scan_sort(flb_handle* h, int mode);
+/* flb_debug_set_map_index: cell index of the following map rebuilds -- 0 automatic (the dense table), 1 dense always,
+ * 2 the sparse index at the configured cell.  Test and measurement aid. */
+int flb_debug_set_map_index(flb_handle* h, int mode);
 
 #ifdef __cplusplus
 }
