@@ -229,6 +229,7 @@ struct flb_handle {
     DevBuf<GridBarrier> barrier; // grid barrier of the persistent kernels
     DevBuf<unsigned long long> pkt;    // pose packet of the persistent kernels (kPktUnits flagged words)
     unsigned pkt_epoch = 0;            // flag base of the next launch (flags are never reused, see next_epoch)
+    DevBuf<P2PLine> arrive_lines;      // persistent kernels: the worker blocks' sums of a pass, tagged with its flag
     DevBuf<unsigned long long> trace;  // [0..kTraceLen) LIO, [kTraceLen..2*kTraceLen) VIO
     DevBuf<unsigned long long> dbg;    // per-block stage stamps of the last LIO pass (tracing only)
     DevBuf<unsigned long long> dbg_vio;
@@ -566,14 +567,34 @@ int flush_state_ops(flb_handle* h) {
 }
 
 // Flag base for one persistent launch: flags epoch+1 .. epoch+4095 belong to it alone.  On wrap-around the
-// packet is cleared (stream-ordered) so that no stale unit can ever match.
+// packet and the arrival lines are cleared (stream-ordered) so that no stale unit can ever match.
 int next_epoch(flb_handle* h, unsigned* epoch) {
     if (h->pkt_epoch >= 0xFFFF0000u || h->pkt_epoch == 0) {
-        if (h->pkt_epoch) FLB_CUDA(h, cudaMemsetAsync(h->pkt.p, 0, kPktUnits * sizeof(unsigned long long), h->stream));
+        if (h->pkt_epoch) {
+            FLB_CUDA(h, cudaMemsetAsync(h->pkt.p, 0, kPktUnits * sizeof(unsigned long long), h->stream));
+            if (h->arrive_lines.p)
+                FLB_CUDA(h, cudaMemsetAsync(h->arrive_lines.p, 0, h->arrive_lines.cap * sizeof(P2PLine), h->stream));
+        }
         h->pkt_epoch = 4096;
     }
     *epoch = h->pkt_epoch;
     h->pkt_epoch += 4096;
+    return FLB_OK;
+}
+
+// Arrival by lines (kernels: "Arrival by lines"): grid x 29 lines, shared by the LIO and VIO launches (their flags
+// differ).  Zeroed when allocated and, by next_epoch, when the flags wrap.  *lines = null selects the counter path:
+// FLB_LL_ARRIVE=0 (A/B measurement).
+int arrive_lines(flb_handle* h, int grid, P2PLine** lines) {
+    static const int env = [] { const char* e = getenv("FLB_LL_ARRIVE"); return e ? atoi(e) : 1; }();
+    *lines = nullptr;
+    if (!env) return FLB_OK;
+    const size_t need = (size_t)grid * std::max(lio_packed(6), kVioPacked);
+    if (need > h->arrive_lines.cap) {
+        FLB_CUDA(h, h->arrive_lines.reserve(need));
+        FLB_CUDA(h, cudaMemsetAsync(h->arrive_lines.p, 0, h->arrive_lines.cap * sizeof(P2PLine), h->stream));
+    }
+    *lines = h->arrive_lines.p;
     return FLB_OK;
 }
 
@@ -617,6 +638,7 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
         a.partials = h->partials.p;
         s.partials = h->partials.p;
         s.nblocks = workers;
+        { int rcl = arrive_lines(h, grid, &s.lines); if (rcl) return rcl; }
         GridBarrier* bar = h->barrier.p;
         unsigned long long* trace = h->tracing ? h->trace.p : nullptr;
         a.probe = h->tracing ? h->trace.p + 112 : nullptr;
@@ -626,9 +648,10 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
             if (env_warm) {
                 WarmList& w = a.warm;
                 const size_t n1 = (size_t)std::max(h->N, 1);
-                const void* ptr[] = {h->scan.p, h->map_pts.p, cell_index(h), h->plane.p, h->sel.p, h->plane_ok.p, h->partials.p, h->states.p};
-                const size_t len[] = {n1 * 16, (size_t)h->M * 16, index_bytes(h), n1 * 16, n1, n1, (size_t)grid * lio_packed(6) * 8,
-                                      5 * sizeof(State18)};
+                const void* sums = s.lines ? (const void*)s.lines : (const void*)h->partials.p;
+                const void* ptr[] = {h->scan.p, h->map_pts.p, cell_index(h), h->plane.p, h->sel.p, h->plane_ok.p, sums, h->states.p};
+                const size_t len[] = {n1 * 16, (size_t)h->M * 16, index_bytes(h), n1 * 16, n1, n1,
+                                      (size_t)grid * lio_packed(6) * (s.lines ? sizeof(P2PLine) : 8), 5 * sizeof(State18)};
                 w.n = 8;
                 for (int k = 0; k < 8; ++k) { w.p[k] = ptr[k]; w.bytes[k] = len[k]; }
             }
@@ -780,6 +803,8 @@ int enqueue_vio_update(flb_handle* h, const flb_vio_params* prm) {
         a.partials = h->partials.p;
         s.partials = h->partials.p;
         s.nblocks = workers;
+        // plain per-patch errors (FLB_DEFER=0, single GPU) are ordered for the leader only by the counter: keep it
+        if (fused || s.err_units) { int rcl = arrive_lines(h, grid, &s.lines); if (rcl) return rcl; }
         GridBarrier* bar = h->barrier.p;
         unsigned long long* trace = h->tracing ? h->trace.p + kTraceLen : nullptr;
         unsigned long long* pkt = h->pkt.p;
@@ -799,8 +824,10 @@ int enqueue_vio_update(flb_handle* h, const flb_vio_params* prm) {
             if (env_warm) {
                 WarmList& w = a.warm;
                 const size_t pn = (size_t)std::max(a.Pn, 1);
-                const void* ptr[] = {h->img.p, h->patch_pos.p, h->patch_ref.p, h->patch_level.p, h->errors.p, h->partials.p};
-                const size_t len[] = {(size_t)h->img_w * h->img_h, pn * 24, pn * 768, pn * 4, 2 * (size_t)h->err_stride * 4, (size_t)grid * kVioPacked * 8};
+                const void* sums = s.lines ? (const void*)s.lines : (const void*)h->partials.p;
+                const void* ptr[] = {h->img.p, h->patch_pos.p, h->patch_ref.p, h->patch_level.p, h->errors.p, sums};
+                const size_t len[] = {(size_t)h->img_w * h->img_h, pn * 24, pn * 768, pn * 4, 2 * (size_t)h->err_stride * 4,
+                                      (size_t)grid * kVioPacked * (s.lines ? sizeof(P2PLine) : 8)};
                 w.n = 6;
                 for (int k = 0; k < 6; ++k) { w.p[k] = ptr[k]; w.bytes[k] = len[k]; }
             }
@@ -962,7 +989,7 @@ int flb_destroy(flb_handle* h) {
     h->plane_ok.release(); h->plane.release(); h->x_world.release(); h->x_nn_d2.release(); h->x_pd2.release();
     h->x_nn_idx.release(); h->x_rowmask.release(); h->x_rows.release(); h->x_meas.release(); h->partials.release();
     h->packed.release(); h->pose12.release(); h->prior.release(); h->scan_raw.release(); h->skeys.release(); h->skeys_sorted.release(); h->svals.release(); h->svals_sorted.release(); h->x_pabcd.release(); h->G_last.release(); h->states.release();
-    h->lio_ctrl.release(); h->vio_ctrl.release(); h->ik_states.release(); h->ik_ctrl.release(); h->barrier.release(); h->pkt.release(); h->trace.release(); h->dbg.release(); h->dbg_vio.release(); h->imu_buf.release(); h->imu_pts.release(); h->imu_heads.release(); h->vm_key.release(); h->vm_val.release(); h->vm_pts.release(); h->vm_win.release(); h->vm_pose.release(); h->img.release(); h->patch_pos.release(); h->patch_ref.release();
+    h->lio_ctrl.release(); h->vio_ctrl.release(); h->ik_states.release(); h->ik_ctrl.release(); h->barrier.release(); h->pkt.release(); h->arrive_lines.release(); h->trace.release(); h->dbg.release(); h->dbg_vio.release(); h->imu_buf.release(); h->imu_pts.release(); h->imu_heads.release(); h->vm_key.release(); h->vm_val.release(); h->vm_pts.release(); h->vm_win.release(); h->vm_pose.release(); h->img.release(); h->patch_pos.release(); h->patch_ref.release();
     h->patch_level.release(); h->errors.release(); h->err_units.release(); h->errors_all.release(); h->x_z.release(); h->x_H.release();
     h->st_map.release(); h->st_scan.release(); h->st_img.release(); h->st_patch.release(); h->st_state.release();
     h->st_misc.release(); h->pin_out.release();

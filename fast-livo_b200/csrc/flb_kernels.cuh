@@ -893,10 +893,35 @@ __device__ __forceinline__ void lio_make_pose(const LioArgs& a, LioPose& pose, b
     m3_T(pose.R_LI, pose.RLIt);
 }
 
+// LL-style 16-byte line {lo32, tag, hi32, tag}: one store instruction whose 8-byte halves are atomic, so a reader that
+// sees the tag in both halves has the whole double -- it polls the data, with no flag and no fence (the fused
+// multi-GPU exchange and the persistent kernels' arrival both use it).
+struct __align__(16) P2PLine { unsigned d0, f0, d1, f1; };
+__device__ __forceinline__ void ll_store_line(P2PLine* p, double v, unsigned tag) {
+    const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+    asm volatile("st.volatile.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"((unsigned)u), "r"(tag),
+                 "r"((unsigned)(u >> 32)), "r"(tag)
+                 : "memory");
+}
+__device__ __forceinline__ uint4 ll_load_raw(const P2PLine* p) {
+    uint4 r;
+    asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
+    return r;
+}
+__device__ __forceinline__ bool ll_line_value(const uint4& r, unsigned tag, double& v) {
+    v = __longlong_as_double((long long)(((unsigned long long)r.z << 32) | r.x));
+    return r.y == tag && r.w == tag;
+}
+__device__ __forceinline__ bool ll_load_line(const P2PLine* p, unsigned tag, double& v) {
+    return ll_line_value(ll_load_raw(p), tag, v);
+}
+
 // Block-level reduction of per-thread accumulators acc[K] -> partials[blockIdx.x][K]:
-// warp shuffle tree, then the warps in fixed order.
+// warp shuffle tree, then the warps in fixed order.  With `lines` (persistent kernels) the K sums go out as lines
+// lines[blockIdx.x * K + q] tagged `tag` instead: that store is the block's arrival (see "Arrival by lines").
 template <int K, int BLOCK>
-__device__ __forceinline__ void block_reduce_store(const double (&acc)[K], double (*s_acc)[K], double* partials) {
+__device__ __forceinline__ void block_reduce_store(const double (&acc)[K], double (*s_acc)[K], double* partials,
+                                                   P2PLine* lines = nullptr, unsigned tag = 0u) {
     constexpr int NW = BLOCK / 32;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if constexpr (K <= 32) {
@@ -914,7 +939,8 @@ __device__ __forceinline__ void block_reduce_store(const double (&acc)[K], doubl
         double s = 0.0;
 #pragma unroll
         for (int w = 0; w < NW; ++w) s += s_acc[w][q];
-        partials[(size_t)blockIdx.x * K + q] = s;
+        if (lines) ll_store_line(lines + (size_t)blockIdx.x * K + q, s, tag);
+        else partials[(size_t)blockIdx.x * K + q] = s;
     }
 }
 
@@ -1000,7 +1026,6 @@ __global__ void __launch_bounds__(32) k_reduce_only(const double* partials, int 
 // ---------------------------------------------------------------------------------------
 constexpr int kP2PMaxWorld = 8;
 constexpr int kP2PErrCap = 16384;        // per-rank patch shard capacity of the error gather
-struct __align__(16) P2PLine { unsigned d0, f0, d1, f1; };
 struct P2PMailbox {
     P2PLine sums[2][kP2PMaxWorld][32];                       // [parity][source rank][k]; k = 31: that rank's patch count
     unsigned long long errs[2][kP2PMaxWorld][kP2PErrCap];    // [parity][source rank][local patch] = {tag : float bits}
@@ -1011,18 +1036,6 @@ struct P2PArgs {
     unsigned long long* seq;             // device-resident exchange counter (same value on every rank)
 };
 
-__device__ __forceinline__ void ll_store_line(P2PLine* p, double v, unsigned tag) {
-    const unsigned long long u = (unsigned long long)__double_as_longlong(v);
-    asm volatile("st.volatile.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"((unsigned)u), "r"(tag),
-                 "r"((unsigned)(u >> 32)), "r"(tag)
-                 : "memory");
-}
-__device__ __forceinline__ bool ll_load_line(const P2PLine* p, unsigned tag, double& v) {
-    unsigned a, b, c, d;
-    asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "l"(p) : "memory");
-    v = __longlong_as_double((long long)(((unsigned long long)c << 32) | a));
-    return b == tag && d == tag;
-}
 __device__ __forceinline__ void ll_store_u64(unsigned long long* p, unsigned long long v) {
     asm volatile("st.volatile.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
@@ -1227,7 +1240,8 @@ __device__ __forceinline__ void vio_make_pose_from(const VioArgs& a, VioPose& po
 
 template <int BLOCK>
 __device__ __forceinline__ void vio_block_reduce_store(double accv, double n_meas, double skipped,
-                                                       double (*s_acc)[kVioPacked], double* partials) {
+                                                       double (*s_acc)[kVioPacked], double* partials,
+                                                       P2PLine* lines = nullptr, unsigned tag = 0u) {
     constexpr int NW = BLOCK / 32;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (lane < 27) s_acc[warp][lane] = accv;
@@ -1237,7 +1251,8 @@ __device__ __forceinline__ void vio_block_reduce_store(double accv, double n_mea
         double s = 0.0;
 #pragma unroll
         for (int w = 0; w < NW; ++w) s += s_acc[w][q];
-        partials[(size_t)blockIdx.x * kVioPacked + q] = s;
+        if (lines) ll_store_line(lines + (size_t)blockIdx.x * kVioPacked + q, s, tag);
+        else partials[(size_t)blockIdx.x * kVioPacked + q] = s;
     }
 }
 
@@ -1345,12 +1360,52 @@ __device__ __forceinline__ void store_state(State18* dst, const State18* src, in
     for (int e = tid; e < n; e += nt) d[e] = s[e];
 }
 
+// Leader-side watchdog of a pass's arrivals (~seconds): a block that never arrives becomes FLB_ERR_TIMEOUT, not a hang.
+constexpr unsigned long long kArriveSpinLimit = 40000000ull;
+
+// Poll the n <= N lines p[0], p[stride], ... until each carries `tag`; v[u] = its value (0.0 for u >= n).  Every
+// attempt loads all lines still missing before checking any (one round trip per attempt) and re-reads only those.
+// False when the watchdog tripped (this thread's limit, or another block's timeout flag): v is then incomplete.
+template <int N>
+__device__ __forceinline__ bool ll_poll_lines(const P2PLine* p, int stride, int n, unsigned tag, double (&v)[N], int* timeout_flag) {
+    // the loaded words are the result: a line is not re-read once its tag matched (no second copy of the values)
+    uint4 r[N];
+    unsigned pending = 0u;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+        r[u] = make_uint4(0u, tag, 0u, tag);          // lines past n: +0.0
+        if (u < n) pending |= 1u << u;
+    }
+    bool ok = true;
+    unsigned long long spins = 0;
+    while (pending) {
+#pragma unroll
+        for (int u = 0; u < N; ++u)
+            if (pending >> u & 1u) r[u] = ll_load_raw(p + (size_t)u * stride);
+#pragma unroll
+        for (int u = 0; u < N; ++u)
+            if (r[u].y == tag && r[u].w == tag) pending &= ~(1u << u);
+        if (pending) {
+            if (++spins > kArriveSpinLimit) { *timeout_flag = 1; ok = false; break; }
+            if ((spins & 0xffff) == 0 && *((volatile int*)timeout_flag)) { ok = false; break; }
+        }
+    }
+#pragma unroll
+    for (int u = 0; u < N; ++u) ll_line_value(r[u], tag, v[u]);
+    return ok;
+}
+
 // Fixed-order reduction of the block partials by a team of TN threads: its first TN/32-1 warps take one
 // contiguous slice of the blocks each (summed in block order from batches of 16 independent L2 loads,
 // guarded at the tail: adding +0.0 is exact), then the slices are combined left to right.  Meanwhile
 // lane 0 of the team's LAST warp forms vec = state_propagat (-) state, which only needs sm.x / sm.xp.
-template <int K, int TN, class TeamT>
-__device__ __forceinline__ void team_reduce_vec(const double* partials, int nblocks, LeaderSmem& sm, int tid) {
+// With `lines` (persistent kernels) the team polls the workers' lines of the pass (tag) instead of waiting for an
+// arrival count first; the values, the slices and the order of the additions are the same, so is the sum.
+// B: loads in flight per thread (one round trip for a slice of up to B blocks; PARTS x B >= 160 covers every H100
+// grid).  A line takes twice the registers of a double, so the persistent VIO kernel (128 registers) uses 16.
+template <int K, int TN, class TeamT, int B = 24>
+__device__ __forceinline__ void team_reduce_vec(const double* partials, int nblocks, LeaderSmem& sm, int tid,
+                                                const P2PLine* lines = nullptr, unsigned tag = 0u, int* timeout_flag = nullptr) {
     constexpr int PARTS = TN / 32 - 1;
     static_assert(PARTS >= 1 && PARTS <= 16 && K <= 32, "LeaderSmem::part is [16][32]");
     const int q = tid & 31, part = tid >> 5;
@@ -1360,12 +1415,16 @@ __device__ __forceinline__ void team_reduce_vec(const double* partials, int nblo
         const int per = (nblocks + PARTS - 1) / PARTS;
         const int b0 = part * per, b1 = min(nblocks, b0 + per);
         double s = 0.0;
-        for (int b = b0; b < b1; b += 24) {       // 24 loads in flight: one round trip for a slice of up to 24 blocks
-            double v[24];
+        for (int b = b0; b < b1; b += B) {
+            double v[B];
+            if (lines) {
+                if (!ll_poll_lines<B>(lines + (size_t)b * K + q, K, b1 - b, tag, v, timeout_flag)) sm.flags[6] = 1;
+            } else {
 #pragma unroll
-            for (int u = 0; u < 24; ++u) v[u] = (b + u < b1) ? __ldcg(partials + (size_t)(b + u) * K + q) : 0.0;
+                for (int u = 0; u < B; ++u) v[u] = (b + u < b1) ? __ldcg(partials + (size_t)(b + u) * K + q) : 0.0;
+            }
 #pragma unroll
-            for (int u = 0; u < 24; ++u) s += v[u];
+            for (int u = 0; u < B; ++u) s += v[u];
         }
         sm.part[part][q] = s;
     }
@@ -1620,6 +1679,7 @@ struct LioSolveArgs {
     // flb_state_reset_enqueue: the saved pair).  The leader copies both into state / state_prop first.
     const State18* init_x;
     const State18* init_xp;
+    P2PLine* lines;          // persistent kernel: the workers' sums as lines (null: `partials` after the arrival count)
 };
 
 // Warp-level publication of the pose packet (see "Pose packet" below): 8-byte units {word, flag}.
@@ -1646,10 +1706,11 @@ __device__ __forceinline__ void pkt_publish_warp(unsigned long long* pkt, const 
 //                      in the persistent kernel (pkt != nullptr), publication of the new pose
 //   lio_leader_finish: covariance update on the stopping pass; stores what later launches / the host need
 #define FLB_STAMP(k) do { if (fine && threadIdx.x == 0) fine[k] = global_ns(); } while (0)
-template <int NT>
+template <int NT, bool LL = false>      // LL: the persistent kernels (arrival by lines possible)
 __device__ __forceinline__ void lio_leader_solve(const LioSolveArgs& s, LeaderSmem& sm, LioCtrl& c, bool first,
                                                  unsigned long long* pkt, unsigned flag, int resident,
-                                                 unsigned long long* fine = nullptr, unsigned p2p_tag = 0u) {
+                                                 unsigned long long* fine = nullptr, unsigned p2p_tag = 0u,
+                                                 unsigned long long* arrived = nullptr) {
     constexpr int K = lio_packed(6);
     constexpr int NC = (int)(sizeof(LioCtrl) / sizeof(unsigned));
     using T = Team<NT, false>;
@@ -1662,7 +1723,8 @@ __device__ __forceinline__ void lio_leader_solve(const LioSolveArgs& s, LeaderSm
     const double pri = (first || resident) ? 0.0 : prior_prefetch(s.prior, tid);
     if (tid == 0) sm.flags[3] = (resident == 2) ? 1 : 0;
     FLB_STAMP(0);
-    team_reduce_vec<K, NT, T>(s.partials, s.nblocks, sm, tid);
+    team_reduce_vec<K, NT, T>(s.partials, s.nblocks, sm, tid, LL ? s.lines : nullptr, flag, s.timeout_flag);
+    if (arrived && tid == 0) *arrived = global_ns();                 // lines: the last one is in
     if (!first && !resident) prior_commit(sm, pri, tid);
     if (p2p_tag) p2p_exchange<K, T>(s.p2p, sm, p2p_tag, tid, s.timeout_flag);
     if (first && !resident) leader_prior<T>(sm, s.prior, tid);
@@ -1703,7 +1765,7 @@ __device__ __forceinline__ void lio_leader_solve(const LioSolveArgs& s, LeaderSm
             sm.flags[1] = ok ? 1 : 0;
         }
         __syncwarp();
-        if (pkt) pkt_publish_warp<NC>(pkt, sm.x, &c, flag, tid);
+        if (pkt && !sm.flags[6]) pkt_publish_warp<NC>(pkt, sm.x, &c, flag, tid);   // [6]: arrival watchdog tripped
     }
     __syncthreads();
     FLB_STAMP(3);
@@ -1795,6 +1857,7 @@ struct VioSolveArgs {
     int* timeout_flag;
     int prior_from_state;    // persistent kernel: state_propagat = state (a pending flb_state_set_prior_enqueue, laserMapping.cpp:1292)
     const unsigned long long* err_units;   // see VioArgs::err_units (null: read `errors`)
+    P2PLine* lines;          // see LioSolveArgs::lines
 };
 
 constexpr int kErrChunk = 2048;          // staging capacity of the kernel-per-pass finalize kernel (static shared memory)
@@ -1805,11 +1868,11 @@ constexpr int kVioDbg = 8 + 4 * 16;   // debug stamps per block (tracing only)
 // One VIO leader step (whole block, NT threads), in two halves like the LIO one.  Requires the 24
 // pose/bias doubles of sm.x / sm.xp and the control block `c` (shared memory); c.level is the pyramid
 // level of the pass just done.
-template <int NT>
+template <int NT, bool LL = false>      // LL: see lio_leader_solve
 __device__ __forceinline__ void vio_leader_solve(const VioSolveArgs& s, LeaderSmem& sm, VioCtrl& c, float* s_err, bool first,
                                                  unsigned long long* pkt, unsigned flag, int resident,
                                                  unsigned long long* fine = nullptr, unsigned p2p_tag = 0u, int err_buf = 0,
-                                                 int err_cap = kErrChunk, int pn_override = -1) {
+                                                 int err_cap = kErrChunk, int pn_override = -1, unsigned long long* arrived = nullptr) {
     constexpr int NC = (int)(sizeof(VioCtrl) / sizeof(unsigned));
     const int tid = threadIdx.x;
     const int pn_total = pn_override >= 0 ? pn_override : s.Pn_total;
@@ -1991,7 +2054,9 @@ __device__ __forceinline__ void vio_leader_solve(const VioSolveArgs& s, LeaderSm
         const double pri = (first || resident) ? 0.0 : prior_prefetch(s.prior, tid);
         if (first) store_state(s.old_state, &sm.x, tid, NT - kErrTeam, false);           // old_state = *state (:747)
         if (tid == 0) sm.flags[3] = (resident == 2) ? 1 : 0;
-        team_reduce_vec<kVioPacked, NT - kErrTeam, T>(s.partials, s.nblocks, sm, tid);
+        team_reduce_vec<kVioPacked, NT - kErrTeam, T, (NT >= 512 ? 16 : 24)>(s.partials, s.nblocks, sm, tid, LL ? s.lines : nullptr, flag,
+                                                                                s.timeout_flag);
+        if (arrived && tid == 0) *arrived = global_ns();             // lines: the last one is in
         FLB_STAMP(1);
         if (!first && !resident) prior_commit(sm, pri, tid);
         if (multi) p2p_exchange<kVioPacked, T>(s.p2p, sm, p2p_tag, tid, s.timeout_flag);
@@ -2015,7 +2080,7 @@ __device__ __forceinline__ void vio_leader_solve(const VioSolveArgs& s, LeaderSm
                 const int it1 = c.iteration + 1;
                 const bool done_p = conv_p || it1 >= s.prm.max_iteration;
                 const bool stop_p = !ok_p || (done_p && (level - 1 < 0 || s.prm.single_level));
-                const int spec = (pkt != nullptr && !stop_p) ? 1 : 0;
+                const int spec = (pkt != nullptr && !stop_p && !sm.flags[6]) ? 1 : 0;
                 sm.flags[4] = spec;
                 sm.flags[5] = 0;
                 if (spec) {
@@ -2086,7 +2151,7 @@ __device__ __forceinline__ void vio_leader_solve(const VioSolveArgs& s, LeaderSm
                 if (tid < 24) reinterpret_cast<double*>(&sm.x)[tid] = __ldcg(reinterpret_cast<const double*>(s.old_state) + tid);
             }                                                                              // *state = old_state (:890)
             __syncwarp();
-            if (pkt && !spec) pkt_publish_warp<NC>(pkt, sm.x, &c, flag, tid);
+            if (pkt && !spec && !sm.flags[6]) pkt_publish_warp<NC>(pkt, sm.x, &c, flag, tid);
             FLB_STAMP(6);
         }
     }
@@ -2210,9 +2275,9 @@ __global__ void k_vio_begin_batched(VioCtrl* const* ctrls, int B, int Pn_total) 
 // Persistent (one launch per update) kernels
 // =======================================================================================
 // All blocks are co-resident (cooperative launch, grid <= SMs x occupancy).  LIO / VIO: worker blocks + one
-// dedicated leader block; a pass ends when every worker has arrived (red.release on a counter the leader
-// acquire-polls), the leader runs the leader step above with its whole block and publishes the pose packet
-// (below).  No host round trip, no empty launch.  Same pass and leader code as the kernel-per-pass path; the two
+// dedicated leader block; a pass ends when every worker has arrived (its sums stored as tagged lines the leader
+// polls, or -- counter path -- red.release on a counter the leader acquire-polls), the leader runs the leader step
+// above with its whole block and publishes the pose packet (below).  No host round trip, no empty launch.  Same pass and leader code as the kernel-per-pass path; the two
 // group a pass's partial sums by different block sizes, so their states agree to rounding, not bit for bit.
 // The IKFoM kernel still uses the classic form below (grid_arrive / grid_release / grid_wait: the last
 // arriver becomes the leader and re-opens a generation barrier).
@@ -2353,14 +2418,24 @@ template <int NT>
 __device__ __forceinline__ int leader_prepare(LeaderSmem& sm, const State18* state, PriorBlock* prior_g) {
     const int tid = threadIdx.x;
     load_cov_l2<NT>(&sm.x, state, tid);
-    if (tid == 0) sm.flags[3] = 0;
+    if (tid == 0) { sm.flags[3] = 0; sm.flags[6] = 0; }
     __syncthreads();
     leader_prior<Team<NT, false>>(sm, prior_g, tid);
     __syncthreads();
     return sm.flags[3] ? 2 : 1;
 }
 
-// Workers: arrive (release) without waiting for the ticket.
+// ---------------------------------------------------------------------------------------
+// Arrival by lines
+// ---------------------------------------------------------------------------------------
+// A worker block arrives by storing its K sums of the pass as lines tagged with the pass flag (epoch + pass + 1,
+// never 0, never reused while the line buffer lives: see next_epoch); the leader's reduce team polls those lines
+// directly (team_reduce_vec).  No release fence, no counter round trip in front of the loads, no trailing
+// __syncthreads.  This needs every other worker output the leader reads in the pass to be self-validating too:
+// the VIO per-patch errors go out as tagged units (single GPU: err_units; fused multi-GPU: the mailboxes).  With
+// plain per-patch errors (FLB_DEFER=0) only the counter's release / acquire orders them, so that case, and
+// FLB_LL_ARRIVE=0 (A/B measurement), keep the counter path below.
+// Workers (counter path): arrive (release) without waiting for the ticket.
 __device__ __forceinline__ void grid_arrive_release(GridBarrier* b) {
     __syncthreads();
     if (threadIdx.x == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(&b->count) : "memory");
@@ -2371,13 +2446,25 @@ __device__ __forceinline__ bool leader_wait_arrivals(GridBarrier* b, unsigned ta
         unsigned ok = 1u;
         unsigned long long spins = 0;
         while (ld_acquire_u32(&b->count) != target) {
-            if (++spins > 40000000ull) { ok = 0u; b->timeout = 1; break; }
+            if (++spins > kArriveSpinLimit) { ok = 0u; b->timeout = 1; break; }
             if ((spins & 0xffff) == 0 && *((volatile int*)&b->timeout)) { ok = 0u; break; }
         }
         s_scratch[1] = ok;
     }
     __syncthreads();
     return s_scratch[1] != 0u;
+}
+// Leader block, arrival by lines: wait until every worker has stored its lines of the pass tagged `tag`, without
+// their values (a discarded pass).  Line 0 of a block suffices: the block stores it after taking the previous packet.
+// False when the watchdog tripped.
+__device__ __forceinline__ bool leader_wait_lines(const P2PLine* lines, int nworkers, int K, unsigned tag, int* timeout_flag,
+                                                  LeaderSmem& sm) {
+    for (int b = threadIdx.x; b < nworkers; b += blockDim.x) {
+        double v[1];
+        if (!ll_poll_lines<1>(lines + (size_t)b * K, K, 1, tag, v, timeout_flag)) sm.flags[6] = 1;
+    }
+    __syncthreads();
+    return !sm.flags[6];
 }
 
 // ---------------------------------------------------------------------------------------
@@ -2393,6 +2480,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_lio_update_persistent(LioArgs a, L
                                                                  unsigned long long* trace, unsigned long long* dbg) {
     constexpr int K = lio_packed(6);
     constexpr int NC = (int)(sizeof(LioCtrl) / sizeof(unsigned));
+    P2PLine* const lines = s.lines;   // arrival by lines; null: counter path
     __shared__ LioPose s_pose;
     __shared__ double s_acc[BLOCK / 32][K];
     __shared__ unsigned s_bar[2];
@@ -2450,15 +2538,20 @@ __global__ void __launch_bounds__(BLOCK, 1) k_lio_update_persistent(LioArgs a, L
     for (;;) {
         const unsigned flag = epoch + (unsigned)pass_no + 1u;
         if (is_leader) {
-            if (!leader_wait_arrivals(bar, (unsigned)nworkers * (unsigned)(pass_no + 1), s_bar)) return;
-            if (trace && tid == 0 && 2 + 2 * pass_no < kTraceLen) trace[1 + 2 * pass_no] = global_ns();
+            // arrival stamp: when the count is complete, or (lines) when the reduce has every line of the pass
+            unsigned long long* arrived = (trace && 2 + 2 * pass_no < kTraceLen) ? trace + 1 + 2 * pass_no : nullptr;
+            if (!lines) {
+                if (!leader_wait_arrivals(bar, (unsigned)nworkers * (unsigned)(pass_no + 1), s_bar)) return;
+                if (arrived && tid == 0) *arrived = global_ns();
+            }
             unsigned long long* fine = (trace && 64 + 8 * pass_no + 8 <= kTraceLen) ? trace + 64 + 8 * pass_no : nullptr;
             const unsigned p2p_tag = multi ? ((unsigned)(s_seq_base + (unsigned long long)pass_no + 1ull) | 0x80000000u) : 0u;
-            lio_leader_solve<BLOCK>(s, sm, s_ctrl, first, pkt, flag, resident, fine, p2p_tag);
+            lio_leader_solve<BLOCK, true>(s, sm, s_ctrl, first, pkt, flag, resident, fine, p2p_tag, lines ? arrived : nullptr);
+            if (sm.flags[6]) return;         // the lines' watchdog tripped: nothing was published
             if (trace && tid == 0 && 2 + 2 * pass_no < kTraceLen) trace[2 + 2 * pass_no] = global_ns();
             lio_leader_finish<BLOCK>(s, sm, s_ctrl, first, false, resident, fine);
             if (s_ctrl.stop && tid == 0) {
-                bar->count = 0;
+                if (!lines) bar->count = 0;
                 if (multi) *s.p2p.seq = s_seq_base + (unsigned long long)pass_no + 1ull;
             }
         } else {
@@ -2484,9 +2577,9 @@ __global__ void __launch_bounds__(BLOCK, 1) k_lio_update_persistent(LioArgs a, L
                 }
             }
             if (dbg && (tid & 31) == 0) dbg[blockIdx.x * 16 + 4 + (tid >> 5)] = global_ns();   // per warp: compute done
-            block_reduce_store<K, BLOCK>(acc, s_acc, a.partials);
+            block_reduce_store<K, BLOCK>(acc, s_acc, a.partials, lines, flag);
             if (dbg && tid == 0) dbg[blockIdx.x * 16 + 2] = global_ns();
-            grid_arrive_release(bar);
+            if (!lines) grid_arrive_release(bar);
             if (dbg && tid == 0) dbg[blockIdx.x * 16 + 3] = global_ns();
             if (!pkt_wait<NC>(pkt, sm.x, &s_ctrl, flag, bar, s_bar, multi ? 40000000ull : 3000000ull)) return;
         }
@@ -2505,6 +2598,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_vio_update_persistent(VioArgs a, V
                                                                     unsigned long long* trace, unsigned long long* dbg, int err_cap) {
     constexpr int NW = BLOCK / 32;
     constexpr int NC = (int)(sizeof(VioCtrl) / sizeof(unsigned));
+    P2PLine* const lines = s.lines;   // arrival by lines (needs self-validating errors: err_units or fused); null: counter path
     __shared__ VioPose s_pose;
     __shared__ float s_lat[NW][128];
     __shared__ double s_res[NW][64];
@@ -2569,10 +2663,15 @@ __global__ void __launch_bounds__(BLOCK, 1) k_vio_update_persistent(VioArgs a, V
         const unsigned flag = epoch + (unsigned)pass_no + 1u;
         const unsigned p2p_tag = multi ? ((unsigned)(s_seq_base + (unsigned long long)pass_no + 1ull) | 0x80000000u) : 0u;
         if (is_leader) {
-            if (!leader_wait_arrivals(bar, (unsigned)nworkers * (unsigned)(pass_no + 1), s_bar)) return;
-            if (trace && tid == 0 && 2 + 2 * pass_no < kTraceLen) trace[1 + 2 * pass_no] = global_ns();
+            unsigned long long* arrived = (trace && 2 + 2 * pass_no < kTraceLen) ? trace + 1 + 2 * pass_no : nullptr;
+            if (!lines) {
+                if (!leader_wait_arrivals(bar, (unsigned)nworkers * (unsigned)(pass_no + 1), s_bar)) return;
+                if (arrived && tid == 0) *arrived = global_ns();
+            }
             unsigned long long* fine = (trace && 32 + 8 * pass_no + 8 <= kTraceLen) ? trace + 32 + 8 * pass_no : nullptr;
-            vio_leader_solve<BLOCK>(s, sm, s_ctrl, s_err, first, pkt, flag, resident, fine, p2p_tag, pass_no & 1, err_cap, Pn);
+            vio_leader_solve<BLOCK, true>(s, sm, s_ctrl, s_err, first, pkt, flag, resident, fine, p2p_tag, pass_no & 1, err_cap, Pn,
+                                    lines ? arrived : nullptr);
+            if (sm.flags[6]) return;         // the lines' watchdog tripped: nothing was published
             if (trace && tid == 0 && 2 + 2 * pass_no < kTraceLen) trace[2 + 2 * pass_no] = global_ns();
             vio_leader_finish<BLOCK>(s, sm, s_ctrl, first, false, resident);
             if (sm.flags[5]) {
@@ -2581,7 +2680,11 @@ __global__ void __launch_bounds__(BLOCK, 1) k_vio_update_persistent(VioArgs a, V
                 // continuation (the rejected step's old_state at the next level, or stop).  Fused multi-GPU mode:
                 // every rank mispredicts identically; one (payload-free) exchange keeps the mailbox parity rule.
                 ++pass_no;
-                if (!leader_wait_arrivals(bar, (unsigned)nworkers * (unsigned)(pass_no + 1), s_bar)) return;
+                if (lines) {
+                    if (!leader_wait_lines(lines, nworkers, kVioPacked, epoch + (unsigned)pass_no + 1u, s.timeout_flag, sm)) return;
+                } else if (!leader_wait_arrivals(bar, (unsigned)nworkers * (unsigned)(pass_no + 1), s_bar)) {
+                    return;
+                }
                 if (trace && tid == 0 && 2 + 2 * pass_no < kTraceLen) trace[1 + 2 * pass_no] = global_ns();
                 if (multi) {
                     const unsigned tag2 = (unsigned)(s_seq_base + (unsigned long long)pass_no + 1ull) | 0x80000000u;
@@ -2592,7 +2695,7 @@ __global__ void __launch_bounds__(BLOCK, 1) k_vio_update_persistent(VioArgs a, V
                 __syncthreads();
             }
             if (s_ctrl.stop && tid == 0) {
-                bar->count = 0;
+                if (!lines) bar->count = 0;
                 if (multi) *s.p2p.seq = s_seq_base + (unsigned long long)pass_no + 1ull;
             }
         } else {
@@ -2619,9 +2722,9 @@ __global__ void __launch_bounds__(BLOCK, 1) k_vio_update_persistent(VioArgs a, V
                               &pend_tiny))
                     pend_i = i;
             }
-            vio_block_reduce_store<BLOCK>(accv, n_meas, skipped, s_acc, a.partials);
+            vio_block_reduce_store<BLOCK>(accv, n_meas, skipped, s_acc, a.partials, lines, flag);
             if (dbg && tid == 0) dbg[blockIdx.x * kVioDbg + 2] = global_ns();
-            grid_arrive_release(bar);
+            if (!lines) grid_arrive_release(bar);
             if (dbg && tid == 0) dbg[blockIdx.x * kVioDbg + 3] = global_ns();
             if (pend_i >= 0) vio_patch_error(a, pend_i, s_res[warp], pend_tiny, p2p_tag, utag, pass_no & 1, wd);
             if (!pkt_wait<NC>(pkt, sm.x, &s_ctrl, flag, bar, s_bar, multi ? 40000000ull : 3000000ull)) return;
