@@ -172,7 +172,7 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_imu_undistort", "flb_visual_candidates", "flb_vio_errors",
            "flb_vio_update_level", "flb_state_download_enqueue", "flb_state_download_wait", "flb_frame_enqueue",
            "flb_vmap_reset", "flb_vmap_select", "flb_vmap_selected", "flb_vmap_grow", "flb_vmap_add_observations", "flb_vmap_counts",
-           "flb_vmap_map_value", "flb_vmap_dump", "flb_colorize", "flb_voxel_grid",
+           "flb_vmap_map_value", "flb_vmap_dump", "flb_vmap_reclaim", "flb_vmap_usage", "flb_vmap_keyframe", "flb_colorize", "flb_voxel_grid",
            "flb_batch_begin", "flb_batch_set_frame", "flb_batch_state_reset_enqueue", "flb_batch_update_enqueue", "flb_batch_state_download",
            "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
            "flb_map_grid_info", "flb_debug_set_map_index"]
@@ -253,6 +253,9 @@ def lib():
         L.flb_vmap_counts.argtypes = [vp] + [C.POINTER(C.c_int)] * 5
         L.flb_vmap_map_value.argtypes = [vp, vp, C.c_int]
         L.flb_vmap_dump.argtypes = [vp, C.c_int, C.c_int] + [vp] * 7
+        L.flb_vmap_reclaim.argtypes = [vp]
+        L.flb_vmap_usage.argtypes = [vp] + [C.POINTER(C.c_int)] * 7 + [C.POINTER(C.c_int64)]
+        L.flb_vmap_keyframe.argtypes = [vp, C.c_int, vp, C.c_int]
         L.flb_vio_update.argtypes = [vp, C.POINTER(VioParams), C.POINTER(State18), C.POINTER(State18), C.POINTER(VioReport)]
         L.flb_state_upload.argtypes = [vp, C.POINTER(State18), C.POINTER(State18)]
         L.flb_state_download.argtypes = [vp, C.POINTER(State18), C.POINTER(LioReport), C.POINTER(VioReport)]
@@ -414,6 +417,7 @@ class Handle:
         c.fx, c.fy, c.cx, c.cy = cam["fx"], cam["fy"], cam["cx"], cam["cy"]
         c.d[:] = cam["d"]
         self._ck(self.L.flb_camera_set(self.h, C.byref(c)))
+        self._cam_wh = (int(cam["width"]), int(cam["height"]))
 
     def load_frame(self, frame):
         """Upload everything a synthetic frame holds."""
@@ -616,6 +620,25 @@ class Handle:
         self._ck(self.L.flb_vmap_dump(self.h, n, m, _p(d["pos"]), _p(d["value"]), _p(d["n_obs"]), _p(d["obs"]), _p(d["ft_geo"]),
                                       _p(d["ft_score"]), _p(d["ft_level_id_img"])))
         return d
+
+    def vmap_reclaim(self):
+        """flb_vmap_reclaim (enqueue-only): drop evicted features, put unreferenced keyframe slots on the free-slot stack."""
+        self._ck(self.L.flb_vmap_reclaim(self.h))
+
+    def vmap_usage(self):
+        """flb_vmap_usage (blocking): the visual map's sizes, capacities and device bytes."""
+        v = [C.c_int() for _ in range(7)]
+        b = C.c_int64()
+        self._ck(self.L.flb_vmap_usage(self.h, *[C.byref(x) for x in v], C.byref(b)))
+        keys = ("points", "features", "dead_features", "feature_capacity", "slots_in_use", "free_slots", "pool_slots")
+        return dict(zip(keys, (x.value for x in v)), device_bytes=b.value)
+
+    def vmap_keyframe(self, slot):
+        """flb_vmap_keyframe: the keyframe image in pool slot `slot` (height, width) uint8."""
+        w, hgt = self._cam_wh
+        out = np.zeros((hgt, w), np.uint8)
+        self._ck(self.L.flb_vmap_keyframe(self.h, int(slot), _p(out), out.size))
+        return out
 
     # ---- IMU propagation + undistortion (row f3)
     def imu_undistort(self, prm: ImuParams, carry: ImuCarry, v_imu, pcl_beg_time, pcl_end_time, pts, offset_index=3):

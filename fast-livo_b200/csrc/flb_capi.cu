@@ -281,7 +281,13 @@ struct flb_handle {
         DevBuf<VmFeature> fts;
         DevBuf<unsigned char> pool;          // keyframe images, pool_slots x (w * h)
         int pool_slots = 0;
-        int pts_ub = 0, fts_ub = 0, img_ub = 0;   // host-side upper bounds of the device counters
+        int pts_ub = 0, fts_ub = 0, img_ub = 0;   // host-side upper bounds of the device counters (img_ub: slots in use)
+        // flb_vmap_reclaim (allocated by its first call): the compaction target (swapped with fts), the free-slot stack of
+        // the pool, scratch for the feature ranks (fts.cap + 1) and the slot flags / ranks (3 x pool_slots), cub's scan scratch
+        DevBuf<VmFeature> fts_alt;
+        DevBuf<int> free_slots, rc_rank, rc_slot;
+        DevBuf<unsigned char> rc_cub;
+        size_t rc_cub_bytes = 0;
         DevBuf<int> counters;
         DevBuf<double> pose, rci;            // T_f_w of the current frame (12) ; Rci | Pci (12)
         DevBuf<float> pg;                    // scan points of the current call
@@ -978,6 +984,7 @@ int flb_destroy(flb_handle* h) {
         vm.cell_err.release(); vm.cell_patch.release(); vm.sel_error.release(); vm.cell_flag.release(); vm.cell_rank.release();
         vm.cell_level.release(); vm.cell_point.release(); vm.sel_index.release(); vm.sel_point.release(); vm.winner.release();
         vm.scan_tmp.release(); vm.st_pg.release();
+        vm.fts_alt.release(); vm.free_slots.release(); vm.rc_rank.release(); vm.rc_slot.release(); vm.rc_cub.release();
     }
     for (auto& ev : h->evs) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
     h->map_raw.release(); h->keys.release(); h->keys_sorted.release(); h->vals.release(); h->vals_sorted.release();
@@ -3037,18 +3044,40 @@ int vm_grow_buf(flb_handle* h, DevBuf<T>& b, size_t used_ub, size_t need) {
     return FLB_OK;
 }
 
+// flb_vmap_reclaim's buffers shadow the feature array and the pool.  The first reclaim allocates them; afterwards
+// vm_ensure_capacity grows them together with those arrays (it has synchronised by then), so a reclaim neither frees
+// memory nor waits for the device.  Nothing in them outlives a reclaim except the free-slot stack, and the pool only
+// grows when every slot is in use, i.e. with that stack empty: none of them needs its contents copied.
+int vm_reclaim_reserve(flb_handle* h) {
+    auto& vm = h->vm;
+    const size_t slots = (size_t)std::max(vm.pool_slots, 1);
+    FLB_CUDA(h, vm.fts_alt.reserve(vm.fts.cap));
+    FLB_CUDA(h, vm.rc_rank.reserve(vm.fts.cap + 1));
+    FLB_CUDA(h, vm.free_slots.reserve(slots));
+    FLB_CUDA(h, vm.rc_slot.reserve(3 * slots));
+    size_t bytes = 0;                        // the scan's scratch only grows with its length: size it for the largest one
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, bytes, vm.rc_rank.p, vm.rc_rank.p, (int)(vm.fts.cap + 1), h->stream));
+    FLB_CUDA(h, vm.rc_cub.reserve(std::max<size_t>(bytes, 1)));
+    vm.rc_cub_bytes = std::max(vm.rc_cub_bytes, bytes);
+    return FLB_OK;
+}
+
 // Make room for `add_p` more points, `add_f` more features and one more keyframe image.  The host only keeps upper
 // bounds of the device counters; when a bound hits the capacity it is refreshed from the device before anything grows.
+// The image bound counts slots in use: after a reclaim, slots on the free-slot stack are room, and the pool grows only
+// when none is left (then the slots in use are exactly the pool's tail).
 int vm_ensure_capacity(flb_handle* h, int add_p, int add_f) {
     auto& vm = h->vm;
     const size_t img_bytes = (size_t)h->img_w * h->img_h;
+    const size_t fts_cap = vm.fts.cap;
+    const int pool_slots = vm.pool_slots;
     if ((size_t)(vm.pts_ub + add_p) > vm.pts.cap || (size_t)(vm.fts_ub + add_f) > vm.fts.cap || vm.img_ub + 1 > vm.pool_slots) {
         int c[VM_COUNTERS];
         FLB_CUDA(h, cudaMemcpyAsync(c, vm.counters.p, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
         FLB_CUDA(h, cudaStreamSynchronize(h->stream));
         vm.pts_ub = c[VM_N_POINTS];
         vm.fts_ub = c[VM_N_FEATS];
-        vm.img_ub = c[VM_N_IMAGES];
+        vm.img_ub = c[VM_N_IMAGES] - c[VM_N_FREE];
     }
     { int rc = vm_grow_buf(h, vm.pts, (size_t)vm.pts_ub, (size_t)(vm.pts_ub + add_p)); if (rc) return rc; }
     { int rc = vm_grow_buf(h, vm.fts, (size_t)vm.fts_ub, (size_t)(vm.fts_ub + add_f)); if (rc) return rc; }
@@ -3062,6 +3091,7 @@ int vm_ensure_capacity(flb_handle* h, int add_p, int add_f) {
         vm.pool = nb;
         vm.pool_slots = slots;
     }
+    if (vm.fts_alt.p && (vm.fts.cap != fts_cap || vm.pool_slots != pool_slots)) return vm_reclaim_reserve(h);
     return FLB_OK;
 }
 
@@ -3219,14 +3249,14 @@ int flb_vmap_grow(flb_handle* h, const double Rcw[9], const double Pcw[3], const
     const size_t img_bytes = (size_t)h->img_w * h->img_h;
     {
         LaunchScope ls(h, FAM_OTHER);
-        k_vm_store_image<<<h->num_sms, 256, 0, h->stream>>>(h->img.p, img_bytes, vm.pool.p, vm.counters.p, frame_id);
+        k_vm_store_image<<<h->num_sms, 256, 0, h->stream>>>(h->img.p, img_bytes, vm.pool.p, vm.counters.p, vm.free_slots.p, frame_id);
         k_vmap_seed<<<(L + 255) / 256, 256, 0, h->stream>>>(vm.map_value.p, L, vm.cand_key.p);
         if (n > 0)
             k_vmap_candidates<<<(n + 127) / 128, 128, 0, h->stream>>>(h->cam, vm.pose.p, h->img.p, vm.pg.p, n, vm.prm.grid_size, vm.prm.grid_n_height,
                                                                       border, vm.cand_key.p);
         k_vmap_resolve<<<(L + 255) / 256, 256, 0, h->stream>>>(vm.cand_key.p, L, vm.map_value.p, vm.winner.p);
         k_vm_materialise<<<1, 1024, 0, h->stream>>>(h->cam, L, vm.pose.p, vm.pg.p, vm.winner.p, vm.map_value.p, vm.scan_tmp.p, vm.pts.p, vm.fts.p,
-                                                    vm.counters.p, frame_id, (int)vm.pts.cap, (int)vm.fts.cap);
+                                                    vm.counters.p, vm.free_slots.p, frame_id, (int)vm.pts.cap, (int)vm.fts.cap);
         FLB_CUDA(h, cudaGetLastError());
         h->launches += 4;
     }
@@ -3248,9 +3278,9 @@ int flb_vmap_add_observations(flb_handle* h, const double Rcw[9], const double P
     const size_t img_bytes = (size_t)h->img_w * h->img_h;
     {
         LaunchScope ls(h, FAM_OTHER);
-        k_vm_store_image<<<h->num_sms, 256, 0, h->stream>>>(h->img.p, img_bytes, vm.pool.p, vm.counters.p, frame_id);
+        k_vm_store_image<<<h->num_sms, 256, 0, h->stream>>>(h->img.p, img_bytes, vm.pool.p, vm.counters.p, vm.free_slots.p, frame_id);
         k_vm_observe<<<1, 1024, 0, h->stream>>>(h->cam, vm.pose.p, h->img.p, vm.sel_point.p, h->patch_level.p, vm.scan_tmp.p, L, vm.pts.p,
-                                                vm.fts.p, vm.counters.p, frame_id, (int)vm.fts.cap);
+                                                vm.fts.p, vm.counters.p, vm.free_slots.p, frame_id, (int)vm.fts.cap);
         FLB_CUDA(h, cudaGetLastError());
         h->launches += 1;
     }
@@ -3306,10 +3336,10 @@ int flb_vmap_counts(flb_handle* h, int* points, int* features, int* images, int*
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
     h->vm.pts_ub = c[VM_N_POINTS];
     h->vm.fts_ub = c[VM_N_FEATS];
-    h->vm.img_ub = c[VM_N_IMAGES];
+    h->vm.img_ub = c[VM_N_IMAGES] - c[VM_N_FREE];
     if (points) *points = c[VM_N_POINTS];
     if (features) *features = c[VM_N_FEATS];
-    if (images) *images = c[VM_N_IMAGES];
+    if (images) *images = c[VM_N_IMAGES] - c[VM_N_FREE];
     if (selected) *selected = c[VM_N_SEL];
     if (last_added) *last_added = c[VM_LAST_ADDED];
     if (c[VM_LAST_ADDED] < 0) return fail(h, FLB_ERR_STATE, "visual map: an append did not fit its buffers (internal capacity bound violated)");
@@ -3354,6 +3384,89 @@ int flb_vmap_dump(flb_handle* h, int cap_points, int cap_features, double* pos, 
         if (ft_score) ft_score[j] = F[j].score;
         if (ft_level_id_img) { ft_level_id_img[3 * (size_t)j] = F[j].level; ft_level_id_img[3 * (size_t)j + 1] = F[j].id; ft_level_id_img[3 * (size_t)j + 2] = F[j].img; }
     }
+    return FLB_OK;
+}
+
+int flb_vmap_reclaim(flb_handle* h) {
+    FLB_CHECK_H(h);
+    if (!h->vm.on) return fail(h, FLB_ERR_STATE, "flb_vmap_reclaim: flb_vmap_reset first");
+    auto& vm = h->vm;
+    { int rc = vm_reclaim_reserve(h); if (rc) return rc; }
+    // The host bounds size the grids and the scan; the kernels stop at the device counts.  Features between the device
+    // count and the bound are never named, so their flags stay 0 and rank[M] is the number of live features.
+    const int M = vm.fts_ub;
+    const size_t point_words = (size_t)std::max(vm.pts_ub, 1) * kVmPointWords, feat_words = (size_t)std::max(M, 1) * kVmFeatWords;
+    auto blocks = [h](size_t words) { return (int)std::min<size_t>((words + 255) / 256, (size_t)h->num_sms * 8); };
+    cudaStream_t s = h->stream;
+    FLB_CUDA(h, cudaMemsetAsync(vm.rc_rank.p, 0, (size_t)(M + 1) * sizeof(int), s));
+    FLB_CUDA(h, cudaMemsetAsync(vm.rc_slot.p, 0, (size_t)vm.pool_slots * sizeof(int), s));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_vm_rc_mark<<<blocks(point_words), 256, 0, s>>>(vm.pts.p, vm.counters.p, vm.rc_rank.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    size_t bytes = vm.rc_cub_bytes;
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(vm.rc_cub.p, bytes, vm.rc_rank.p, vm.rc_rank.p, M + 1, s));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_vm_rc_compact<<<blocks(feat_words), 256, 0, s>>>(vm.fts.p, vm.fts_alt.p, vm.rc_rank.p, vm.counters.p, vm.rc_slot.p);
+        k_vm_rc_remap<<<blocks(point_words), 256, 0, s>>>(vm.pts.p, vm.rc_rank.p, vm.counters.p);
+        k_vm_rc_slots<<<1, 1024, 0, s>>>(vm.counters.p, vm.rc_rank.p + M, vm.rc_slot.p, std::max(vm.pool_slots, 1), vm.free_slots.p);
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches += 4;                   // + the scan's two kernels
+    }
+    std::swap(vm.fts, vm.fts_alt);
+    return FLB_OK;
+}
+
+int flb_vmap_usage(flb_handle* h, int* points, int* features, int* dead_features, int* feature_capacity, int* slots_in_use, int* free_slots,
+                   int* pool_slots, int64_t* device_bytes) {
+    FLB_CHECK_H(h);
+    if (!h->vm.on) return fail(h, FLB_ERR_STATE, "flb_vmap_usage: flb_vmap_reset first");
+    auto& vm = h->vm;
+    int c[VM_COUNTERS];
+    FLB_CUDA(h, cudaMemcpyAsync(c, vm.counters.p, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    vm.pts_ub = c[VM_N_POINTS];
+    vm.fts_ub = c[VM_N_FEATS];
+    vm.img_ub = c[VM_N_IMAGES] - c[VM_N_FREE];
+    if (dead_features) {
+        std::vector<VmPoint> P((size_t)c[VM_N_POINTS]);
+        if (!P.empty()) FLB_CUDA(h, cudaMemcpy(P.data(), vm.pts.p, P.size() * sizeof(VmPoint), cudaMemcpyDeviceToHost));
+        std::vector<unsigned char> named((size_t)c[VM_N_FEATS], 0);
+        for (const VmPoint& p : P)
+            for (int q = 0; q < p.n_obs; ++q) named[p.obs[q]] = 1;
+        *dead_features = c[VM_N_FEATS] - (int)std::count(named.begin(), named.end(), 1);
+    }
+    if (points) *points = c[VM_N_POINTS];
+    if (features) *features = c[VM_N_FEATS];
+    if (feature_capacity) *feature_capacity = (int)vm.fts.cap;
+    if (slots_in_use) *slots_in_use = c[VM_N_IMAGES] - c[VM_N_FREE];
+    if (free_slots) *free_slots = c[VM_N_FREE];
+    if (pool_slots) *pool_slots = vm.pool_slots;
+    if (device_bytes) {
+        int64_t b = 0;
+        auto add = [&b](const auto& buf) { b += (int64_t)(buf.cap * sizeof(*buf.p)); };
+        add(vm.pts); add(vm.fts); add(vm.fts_alt); add(vm.pool); add(vm.counters); add(vm.pose); add(vm.rci); add(vm.pg);
+        add(vm.depth); add(vm.keyset); add(vm.cell_best); add(vm.cand_key); add(vm.cell_type); add(vm.map_value); add(vm.cell_err);
+        add(vm.cell_patch); add(vm.sel_error); add(vm.cell_flag); add(vm.cell_rank); add(vm.cell_level); add(vm.cell_point);
+        add(vm.sel_index); add(vm.sel_point); add(vm.winner); add(vm.scan_tmp); add(vm.free_slots); add(vm.rc_rank); add(vm.rc_slot);
+        add(vm.rc_cub);
+        *device_bytes = b;
+    }
+    return FLB_OK;
+}
+
+int flb_vmap_keyframe(flb_handle* h, int slot, uint8_t* gray, int capacity) {
+    FLB_CHECK_H(h);
+    if (!h->vm.on) return fail(h, FLB_ERR_STATE, "flb_vmap_keyframe: flb_vmap_reset first");
+    const size_t img_bytes = (size_t)h->img_w * h->img_h;
+    if (!gray || capacity < 0 || (size_t)capacity < img_bytes) return fail(h, FLB_ERR_INVALID, "flb_vmap_keyframe: bad arguments");
+    int tail = 0;
+    FLB_CUDA(h, cudaMemcpyAsync(&tail, h->vm.counters.p + VM_N_IMAGES, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (slot < 0 || slot >= tail) return fail(h, FLB_ERR_INVALID, "flb_vmap_keyframe: slot %d outside the pool's %d slots", slot, tail);
+    FLB_CUDA(h, cudaMemcpy(gray, h->vm.pool.p + (size_t)slot * img_bytes, img_bytes, cudaMemcpyDeviceToHost));
     return FLB_OK;
 }
 

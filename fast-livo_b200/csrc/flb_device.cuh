@@ -11,6 +11,7 @@
 #pragma once
 
 #include <math.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <string.h>
 #if !defined(__CUDACC__)
@@ -1112,6 +1113,31 @@ struct VmPoint {
     int obs[kVmMaxObs + 1];              // obs[0] = newest (addFrameRef: push_front)
     int pad;
 };
+// Reclaim (flb_vmap_reclaim).  The reference's Feature is owned by Point::obs_ alone and its keyframe image by the
+// Features that point to it (src/lidar_selection.cpp:183, :946-957), so both die with their last reference.  The device
+// map restates that lifetime in one pass: a feature is live iff some point's obs[0..n_obs) names it; live features
+// move to their rank among live features (creation order kept); an image slot is live iff a live feature names it.
+// The point array is read as 32-bit words, one word per thread, so the passes over it are coalesced.
+constexpr int kVmPointWords = (int)(sizeof(VmPoint) / 4);
+constexpr int kVmNObsWord = (int)(offsetof(VmPoint, n_obs) / 4);
+constexpr int kVmObsWord = (int)(offsetof(VmPoint, obs) / 4);
+static_assert(sizeof(VmPoint) % 4 == 0, "VmPoint is read as 32-bit words");
+
+// The live test: the feature id that word k of a point names (obs[q] with q < n_obs), or -1.
+FLB_HD int vm_point_word_feature(const int* point_words, int k) {
+    const int q = k - kVmObsWord;
+    return (q >= 0 && q < point_words[kVmNObsWord]) ? point_words[k] : -1;
+}
+// rank = exclusive scan of the live flags over [0, n_features]: feature f is live iff its rank steps, and its new id is its
+// rank (rank[n_features] = live features).
+FLB_HD bool vm_feature_live(const int* rank, int f) { return rank[f + 1] != rank[f]; }
+FLB_HD int vm_feature_remap(const int* rank, int f) { return rank[f]; }
+// A slot goes onto the free-slot stack when no live feature names it and it is not the current frame's slot (pinned: a
+// reclaim between select and grow / add_observations of one frame must leave that frame's committed image alone).
+FLB_HD bool vm_slot_free(const int* slot_live, int pinned, int s) { return !slot_live[s] && s != pinned; }
+// The slot the next keyframe image goes to: the top of the free-slot stack when it holds any, else the pool's tail.
+FLB_HD int vm_image_slot(int n_free, const int* free_stack, int tail) { return n_free > 0 ? free_stack[n_free - 1] : tail; }
+
 struct VmParams {
     int grid_size, grid_n_width, grid_n_height, length;
     int halfpatch;                       // patch_size_half = 4

@@ -8,8 +8,11 @@
 //            then one new Point + Feature per won cell
 //   observe  LidarSelector::addObservation (:913-965): new observations of the selected points, oldest-view eviction
 //
-// The map is three flat arrays (VmPoint, VmFeature, keyframe images) that only ever grow at the tail, so ids are
-// stable and equal to the reference's creation order.  Every per-element function lives in flb_device.cuh and is
+//   reclaim  the lifetimes of Feature (owned by Point::obs_) and its keyframe image (owned by the Features, :183, :957):
+//            evicted features are compacted away, unreferenced image slots go onto a free-slot stack (opt-in)
+//
+// The map is three flat arrays (VmPoint, VmFeature, keyframe images) that grow at the tail, so ids are creation order;
+// a reclaim keeps live features in that order and reuses freed image slots in place.  Every per-element function lives in flb_device.cuh and is
 // checked bit for bit against the oracle on the CPU (tests/hostemu); the kernels below only distribute the work:
 // per-point kernels use 64-bit atomics whose winner is order-independent ({distance bits : ~index} minimum,
 // {index : depth bits} maximum), per-cell work is one warp per cell, appends are ordered by a block-wide scan.
@@ -20,8 +23,10 @@
 
 namespace flb {
 
-// counters (device-resident; mirrored on the host only when a caller asks)
-enum { VM_N_POINTS = 0, VM_N_FEATS = 1, VM_N_SEL = 2, VM_N_IMAGES = 3, VM_IMG_FRAME = 4, VM_IMG_SLOT = 5, VM_LAST_ADDED = 6, VM_COUNTERS = 8 };
+// counters (device-resident; mirrored on the host only when a caller asks).  VM_N_IMAGES is the pool's tail (slots ever
+// handed out), VM_N_FREE the depth of the free-slot stack: slots in use = VM_N_IMAGES - VM_N_FREE.
+enum { VM_N_POINTS = 0, VM_N_FEATS = 1, VM_N_SEL = 2, VM_N_IMAGES = 3, VM_IMG_FRAME = 4, VM_IMG_SLOT = 5, VM_LAST_ADDED = 6, VM_N_FREE = 7,
+       VM_COUNTERS = 8 };
 
 constexpr unsigned long long kVmEmpty = ~0ull;
 
@@ -234,11 +239,12 @@ __global__ void __launch_bounds__(256) k_vm_scatter(int length, const int* __res
 }
 
 // The keyframe image of the current frame goes into the next free pool slot unless this frame already has one.  The
-// slot only becomes part of the map when a feature referencing it is appended (k_vm_materialise / k_vm_observe).
+// slot only becomes part of the map when a feature referencing it is appended (k_vm_materialise / k_vm_observe); both
+// pick it with vm_image_slot from the same counters, in stream order.
 __global__ void k_vm_store_image(const unsigned char* __restrict__ img, size_t bytes, unsigned char* __restrict__ pool, const int* counters,
-                                 int frame_id) {
+                                 const int* __restrict__ free_slots, int frame_id) {
     if (counters[VM_IMG_FRAME] == frame_id && counters[VM_IMG_SLOT] >= 0) return;
-    unsigned char* dst = pool + (size_t)counters[VM_N_IMAGES] * bytes;
+    unsigned char* dst = pool + (size_t)vm_image_slot(counters[VM_N_FREE], free_slots, counters[VM_N_IMAGES]) * bytes;
     const size_t n16 = bytes / 16;
     const uint4* s4 = reinterpret_cast<const uint4*>(img);
     uint4* d4 = reinterpret_cast<uint4*>(dst);
@@ -247,10 +253,12 @@ __global__ void k_vm_store_image(const unsigned char* __restrict__ img, size_t b
     for (size_t e = n16 * 16 + i; e < bytes; e += stride) dst[e] = img[e];
 }
 
-__device__ __forceinline__ int vm_commit_image(int* counters, int frame_id) {     // thread 0 only
+__device__ __forceinline__ int vm_commit_image(int* counters, const int* free_slots, int frame_id) {     // thread 0 only
     if (!(counters[VM_IMG_FRAME] == frame_id && counters[VM_IMG_SLOT] >= 0)) {
-        counters[VM_IMG_SLOT] = counters[VM_N_IMAGES];
-        counters[VM_N_IMAGES] += 1;
+        const int n_free = counters[VM_N_FREE];
+        counters[VM_IMG_SLOT] = vm_image_slot(n_free, free_slots, counters[VM_N_IMAGES]);
+        if (n_free > 0) counters[VM_N_FREE] = n_free - 1;
+        else counters[VM_N_IMAGES] += 1;
         counters[VM_IMG_FRAME] = frame_id;
     }
     return counters[VM_IMG_SLOT];
@@ -270,7 +278,7 @@ __global__ void __launch_bounds__(1024) k_vm_materialise(CamModel cam, int lengt
                                                          const float* __restrict__ pg, const int* __restrict__ winner,
                                                          const float* __restrict__ map_value, int* __restrict__ rank_tmp,
                                                          VmPoint* __restrict__ pts, VmFeature* __restrict__ feats, int* counters,
-                                                         int frame_id, int pts_cap, int fts_cap) {
+                                                         const int* __restrict__ free_slots, int frame_id, int pts_cap, int fts_cap) {
     __shared__ int s_slot, s_base_p, s_base_f;
     // flags = winner >= 0 (rank_tmp doubles as the flag array first)
     for (int i = threadIdx.x; i < length; i += 1024) rank_tmp[length + i] = winner[i] >= 0 ? 1 : 0;
@@ -281,7 +289,7 @@ __global__ void __launch_bounds__(1024) k_vm_materialise(CamModel cam, int lengt
         s_base_p = counters[VM_N_POINTS];
         s_base_f = counters[VM_N_FEATS];
         const bool fits = s_base_p + total <= pts_cap && s_base_f + total <= fts_cap;
-        s_slot = (total > 0 && fits) ? vm_commit_image(counters, frame_id) : -1;
+        s_slot = (total > 0 && fits) ? vm_commit_image(counters, free_slots, frame_id) : -1;
         counters[VM_LAST_ADDED] = fits ? total : -1;
         if (fits) { counters[VM_N_POINTS] = s_base_p + total; counters[VM_N_FEATS] = s_base_f + total; }
     }
@@ -310,7 +318,8 @@ __global__ void __launch_bounds__(1024) k_vm_materialise(CamModel cam, int lengt
 __global__ void __launch_bounds__(1024) k_vm_observe(CamModel cam, const double* __restrict__ pose12, const unsigned char* __restrict__ img,
                                                      const int* __restrict__ sel_point, const int* __restrict__ patch_level,
                                                      int* __restrict__ flag_rank /* 2 x cap */, int cap, VmPoint* __restrict__ pts,
-                                                     VmFeature* __restrict__ feats, int* counters, int frame_id, int fts_cap) {
+                                                     VmFeature* __restrict__ feats, int* counters, const int* __restrict__ free_slots,
+                                                     int frame_id, int fts_cap) {
     __shared__ int s_slot, s_base_f;
     const int n = counters[VM_N_SEL];
     if (n <= 0) {
@@ -337,7 +346,7 @@ __global__ void __launch_bounds__(1024) k_vm_observe(CamModel cam, const double*
     if (threadIdx.x == 0) {
         s_base_f = counters[VM_N_FEATS];
         const bool fits = s_base_f + total <= fts_cap;
-        s_slot = (total > 0 && fits) ? vm_commit_image(counters, frame_id) : -1;
+        s_slot = (total > 0 && fits) ? vm_commit_image(counters, free_slots, frame_id) : -1;
         counters[VM_LAST_ADDED] = fits ? total : -1;
         if (fits) counters[VM_N_FEATS] = s_base_f + total;
     }
@@ -355,6 +364,69 @@ __global__ void __launch_bounds__(1024) k_vm_observe(CamModel cam, const double*
         for (int q = pt.n_obs; q > 0; --q) pt.obs[q] = pt.obs[q - 1];            // addFrameRef: push_front
         pt.obs[0] = fi;
         pt.n_obs++;
+    }
+}
+
+// ---- reclaim (flb_vmap_reclaim): mark -> exclusive scan of the marks (cub, in place) -> compact + remap -> free slots.
+// Kernels over the point array take one 32-bit word per thread and over the feature array one 64-bit word per thread,
+// so every pass reads (and the compaction writes) whole lines; grid-stride loops bounded by the device counts.
+constexpr int kVmFeatWords = (int)(sizeof(VmFeature) / 8);
+static_assert(sizeof(VmFeature) % 8 == 0, "VmFeature is copied as 64-bit words");
+
+// rank[f] = 1 for every feature some point's obs[0..n_obs) names (rank[] zeroed before)
+__global__ void __launch_bounds__(256) k_vm_rc_mark(const VmPoint* __restrict__ pts, const int* __restrict__ counters, int* __restrict__ rank) {
+    const int* words = reinterpret_cast<const int*>(pts);
+    const size_t n = (size_t)counters[VM_N_POINTS] * kVmPointWords;
+    for (size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x; w < n; w += (size_t)gridDim.x * blockDim.x) {
+        const size_t j = w / kVmPointWords;
+        const int f = vm_point_word_feature(words + j * kVmPointWords, (int)(w - j * kVmPointWords));
+        if (f >= 0) rank[f] = 1;
+    }
+}
+
+// live features -> dst[rank] (creation order kept; dst is the second feature buffer: an in-place move would race with
+// the live feature still sitting in the target slot); the image slots they name are marked live
+__global__ void __launch_bounds__(256) k_vm_rc_compact(const VmFeature* __restrict__ src, VmFeature* __restrict__ dst, const int* __restrict__ rank,
+                                                       const int* __restrict__ counters, int* __restrict__ slot_live) {
+    const unsigned long long* s = reinterpret_cast<const unsigned long long*>(src);
+    unsigned long long* d = reinterpret_cast<unsigned long long*>(dst);
+    const size_t n = (size_t)counters[VM_N_FEATS] * kVmFeatWords;
+    for (size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x; w < n; w += (size_t)gridDim.x * blockDim.x) {
+        const int f = (int)(w / kVmFeatWords), k = (int)(w - (size_t)f * kVmFeatWords);
+        if (!vm_feature_live(rank, f)) continue;
+        d[(size_t)vm_feature_remap(rank, f) * kVmFeatWords + k] = s[w];
+        if (k == 0) slot_live[src[f].img] = 1;
+    }
+}
+
+// every point's observation ids through the ranks (each thread rewrites only its own word)
+__global__ void __launch_bounds__(256) k_vm_rc_remap(VmPoint* __restrict__ pts, const int* __restrict__ rank, const int* __restrict__ counters) {
+    int* words = reinterpret_cast<int*>(pts);
+    const size_t n = (size_t)counters[VM_N_POINTS] * kVmPointWords;
+    for (size_t w = (size_t)blockIdx.x * blockDim.x + threadIdx.x; w < n; w += (size_t)gridDim.x * blockDim.x) {
+        const size_t j = w / kVmPointWords;
+        const int f = vm_point_word_feature(words + j * kVmPointWords, (int)(w - j * kVmPointWords));
+        if (f >= 0) words[w] = vm_feature_remap(rank, f);
+    }
+}
+
+// One block: the free-slot stack is rebuilt from scratch -- every slot below the tail that no live feature names and that
+// is not pinned -- lowest slot on top; then the counters.  slot_tmp = {slot_live | flags | ranks}, pool_slots each.
+__global__ void __launch_bounds__(1024) k_vm_rc_slots(int* counters, const int* __restrict__ n_live, int* slot_tmp, int pool_slots,
+                                                      int* __restrict__ free_slots) {
+    const int tail = counters[VM_N_IMAGES], pinned = counters[VM_IMG_SLOT];
+    const int* slot_live = slot_tmp;
+    int* flag = slot_tmp + pool_slots;
+    int* rank = slot_tmp + 2 * pool_slots;
+    for (int s = threadIdx.x; s < tail; s += 1024) flag[s] = vm_slot_free(slot_live, pinned, s) ? 1 : 0;
+    __syncthreads();
+    int total;
+    vm_block_scan(flag, tail, rank, &total);
+    for (int s = threadIdx.x; s < tail; s += 1024)
+        if (flag[s]) free_slots[total - 1 - rank[s]] = s;
+    if (threadIdx.x == 0) {
+        counters[VM_N_FREE] = total;
+        counters[VM_N_FEATS] = *n_live;
     }
 }
 

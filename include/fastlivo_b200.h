@@ -320,7 +320,7 @@ typedef struct flb_vmap_params {
     double Rcl[9], Pcl[3];     /* sparse_map->Rcl / Pcl */
     double R_LI[9], t_LI[3];   /* set_extrinsic(transl, rot), :35-39 */
 } flb_vmap_params;
-/* clears the map (LidarSelector::init, :41-79) */
+/* clears the map (LidarSelector::init, :41-79), the free-slot stack of flb_vmap_reclaim included */
 int flb_vmap_reset(flb_handle* h, const flb_vmap_params* p);
 /* LidarSelector::addFromSparseMap (:346-587).  pg_down: the scan in the world frame after the caller's
  * pcl::VoxelGrid (0.2 m, :7, :351-352), n x stride floats.  Builds sub_sparse_map on the device: positions, warped
@@ -345,12 +345,31 @@ int flb_vmap_add_observations(flb_handle* h, const double Rcw[9], const double P
  * is the input order.  Rcw / Pcw NULL: from the device state (after flb_vmap_reset).  Blocking. */
 int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, const float* world_xyz, int n,
                  int stride_floats, uint8_t* rgb, uint8_t* valid);
+/* Gives back what the reference frees (opt-in; enqueue-only, no host synchronisation).  A Feature is owned by
+ * Point::obs_ alone, so it dies when addObservation evicts it (deleteFeatureRef(getFurthestViewObs),
+ * src/lidar_selection.cpp:946-950); its keyframe image (Feature::img, :183, :957) dies with the last Feature that refers
+ * to it; Points are never freed (feat_map keeps them).  The call compacts the feature array to the features some
+ * observation list names -- creation order kept, the lists remapped -- and puts every keyframe slot no live feature
+ * names (except the current frame's) on a free-slot stack that the following frames fill before the pool grows.  Image
+ * data never moves.  Selections, patches, errors and observation lists are unchanged by it: nothing refers to a feature
+ * id across calls.  Call it between any two visual-map calls (e.g. after flb_vmap_add_observations) at the cadence the
+ * caller chooses; without it nothing changes. */
+int flb_vmap_reclaim(flb_handle* h);
+/* memory of the visual map (blocking; any pointer may be NULL): points; features in the array, of which `dead` are no
+ * longer named by any observation list (reclaimable); feature-array capacity; keyframe slots in use, on the free-slot
+ * stack, and the pool's capacity in slots; device bytes the visual map holds. */
+int flb_vmap_usage(flb_handle* h, int* points, int* features, int* dead_features, int* feature_capacity, int* slots_in_use,
+                   int* free_slots, int* pool_slots, int64_t* device_bytes);
+/* the keyframe image in pool slot `slot` (tests, debugging; blocking): width x height bytes into gray (capacity bytes). */
+int flb_vmap_keyframe(flb_handle* h, int slot, uint8_t* gray, int capacity);
 /* sizes (blocking): points, features, keyframe images, patches of the last selection, items appended by the last
- * grow / add_observations call.  Any pointer may be NULL. */
+ * grow / add_observations call.  Any pointer may be NULL.  After a flb_vmap_reclaim, features is the compacted array's
+ * length and images the keyframe slots in use. */
 int flb_vmap_counts(flb_handle* h, int* points, int* features, int* images, int* selected, int* last_added);
 int flb_vmap_map_value(flb_handle* h, float* out, int capacity);       /* map_value[length] (:356, :455, :162) */
 /* the whole map (tests, debugging; blocking): per point pos (3 doubles), value, n_obs, newest-first feature ids
- * (20, -1 padded); per feature px(2) f(3) T_f_w R(9) t(3) = 17 doubles, score, {level, frame id, image slot}. */
+ * (20, -1 padded); per feature px(2) f(3) T_f_w R(9) t(3) = 17 doubles, score, {level, frame id, image slot}.
+ * After a flb_vmap_reclaim: the surviving features in creation order, the ids as remapped. */
 int flb_vmap_dump(flb_handle* h, int cap_points, int cap_features, double* pos, float* value, int* n_obs, int* obs20, double* ft_geo17,
                   float* ft_score, int* ft_level_id_img);
 
