@@ -14,6 +14,8 @@
 //        LidarSelector::ComputeJ(cv::Mat)  src/lidar_selection.cpp:967-983
 //   flb::undistort_pcl(h, prm, carry, v_imu, pcl_beg_time, pcl_end_time, state_inout, pcl_out)   replaces
 //        ImuProcess::UndistortPcl from src/IMU_Processing.cpp:655 on (propagation + undistortion)
+//   flb::map_incremental(h, lio_prm, filter_size_map_min)  /  flb::map_incremental(h, lio_prm, R, p, filter_size_map_min)   replace
+//        map_incremental()  src/laserMapping.cpp:692-706  (the uploaded scan into the map, no host transform)
 //
 // Type requirements (all met by the reference's types):
 //   Mat3  : operator()(i,j) read/write (Eigen::Matrix3d)          Vec3 : operator()(i) / [i]
@@ -110,6 +112,26 @@ inline flb_lio_report lio_update(flb_handle* h, const flb_lio_params& prm, State
     check(h, flb_lio_update(h, &prm, &x, &xp, &rep));
     from_abi(x, state);
     return rep;
+}
+
+// ---- map_incremental (src/laserMapping.cpp:692-706) from the uploaded scan ---------------------
+// Replaces the pointBodyToWorld loop over feats_down_body and ikdtree.Add_Points(feats_down_world, true) with
+// downsample_size = filter_size_map_min: the scan uploaded for this frame (upload_scan) is transformed on the device.
+// 18-DoF path: at the device state the LIO update just left (call it right after lio_update).
+inline void map_incremental(flb_handle* h, const flb_lio_params& lio_prm, float filter_size_map_min) {
+    check(h, flb_map_add_scan(h, &lio_prm, nullptr, nullptr, filter_size_map_min));
+}
+// Explicit pose (R: Mat3 with operator()(i, j), p: Vec3) with lio_prm's extrinsic.  IKFoM callers (RGBpointBodyToWorld
+// under USE_IKFOM): R = s.rot.toRotationMatrix(), p = s.pos, and lio_prm.R_LI / t_LI from s.offset_R_L_I.toRotationMatrix()
+// / s.offset_T_L_I (make_lio_params).
+template <class Mat3, class Vec3>
+inline void map_incremental(flb_handle* h, const flb_lio_params& lio_prm, const Mat3& R, const Vec3& p, float filter_size_map_min) {
+    double Rm[9], pv[3];
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) Rm[3 * i + j] = R(i, j);
+        pv[i] = p(i);
+    }
+    check(h, flb_map_add_scan(h, &lio_prm, Rm, pv, filter_size_map_min));
 }
 
 // ---- IKFoM-typed measurement callback (src/laserMapping.cpp:960-1094) ------------------------

@@ -164,7 +164,7 @@ class VioEq(C.Structure):
 
 # every symbol include/fastlivo_b200.h declares (checked by the CPU-only test tier)
 SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "flb_set_stream", "flb_synchronize", "flb_host_alloc", "flb_host_free",
-           "flb_map_upload", "flb_map_add_points", "flb_map_delete_boxes", "flb_map_size", "flb_map_download", "flb_scan_upload", "flb_knn", "flb_lio_pass", "flb_lio_export", "flb_lio_update", "flb_lio_update_ikfom",
+           "flb_map_upload", "flb_map_add_points", "flb_map_add_scan", "flb_map_delete_boxes", "flb_map_size", "flb_map_download", "flb_scan_upload", "flb_knn", "flb_lio_pass", "flb_lio_export", "flb_lio_update", "flb_lio_update_ikfom",
            "flb_image_upload", "flb_patches_upload", "flb_camera_set", "flb_vio_pass", "flb_vio_export",
            "flb_vio_update", "flb_state_upload", "flb_state_download", "flb_lio_update_enqueue",
            "flb_vio_update_enqueue", "flb_state_reset_enqueue", "flb_state_set_prior_enqueue", "flb_profile_start", "flb_profile_stop",
@@ -215,6 +215,7 @@ def lib():
         L.flb_map_upload.argtypes = [vp, vp, C.c_int, C.c_int]
         L.flb_scan_upload.argtypes = [vp, vp, C.c_int, C.c_int]
         L.flb_map_add_points.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float]
+        L.flb_map_add_scan.argtypes = [vp, C.POINTER(LioParams), vp, vp, C.c_float]
         L.flb_map_delete_boxes.argtypes = [vp, vp, C.c_int]
         L.flb_map_size.argtypes = [vp]
         L.flb_map_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
@@ -353,6 +354,13 @@ class Handle:
     def map_add_points(self, world_xyz, downsample_size):
         a = np.ascontiguousarray(world_xyz, np.float32)
         self._ck(self.L.flb_map_add_points(self.h, _p(a), a.shape[0], a.shape[1], C.c_float(downsample_size)))
+        self.M = self.L.flb_map_size(self.h)
+
+    def map_add_scan(self, prm, downsample_size, R=None, p=None):
+        """flb_map_add_scan: Add_Points of the uploaded scan at pose (R, p), or at the device state x when both are None."""
+        R = None if R is None else np.ascontiguousarray(R, np.float64)
+        p = None if p is None else np.ascontiguousarray(p, np.float64)
+        self._ck(self.L.flb_map_add_scan(self.h, C.byref(prm) if prm is not None else None, _p(R), _p(p), C.c_float(downsample_size)))
         self.M = self.L.flb_map_size(self.h)
 
     def map_delete_boxes(self, boxes):

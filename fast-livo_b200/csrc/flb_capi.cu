@@ -183,6 +183,8 @@ struct flb_handle {
     DevBuf<unsigned long long> vkeys, vkeys_sorted;
     DevBuf<unsigned char> keep;
     DevBuf<int> sel_idx;
+    DevBuf<float> add_xyz;                     // Add_Points: the new points on the device (packed xyz, input order)
+    DevBuf<unsigned> add_rec;                  // flb_map_add_scan: bounds + non-finite record (kScanRec*)
 
     // scan + per-point persistent
     int N = 0;
@@ -201,6 +203,7 @@ struct flb_handle {
     cudaEvent_t ev_scan_free[2] = {nullptr, nullptr};   // [slot]: everything on `stream` that reads that slot has been enqueued before it
     bool scan_free_valid[2] = {false, false};
     int scan_slot = 0;
+    bool scan_valid = false;                            // the current set holds an uploaded scan (not flb_voxel_grid's scratch)
     DevBuf<unsigned char> scan_cub_tmp;                 // the upload's own sort scratch (cub_tmp belongs to `stream`)
     int pers_sms = 0;                                   // SMs the persistent kernels may fill (one is left to the scan stream)
     int scan_sort_mode = 0;                             // 0 auto, 1 one-block ordering kernel, 2 device-wide sort (flb_debug_set_scan_sort)
@@ -989,6 +992,7 @@ int flb_destroy(flb_handle* h) {
     for (auto& ev : h->evs) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
     h->map_raw.release(); h->keys.release(); h->keys_sorted.release(); h->vals.release(); h->vals_sorted.release();
     h->map_comb.release(); h->boxes.release(); h->vkeys.release(); h->vkeys_sorted.release(); h->keep.release(); h->sel_idx.release();
+    h->add_xyz.release(); h->add_rec.release();
     h->cell_table.release(); h->cell_keys.release(); h->cell_keys_alt.release();
     h->map_pts_alt.release(); h->cell_start_alt.release(); h->map_raw_alt.release(); h->dead.release(); h->ins.release();
     h->dead_before.release(); h->merge_counts.release(); h->bbox_dev.release();
@@ -1260,7 +1264,7 @@ static int compact_and_rebuild(flb_handle* h, const int* idx_in, int total) {
 
 // Full path of Add_Points: (existing + new) points sorted by downsample voxel, one thread per voxel, compaction, grid
 // rebuilt from scratch.  Taken when a new point lies outside the box the kNN grid covers (the grid has to grow).
-static int map_add_points_full(flb_handle* h, const float* st, int n, float downsample_size) {
+static int map_add_points_full(flb_handle* h, const float* nxyz, int n, float downsample_size) {
     const int M = h->M, total = M + n;
     FLB_CUDA(h, h->map_comb.reserve((size_t)total * 3));
     FLB_CUDA(h, h->vkeys.reserve(total));
@@ -1269,8 +1273,9 @@ static int map_add_points_full(flb_handle* h, const float* st, int n, float down
     FLB_CUDA(h, h->vals_sorted.reserve(total));
     FLB_CUDA(h, h->keep.reserve(total));
     FLB_CUDA(h, cudaMemcpyAsync(h->map_comb.p, h->map_raw.p, (size_t)M * 3 * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
-    FLB_CUDA(h, cudaMemcpyAsync(h->map_comb.p + (size_t)M * 3, st, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-    FLB_CUDA(h, h->st_map.mark(h->stream));
+    // The new points arrive in add_xyz (both entry points fill it before the path is known), so this path -- the rare one,
+    // whose cost is the radix sort of all M + n points -- pays one n x 12 B device-to-device copy to put them behind the map.
+    FLB_CUDA(h, cudaMemcpyAsync(h->map_comb.p + (size_t)M * 3, nxyz, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
     const int nb = (total + 255) / 256;
     {
         LaunchScope ls(h, FAM_OTHER);
@@ -1301,7 +1306,7 @@ static int bits_for(long long span) {
 
 // Incremental Add_Points on the sparse index (always: there is no box to leave).  The steps of the dense incremental path
 // below, on 64-bit cell keys; the hash table is then rebuilt from the merged key array.  Nothing scales with the extent.
-static int map_add_points_sparse(flb_handle* h, const float* st, int n, float ds, const float* lo, const float* hi) {
+static int map_add_points_sparse(flb_handle* h, const float* nxyz, int n, float ds, const float* lo, const float* hi) {
     const int M = h->M;
     const GridDesc g = h->grid;
     // voxel keys relative to the new points' own box (absolute 21-bit keys if that box needs more than 62 bits)
@@ -1310,7 +1315,6 @@ static int map_add_points_sparse(flb_handle* h, const float* st, int n, float ds
               wz = bits_for((long long)std::floor(hi[2] / ds) + 2 - bz);
     const bool rel = wx + wy + wz <= 62;
     const int vbits = rel ? wx + wy + wz : 63;
-    FLB_CUDA(h, h->map_comb.reserve((size_t)n * 3));
     FLB_CUDA(h, h->vkeys.reserve(n));
     FLB_CUDA(h, h->vkeys_sorted.reserve(n));
     FLB_CUDA(h, h->vals.reserve(n));
@@ -1322,9 +1326,6 @@ static int map_add_points_sparse(flb_handle* h, const float* st, int n, float ds
     FLB_CUDA(h, h->map_pts_alt.reserve((size_t)M + n));
     FLB_CUDA(h, h->map_raw_alt.reserve(((size_t)M + n) * 3));
     FLB_CUDA(h, h->cell_keys_alt.reserve((size_t)M + n));
-    float* nxyz = h->map_comb.p;
-    FLB_CUDA(h, cudaMemcpyAsync(nxyz, st, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-    FLB_CUDA(h, h->st_map.mark(h->stream));
     FLB_CUDA(h, cudaMemsetAsync(h->dead.p, 0, M, h->stream));
     FLB_CUDA(h, cudaMemsetAsync(h->ins.p, 0, n, h->stream));
     const int gn = (n + 255) / 256, gm = (M + 255) / 256;
@@ -1376,66 +1377,32 @@ static int map_add_points_sparse(flb_handle* h, const float* st, int n, float ds
     return build_sparse_table(h, h->M);
 }
 
-int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride, float downsample_size) {
-    FLB_CHECK_H(h);
-    if (h->M <= 0) return fail(h, FLB_ERR_STATE, "flb_map_add_points: no map uploaded");
-    if (!world_xyz || n < 0 || stride < 3 || !(downsample_size > 0)) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: bad arguments");
-    if (n == 0) return FLB_OK;
-    const int M = h->M;
-    void* stv = nullptr;
-    FLB_CUDA(h, h->st_map.acquire((size_t)n * 3 * sizeof(float), &stv));
-    float* st = static_cast<float*>(stv);
-    float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-    if (stride == 3) std::memcpy(st, world_xyz, (size_t)n * 3 * sizeof(float));
-    else
-        for (int i = 0; i < n; ++i) {
-            st[3 * (size_t)i] = world_xyz[(size_t)i * stride];
-            st[3 * (size_t)i + 1] = world_xyz[(size_t)i * stride + 1];
-            st[3 * (size_t)i + 2] = world_xyz[(size_t)i * stride + 2];
-        }
-    {
-        // bounds + finiteness over the packed floats, 24 (= 8 points) at a time into independent accumulators (vectorises)
-        float mn[24], mx[24];
-        for (int j = 0; j < 24; ++j) { mn[j] = INFINITY; mx[j] = -INFINITY; }
-        unsigned bad = 0;
-        const size_t n3 = (size_t)n * 3;
-        size_t i = 0;
-        for (; i + 24 <= n3; i += 24)
-            for (int j = 0; j < 24; ++j) {
-                const float v = st[i + j];
-                unsigned bits;
-                std::memcpy(&bits, &v, sizeof(bits));
-                bad |= ((bits & 0x7F800000u) == 0x7F800000u) ? 1u : 0u;
-                mn[j] = v < mn[j] ? v : mn[j];
-                mx[j] = v > mx[j] ? v : mx[j];
-            }
-        for (; i < n3; ++i) {
-            const float v = st[i];
-            const int j = (int)(i % 24);
-            bad |= std::isfinite(v) ? 0u : 1u;
-            mn[j] = v < mn[j] ? v : mn[j];
-            mx[j] = v > mx[j] ? v : mx[j];
-        }
-        if (bad) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: non-finite coordinate");
-        for (int j = 0; j < 24; ++j) { lo[j % 3] = std::min(lo[j % 3], mn[j]); hi[j % 3] = std::max(hi[j % 3], mx[j]); }
-        const float lim = 1.0e6f * downsample_size;
-        for (int k = 0; k < 3; ++k)
-            if (lo[k] < -lim || hi[k] > lim) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: coordinate / downsample_size exceeds 2^20 voxels");
-        if (h->sparse) {
-            // the sparse index has no box to leave, but every cell needs a key: within 2^20 cells of the anchor
-            const float o[3] = {h->grid.ox, h->grid.oy, h->grid.oz}, lk = (float)kCellKeyBias;
-            for (int k = 0; k < 3; ++k) {
-                const float a = (lo[k] - o[k]) * h->grid.inv_cell, b = (hi[k] - o[k]) * h->grid.inv_cell;
-                if (!(a >= -lk && b < lk)) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: point more than 2^20 cells from the map's anchor");
-            }
+// The voxel-key and cell-key limits of new points with bounds lo / hi (shared by both Add_Points entry points).
+static int map_add_check_bounds(flb_handle* h, const char* who, const float* lo, const float* hi, float downsample_size) {
+    const float lim = 1.0e6f * downsample_size;
+    for (int k = 0; k < 3; ++k)
+        if (lo[k] < -lim || hi[k] > lim) return fail(h, FLB_ERR_INVALID, "%s: coordinate / downsample_size exceeds 2^20 voxels", who);
+    if (h->sparse) {
+        // the sparse index has no box to leave, but every cell needs a key: within 2^20 cells of the anchor
+        const float o[3] = {h->grid.ox, h->grid.oy, h->grid.oz}, lk = (float)kCellKeyBias;
+        for (int k = 0; k < 3; ++k) {
+            const float a = (lo[k] - o[k]) * h->grid.inv_cell, b = (hi[k] - o[k]) * h->grid.inv_cell;
+            if (!(a >= -lk && b < lk)) return fail(h, FLB_ERR_INVALID, "%s: point more than 2^20 cells from the map's anchor", who);
         }
     }
-    // the input is valid from here on: only now does the map box take it in
+    return FLB_OK;
+}
+
+// Add_Points (downsample = true) of n >= 1 validated new points already on the device (nxyz, packed, in input order;
+// bounds lo / hi): the map box takes them in, then the sparse-index merge, the full rebuild or the dense incremental
+// merge runs.  flb_map_add_points and flb_map_add_scan differ only in how the points get to nxyz.
+static int map_add_points_dev(flb_handle* h, const float* nxyz, int n, float downsample_size, const float* lo, const float* hi) {
+    const int M = h->M;
     bool inside = true;
     for (int k = 0; k < 3; ++k) inside = inside && lo[k] >= h->grid_lo[k] && hi[k] <= h->grid_hi[k];
     for (int k = 0; k < 3; ++k) { h->map_lo[k] = std::min(h->map_lo[k], lo[k]); h->map_hi[k] = std::max(h->map_hi[k], hi[k]); }
-    if (h->sparse) return map_add_points_sparse(h, st, n, downsample_size, lo, hi);
-    if (!inside) return map_add_points_full(h, st, n, downsample_size);
+    if (h->sparse) return map_add_points_sparse(h, nxyz, n, downsample_size, lo, hi);
+    if (!inside) return map_add_points_full(h, nxyz, n, downsample_size);
 
     // ---- incremental path: every new point lies inside the box the grid covers
     const GridDesc g = h->grid;
@@ -1445,8 +1412,7 @@ int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride,
     const int bx = (int)std::floor(h->grid_lo[0] / ds) - 1, by = (int)std::floor(h->grid_lo[1] / ds) - 1, bz = (int)std::floor(h->grid_lo[2] / ds) - 1;
     const int wx = bits_for((long long)std::floor(h->grid_hi[0] / ds) + 2 - bx), wy = bits_for((long long)std::floor(h->grid_hi[1] / ds) + 2 - by),
               wz = bits_for((long long)std::floor(h->grid_hi[2] / ds) + 2 - bz);
-    if (wx + wy + wz > 62) return map_add_points_full(h, st, n, downsample_size);
-    FLB_CUDA(h, h->map_comb.reserve((size_t)n * 3));
+    if (wx + wy + wz > 62) return map_add_points_full(h, nxyz, n, downsample_size);
     FLB_CUDA(h, h->vkeys.reserve(n));
     FLB_CUDA(h, h->vkeys_sorted.reserve(n));
     FLB_CUDA(h, h->vals.reserve(std::max(n, M)));
@@ -1460,9 +1426,6 @@ int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride,
     FLB_CUDA(h, h->map_pts_alt.reserve((size_t)M + n));
     FLB_CUDA(h, h->map_raw_alt.reserve(((size_t)M + n) * 3));
     FLB_CUDA(h, h->cell_start_alt.reserve((size_t)ncell + 1));
-    float* nxyz = h->map_comb.p;
-    FLB_CUDA(h, cudaMemcpyAsync(nxyz, st, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-    FLB_CUDA(h, h->st_map.mark(h->stream));
     FLB_CUDA(h, cudaMemsetAsync(h->dead.p, 0, M, h->stream));
     FLB_CUDA(h, cudaMemsetAsync(h->ins.p, 0, n, h->stream));
     const int gn = (n + 255) / 256, gm = (M + 255) / 256;
@@ -1516,6 +1479,103 @@ int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride,
     h->M = M - counts[0] + counts[1];
     h->last_pass_valid = false;
     return FLB_OK;
+}
+
+int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride, float downsample_size) {
+    FLB_CHECK_H(h);
+    if (h->M <= 0) return fail(h, FLB_ERR_STATE, "flb_map_add_points: no map uploaded");
+    if (!world_xyz || n < 0 || stride < 3 || !(downsample_size > 0)) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: bad arguments");
+    if (n == 0) return FLB_OK;
+    void* stv = nullptr;
+    FLB_CUDA(h, h->st_map.acquire((size_t)n * 3 * sizeof(float), &stv));
+    float* st = static_cast<float*>(stv);
+    float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+    if (stride == 3) std::memcpy(st, world_xyz, (size_t)n * 3 * sizeof(float));
+    else
+        for (int i = 0; i < n; ++i) {
+            st[3 * (size_t)i] = world_xyz[(size_t)i * stride];
+            st[3 * (size_t)i + 1] = world_xyz[(size_t)i * stride + 1];
+            st[3 * (size_t)i + 2] = world_xyz[(size_t)i * stride + 2];
+        }
+    {
+        // bounds + finiteness over the packed floats, 24 (= 8 points) at a time into independent accumulators (vectorises)
+        float mn[24], mx[24];
+        for (int j = 0; j < 24; ++j) { mn[j] = INFINITY; mx[j] = -INFINITY; }
+        unsigned bad = 0;
+        const size_t n3 = (size_t)n * 3;
+        size_t i = 0;
+        for (; i + 24 <= n3; i += 24)
+            for (int j = 0; j < 24; ++j) {
+                const float v = st[i + j];
+                unsigned bits;
+                std::memcpy(&bits, &v, sizeof(bits));
+                bad |= ((bits & 0x7F800000u) == 0x7F800000u) ? 1u : 0u;
+                mn[j] = v < mn[j] ? v : mn[j];
+                mx[j] = v > mx[j] ? v : mx[j];
+            }
+        for (; i < n3; ++i) {
+            const float v = st[i];
+            const int j = (int)(i % 24);
+            bad |= std::isfinite(v) ? 0u : 1u;
+            mn[j] = v < mn[j] ? v : mn[j];
+            mx[j] = v > mx[j] ? v : mx[j];
+        }
+        if (bad) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: non-finite coordinate");
+        for (int j = 0; j < 24; ++j) { lo[j % 3] = std::min(lo[j % 3], mn[j]); hi[j % 3] = std::max(hi[j % 3], mx[j]); }
+    }
+    { int rcb = map_add_check_bounds(h, "flb_map_add_points", lo, hi, downsample_size); if (rcb) return rcb; }
+    // the input is valid from here on: only now does it go to the device and the map box take it in
+    FLB_CUDA(h, h->add_xyz.reserve((size_t)n * 3));
+    FLB_CUDA(h, cudaMemcpyAsync(h->add_xyz.p, st, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    FLB_CUDA(h, h->st_map.mark(h->stream));
+    return map_add_points_dev(h, h->add_xyz.p, n, downsample_size, lo, hi);
+}
+
+// map_incremental (src/laserMapping.cpp:692-706) from what is on the device: the uploaded scan, transformed at (R, p) or
+// at the device state x, enters Add_Points in the caller's order.  One kernel (transform + bounds) and one small
+// readback replace flb_map_add_points' staging, host checks and copy; the merge is the same code.
+int flb_map_add_scan(flb_handle* h, const flb_lio_params* prm, const double R[9], const double p[3], float downsample_size) {
+    FLB_CHECK_H(h);
+    if (h->M <= 0) return fail(h, FLB_ERR_STATE, "flb_map_add_scan: no map uploaded");
+    if (!prm || (R == nullptr) != (p == nullptr) || !(downsample_size > 0))
+        return fail(h, FLB_ERR_INVALID, "flb_map_add_scan: bad arguments (prm, R and p both or neither, downsample_size > 0)");
+    if (h->comm || h->p2p.world > 0)
+        return fail(h, FLB_ERR_STATE, "flb_map_add_scan: single GPU only (each rank holds only its shard of the scan)");
+    if (!h->scan_valid)
+        return fail(h, FLB_ERR_STATE, "flb_map_add_scan: no scan uploaded since the last flb_voxel_grid (or ever)");
+    if (!R && !h->state_valid) return fail(h, FLB_ERR_STATE, "flb_map_add_scan: no pose given and no device state");
+    const int n = h->N;
+    if (n == 0) return FLB_OK;
+    if (!R) { int rcf = flush_state_ops(h); if (rcf) return rcf; }
+    LioPose pose{};
+    std::memcpy(pose.R_LI, prm->R_LI, sizeof(pose.R_LI));
+    std::memcpy(pose.t_LI, prm->t_LI, sizeof(pose.t_LI));
+    if (R) {
+        std::memcpy(pose.R, R, sizeof(pose.R));
+        std::memcpy(pose.p, p, sizeof(pose.p));
+    }
+    FLB_CUDA(h, h->add_xyz.reserve((size_t)n * 3));
+    FLB_CUDA(h, h->add_rec.reserve(kScanRecWords));
+    FLB_CUDA(h, cudaMemsetAsync(h->add_rec.p, 0, kScanRecWords * sizeof(unsigned), h->stream));
+    {
+        // h->scan is the current set of the double-buffered scan.  This call ends with a stream synchronise, so a later
+        // flb_scan_upload (which fills the other set, and this one only after the next swap) cannot overwrite it under us.
+        LaunchScope ls(h, FAM_OTHER);
+        k_map_scan_world<<<(n + 255) / 256, 256, 0, h->stream>>>(h->scan.p, n, pose, R ? nullptr : &h->states.p[0], h->add_xyz.p,
+                                                                  h->add_rec.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    unsigned* rec = static_cast<unsigned*>(h->pin_out.p);
+    FLB_CUDA(h, cudaMemcpyAsync(rec, h->add_rec.p, kScanRecWords * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (rec[kScanRecBad]) return fail(h, FLB_ERR_INVALID, "flb_map_add_scan: non-finite coordinate");
+    float lo[3], hi[3];
+    for (int k = 0; k < 3; ++k) {
+        lo[k] = f32_from_order_key(~rec[kScanRecMin + k]);
+        hi[k] = f32_from_order_key(rec[kScanRecMax + k]);
+    }
+    { int rcb = map_add_check_bounds(h, "flb_map_add_scan", lo, hi, downsample_size); if (rcb) return rcb; }
+    return map_add_points_dev(h, h->add_xyz.p, n, downsample_size, lo, hi);
 }
 
 int flb_map_delete_boxes(flb_handle* h, const float* boxes, int nb) {
@@ -1772,6 +1832,7 @@ int flb_voxel_grid(flb_handle* h, const float* xyz, int n, int stride, float lea
         FLB_CUDA(h, cudaStreamSynchronize(h->stream));
     }
     h->N = 0;                                    // the scan slot was used as scratch
+    h->scan_valid = false;
     h->last_pass_valid = false;
     return FLB_OK;
 }
@@ -1899,6 +1960,7 @@ int flb_scan_upload(flb_handle* h, const float* body_xyz, int N, int stride) {
     std::swap(h->plane, h->plane_alt);
     h->scan_slot = alt;
     h->N = N;     // enqueue-only: everything later on this handle's stream is ordered after the upload
+    h->scan_valid = true;
     h->last_pass_valid = false;
     return FLB_OK;
 }

@@ -420,6 +420,32 @@ struct map_pt { float x, y, z, w; };
 #define FLB_LDGI(ptr) (*(ptr))
 #endif
 
+// ------------------------------------------------------------------ map_incremental from the uploaded scan
+// map_incremental (src/laserMapping.cpp:692-706), one point: the ordered scan entry `b` (body xyz, the caller's index in
+// w) -> pointBodyToWorld of it (:272-286) in pw.  Returns the caller's index, where the world point goes.
+FLB_HD int map_scan_point(const LioPose& c, const map_pt& b, float* pw) {
+    const float pb[3] = {b.x, b.y, b.z};
+    double pI[3];
+    lio_body_to_world(c, pb, pI, pw);
+    return (int)float_as_u32(b.w);
+}
+
+// Whether all three floats are finite (exponent field not all ones), as flb_map_add_points tests its input.
+FLB_HD bool finite3(const float* v) {
+    return ((float_as_u32(v[0]) & 0x7F800000u) != 0x7F800000u) && ((float_as_u32(v[1]) & 0x7F800000u) != 0x7F800000u) &&
+           ((float_as_u32(v[2]) & 0x7F800000u) != 0x7F800000u);
+}
+
+// Bounds record of the new points: an unsigned key that orders like the float, so that an atomic maximum on a zeroed
+// word yields the maximum (of key) and the minimum (of ~key).  -0.0 orders below +0.0; nothing downstream of the bounds
+// tells the two apart.
+enum { kScanRecMax = 0, kScanRecMin = 3, kScanRecBad = 6, kScanRecWords = 8 };
+FLB_HD unsigned f32_order_key(float f) {
+    const unsigned b = float_as_u32(f);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+FLB_HD float f32_from_order_key(unsigned k) { return u32_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+
 // Row bounds, the one reader of a cell index: the points of cells [xa, xb] of row (z, y) are one contiguous run of the
 // sorted array; returns its [start, end).  Dense: two table reads (the caller clips to the grid).  Sparse: start of the
 // first occupied cell, end of the last; (0, 0) when none is occupied.

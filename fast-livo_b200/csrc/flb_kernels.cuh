@@ -240,6 +240,53 @@ __global__ void k_bbox(const float* __restrict__ xyz, int n, int* __restrict__ b
 // device version sorts (existing + new) points by voxel and lets one thread replay that sequential
 // rule over each voxel's handful of points.
 // ---------------------------------------------------------------------------------------
+// map_incremental from the uploaded scan (flb_map_add_scan): one thread per point of the ordered scan writes
+// pointBodyToWorld of it to the caller's index in packed xyz, and the block folds its points into rec (kScanRec*: the
+// per-axis max and ~min order keys, the non-finite flag; zeroed before the launch) with one atomic maximum per word.
+// The pose is `pose`, or -- x non-null -- the device state's rot / pos with pose's extrinsic.
+__global__ void __launch_bounds__(256) k_map_scan_world(const float4* __restrict__ scan, int n, LioPose pose, const State18* __restrict__ x,
+                                                        float* __restrict__ out, unsigned* __restrict__ rec) {
+    __shared__ LioPose s_pose;
+    __shared__ unsigned s_red[8][kScanRecBad + 1];
+    if (threadIdx.x == 0) {
+        s_pose = pose;
+        if (x) {
+            for (int k = 0; k < 9; ++k) s_pose.R[k] = x->rot[k];
+            for (int k = 0; k < 3; ++k) s_pose.p[k] = x->pos[k];
+        }
+    }
+    __syncthreads();
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned v[kScanRecBad + 1] = {0, 0, 0, 0, 0, 0, 0};   // 0: the identity of the maximum for every word
+    if (i < n) {
+        float pw[3];
+        const int oi = map_scan_point(s_pose, scan[i], pw);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) out[3 * (size_t)oi + k] = pw[k];
+        if (finite3(pw)) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                v[kScanRecMax + k] = f32_order_key(pw[k]);
+                v[kScanRecMin + k] = ~v[kScanRecMax + k];
+            }
+        } else {
+            v[kScanRecBad] = 1;
+        }
+    }
+#pragma unroll
+    for (int w = 0; w <= kScanRecBad; ++w)
+        for (int o = 16; o > 0; o >>= 1) v[w] = max(v[w], __shfl_xor_sync(0xffffffffu, v[w], o));
+    if ((threadIdx.x & 31) == 0)
+#pragma unroll
+        for (int w = 0; w <= kScanRecBad; ++w) s_red[threadIdx.x >> 5][w] = v[w];
+    __syncthreads();
+    if (threadIdx.x <= kScanRecBad) {
+        unsigned m = 0;
+        for (int wp = 0; wp < (int)(blockDim.x >> 5); ++wp) m = max(m, s_red[wp][threadIdx.x]);
+        if (m) atomicMax(rec + threadIdx.x, m);
+    }
+}
+
 __device__ __forceinline__ unsigned long long vox_key(float x, float y, float z, float ds) {
     // floor(p / downsample_size) per axis (ikd_Tree.cpp:392-396), biased into 21 bits each
     const long long ix = (long long)floorf(x / ds) + (1ll << 20), iy = (long long)floorf(y / ds) + (1ll << 20),

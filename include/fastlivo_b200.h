@@ -100,6 +100,19 @@ int flb_map_upload(flb_handle* h, const float* xyz, int M, int stride_floats);
  * After either call map indices (flb_knn / flb_lio_export nn_idx) refer to the order flb_map_download
  * returns.  |coordinate / downsample_size| must stay below 2^20. */
 int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride_floats, float downsample_size);
+/* map_incremental (src/laserMapping.cpp:692-706) from what is on the device: every point of the scan most recently
+ * uploaded (flb_scan_upload / flb_frame_enqueue / flb_batch_set_frame), in the caller's original order, transformed by
+ * pointBodyToWorld (:272-286; double math, float store) at pose (R, p) with prm->R_LI / prm->t_LI, then
+ * Add_Points(..., downsample_size) exactly as flb_map_add_points: the same map bytes, order and grid as that call on the
+ * host-transformed scan.  R == p == NULL: the device state x as it stands in stream order (call it right after the LIO
+ * update for the reference's order).  IKFoM callers pass R = rot, p = pos and offset_R_L_I / offset_T_L_I as the
+ * extrinsic (RGBpointBodyToWorld under USE_IKFOM).  Blocking, like flb_map_add_points.  Single GPU.
+ * Errors, all leaving the map unchanged: FLB_ERR_STATE without a map, without a scan, after flb_voxel_grid used the scan
+ * slot as scratch, without a device state for R == NULL, and after flb_comm_init / flb_p2p_attach (each rank holds only
+ * its shard of the scan); FLB_ERR_INVALID for prm == NULL, exactly one of R / p NULL, downsample_size <= 0, and a
+ * transformed point that is not finite or beyond flb_map_add_points' limits. */
+struct flb_lio_params;
+int flb_map_add_scan(flb_handle* h, const struct flb_lio_params* prm, const double R[9], const double p[3], float downsample_size);
 int flb_map_delete_boxes(flb_handle* h, const float* boxes, int nb);
 int flb_map_size(const flb_handle* h);
 int flb_map_download(flb_handle* h, float* xyz, int capacity_points, int* M_out);
