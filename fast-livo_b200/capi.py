@@ -162,6 +162,8 @@ class VioEq(C.Structure):
                 ("n_meas", C.c_int64), ("skipped", C.c_int)]
 
 
+CLOUD_SCAN, CLOUD_UNDISTORTED = 0, 1       # flb_world_cloud sources (FLB_CLOUD_*)
+
 # every symbol include/fastlivo_b200.h declares (checked by the CPU-only test tier)
 SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "flb_set_stream", "flb_synchronize", "flb_host_alloc", "flb_host_free",
            "flb_map_upload", "flb_map_add_points", "flb_map_add_scan", "flb_map_delete_boxes", "flb_map_size", "flb_map_download", "flb_scan_upload", "flb_knn", "flb_lio_pass", "flb_lio_export", "flb_lio_update", "flb_lio_update_ikfom",
@@ -173,6 +175,7 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_vio_update_level", "flb_state_download_enqueue", "flb_state_download_wait", "flb_frame_enqueue",
            "flb_vmap_reset", "flb_vmap_select", "flb_vmap_selected", "flb_vmap_grow", "flb_vmap_add_observations", "flb_vmap_counts",
            "flb_vmap_map_value", "flb_vmap_dump", "flb_vmap_reclaim", "flb_vmap_usage", "flb_vmap_keyframe", "flb_colorize", "flb_voxel_grid",
+           "flb_world_cloud", "flb_world_cloud_download", "flb_vmap_select_cloud", "flb_vmap_grow_cloud", "flb_colorize_cloud",
            "flb_batch_begin", "flb_batch_set_frame", "flb_batch_state_reset_enqueue", "flb_batch_update_enqueue", "flb_batch_state_download",
            "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
            "flb_map_grid_info", "flb_debug_set_map_index"]
@@ -246,6 +249,11 @@ def lib():
         L.flb_batch_state_download.argtypes = [vp, C.c_int, C.POINTER(State18), C.POINTER(LioReport), C.POINTER(VioReport)]
         L.flb_voxel_grid.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float, vp, C.c_int, C.POINTER(C.c_int)]
         L.flb_colorize.argtypes = [vp, vp, vp, vp, C.c_int, vp, C.c_int, C.c_int, vp, vp]
+        L.flb_world_cloud.argtypes = [vp, C.POINTER(LioParams), vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_world_cloud_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_vmap_select_cloud.argtypes = [vp, vp, vp, C.c_float, vp]
+        L.flb_vmap_grow_cloud.argtypes = [vp, vp, vp, C.c_int]
+        L.flb_colorize_cloud.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp]
         L.flb_vmap_reset.argtypes = [vp, C.POINTER(VmapParams)]
         L.flb_vmap_select.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, vp]
         L.flb_vmap_selected.argtypes = [vp, C.c_int, C.POINTER(C.c_int)] + [vp] * 6
@@ -325,6 +333,7 @@ class Handle:
         if rc != FLB_OK:
             raise FlbError(rc, self.L.flb_last_error(None).decode())
         self.N = self.M = self.Pn = 0
+        self._wc_n = 0                  # points of the world cloud flb_world_cloud last built
 
     def close(self):
         if getattr(self, "h", None):
@@ -608,6 +617,48 @@ class Handle:
         rgb = np.zeros((len(pts), 3), np.uint8)
         val = np.zeros(len(pts), np.uint8)
         self._ck(self.L.flb_colorize(self.h, pr, pp, _p(img), img.shape[1] * 3, _p(pts), len(pts), 3, _p(rgb), _p(val)))
+        return rgb, val.astype(bool)
+
+    # ---- the frame's world cloud (pcl_wait_pub) on the device
+    def world_cloud(self, prm, source=CLOUD_UNDISTORTED, R=None, p=None):
+        """flb_world_cloud: the source cloud (CLOUD_SCAN / CLOUD_UNDISTORTED) at pose (R, p), or at the device state x
+        when both are None; returns its number of points."""
+        R = None if R is None else np.ascontiguousarray(R, np.float64)
+        p = None if p is None else np.ascontiguousarray(p, np.float64)
+        n = C.c_int()
+        self._wc_n = 0
+        self._ck(self.L.flb_world_cloud(self.h, C.byref(prm) if prm is not None else None, _p(R), _p(p), int(source), C.byref(n)))
+        self._wc_n = n.value
+        return n.value
+
+    def world_cloud_download(self):
+        """flb_world_cloud_download: the world cloud (n, 3) float32."""
+        out = np.zeros((self._wc_n, 3), np.float32)
+        n = C.c_int()
+        self._ck(self.L.flb_world_cloud_download(self.h, _p(out), len(out), C.byref(n)))
+        return out[:n.value]
+
+    def vmap_select_cloud(self, Rcw, Pcw, leaf=0.2, blocking=True):
+        """flb_vmap_select_cloud: vmap_select of downSizeFilter(world cloud, leaf), all on the device."""
+        R, P, pr, pp = self._pose(Rcw, Pcw)
+        n = C.c_int()
+        self._ck(self.L.flb_vmap_select_cloud(self.h, pr, pp, C.c_float(leaf), C.byref(n) if blocking else None))
+        if blocking:
+            self.Pn = n.value
+            return n.value
+        return None
+
+    def vmap_grow_cloud(self, Rcw, Pcw, frame_id):
+        R, P, pr, pp = self._pose(Rcw, Pcw)
+        self._ck(self.L.flb_vmap_grow_cloud(self.h, pr, pp, int(frame_id)))
+
+    def colorize_cloud(self, Rcw, Pcw, bgr):
+        """flb_colorize_cloud: (rgb (n, 3) uint8, valid (n,) bool) of the world cloud."""
+        R, P, pr, pp = self._pose(Rcw, Pcw)
+        img = np.ascontiguousarray(bgr, np.uint8)
+        rgb = np.zeros((self._wc_n, 3), np.uint8)
+        val = np.zeros(self._wc_n, np.uint8)
+        self._ck(self.L.flb_colorize_cloud(self.h, pr, pp, _p(img), img.shape[1] * 3, _p(rgb), _p(val)))
         return rgb, val.astype(bool)
 
     def vmap_counts(self):

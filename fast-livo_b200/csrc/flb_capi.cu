@@ -239,6 +239,19 @@ struct flb_handle {
     DevBuf<double> imu_buf;            // flb_imu_undistort: samples | carry | aux | poses
     DevBuf<float4> imu_pts;            // in | out
     DevBuf<int> imu_heads;
+    // the output of the last successful flb_imu_undistort (feats_undistort): inside imu_pts, where depends on its point
+    // count.  undist_n < 0: none (no call yet, or the last one failed)
+    const float4* undist_pts = nullptr;
+    int undist_n = -1;
+    // flb_world_cloud: pcl_wait_pub (packed xyz, the caller's order) with its exact bounds; wc_n < 0: no cloud held
+    DevBuf<float> wc_xyz;
+    DevBuf<unsigned> wc_rec;           // bounds + non-finite record of the transform (kScanRec*)
+    int wc_n = -1;
+    float wc_lo[3] = {0, 0, 0}, wc_hi[3] = {0, 0, 0};
+    // flb_vmap_select_cloud: downSizeFilter of the world cloud and its scratch (the scan slot's stays untouched)
+    DevBuf<float> wc_down;
+    DevBuf<unsigned> wc_keys, wc_keys_sorted;
+    DevBuf<int> wc_vals, wc_vals_sorted, wc_heads, wc_box;   // heads: head flags | ranks; box: k_bbox box | overflow | count
     DevBuf<unsigned long long> vm_key;   // flb_visual_candidates: per-cell {score, ~index}
     DevBuf<float> vm_val, vm_pts;
     DevBuf<int> vm_win;
@@ -993,6 +1006,8 @@ int flb_destroy(flb_handle* h) {
     h->map_raw.release(); h->keys.release(); h->keys_sorted.release(); h->vals.release(); h->vals_sorted.release();
     h->map_comb.release(); h->boxes.release(); h->vkeys.release(); h->vkeys_sorted.release(); h->keep.release(); h->sel_idx.release();
     h->add_xyz.release(); h->add_rec.release();
+    h->wc_xyz.release(); h->wc_rec.release(); h->wc_down.release(); h->wc_keys.release(); h->wc_keys_sorted.release();
+    h->wc_vals.release(); h->wc_vals_sorted.release(); h->wc_heads.release(); h->wc_box.release();
     h->cell_table.release(); h->cell_keys.release(); h->cell_keys_alt.release();
     h->map_pts_alt.release(); h->cell_start_alt.release(); h->map_raw_alt.release(); h->dead.release(); h->ins.release();
     h->dead_before.release(); h->merge_counts.release(); h->bbox_dev.release();
@@ -1578,6 +1593,85 @@ int flb_map_add_scan(flb_handle* h, const flb_lio_params* prm, const double R[9]
     return map_add_points_dev(h, h->add_xyz.p, n, downsample_size, lo, hi);
 }
 
+// pcl_wait_pub (src/laserMapping.cpp:1763-1772) from what is on the device: the uploaded scan (feats_down_body) or the
+// last flb_imu_undistort output (feats_undistort), transformed at (R, p) or at the device state x into wc_xyz, in the
+// caller's order.  The kernel of flb_map_add_scan; its bounds record is the one read back, and it is kept for the
+// overflow test of flb_vmap_select_cloud.  The visual-map consumers (*_cloud) read wc_xyz on the device.
+int flb_world_cloud(flb_handle* h, const flb_lio_params* prm, const double R[9], const double p[3], int source, int* n_out) {
+    FLB_CHECK_H(h);
+    h->wc_n = -1;                                     // on any error below, no cloud is held
+    if (n_out) *n_out = 0;
+    if (!prm || (R == nullptr) != (p == nullptr) || (source != FLB_CLOUD_SCAN && source != FLB_CLOUD_UNDISTORTED))
+        return fail(h, FLB_ERR_INVALID, "flb_world_cloud: bad arguments (prm, R and p both or neither, source)");
+    const float4* src = nullptr;
+    int n = 0;
+    if (source == FLB_CLOUD_SCAN) {
+        if (h->comm || h->p2p.world > 0)
+            return fail(h, FLB_ERR_STATE, "flb_world_cloud: FLB_CLOUD_SCAN is single GPU only (each rank holds only its shard of the scan)");
+        if (!h->scan_valid) return fail(h, FLB_ERR_STATE, "flb_world_cloud: no scan uploaded since the last flb_voxel_grid (or ever)");
+        src = h->scan.p;
+        n = h->N;
+    } else {
+        if (h->undist_n < 0) return fail(h, FLB_ERR_STATE, "flb_world_cloud: no flb_imu_undistort output (none yet, or the last call failed)");
+        src = h->undist_pts;
+        n = h->undist_n;
+    }
+    if (!R && !h->state_valid) return fail(h, FLB_ERR_STATE, "flb_world_cloud: no pose given and no device state");
+    float lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0};
+    if (n > 0) {
+        if (!R) { int rcf = flush_state_ops(h); if (rcf) return rcf; }
+        LioPose pose{};
+        std::memcpy(pose.R_LI, prm->R_LI, sizeof(pose.R_LI));
+        std::memcpy(pose.t_LI, prm->t_LI, sizeof(pose.t_LI));
+        if (R) {
+            std::memcpy(pose.R, R, sizeof(pose.R));
+            std::memcpy(pose.p, p, sizeof(pose.p));
+        }
+        FLB_CUDA(h, h->wc_xyz.reserve((size_t)n * 3));
+        FLB_CUDA(h, h->wc_rec.reserve(kScanRecWords));
+        FLB_CUDA(h, cudaMemsetAsync(h->wc_rec.p, 0, kScanRecWords * sizeof(unsigned), h->stream));
+        {
+            // Both sources stay put until the synchronise below: a later flb_scan_upload fills the other scan set, and
+            // flb_imu_undistort is blocking.  wc_xyz is a copy, so neither changes the cloud afterwards.
+            LaunchScope ls(h, FAM_OTHER);
+            const State18* x = R ? nullptr : &h->states.p[0];
+            if (source == FLB_CLOUD_SCAN)
+                k_map_scan_world<true><<<(n + 255) / 256, 256, 0, h->stream>>>(src, n, pose, x, h->wc_xyz.p, h->wc_rec.p);
+            else
+                k_map_scan_world<false><<<(n + 255) / 256, 256, 0, h->stream>>>(src, n, pose, x, h->wc_xyz.p, h->wc_rec.p);
+            FLB_CUDA(h, cudaGetLastError());
+        }
+        unsigned* rec = static_cast<unsigned*>(h->pin_out.p);
+        FLB_CUDA(h, cudaMemcpyAsync(rec, h->wc_rec.p, kScanRecWords * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+        if (rec[kScanRecBad]) return fail(h, FLB_ERR_INVALID, "flb_world_cloud: non-finite coordinate");
+        for (int k = 0; k < 3; ++k) {
+            lo[k] = f32_from_order_key(~rec[kScanRecMin + k]);
+            hi[k] = f32_from_order_key(rec[kScanRecMax + k]);
+            // the visual map's coordinate limit (vm_upload_points: |v| <= 5e5, 2^20 voxels of its 0.5 m key)
+            if (lo[k] < -5.0e5f || hi[k] > 5.0e5f) return fail(h, FLB_ERR_INVALID, "flb_world_cloud: coordinate beyond 2^20 visual-map voxels");
+        }
+    }
+    std::memcpy(h->wc_lo, lo, sizeof(lo));
+    std::memcpy(h->wc_hi, hi, sizeof(hi));
+    h->wc_n = n;
+    if (n_out) *n_out = n;
+    return FLB_OK;
+}
+
+int flb_world_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out) {
+    FLB_CHECK_H(h);
+    if (capacity < 0 || (capacity > 0 && !xyz)) return fail(h, FLB_ERR_INVALID, "flb_world_cloud_download: bad arguments");
+    if (h->wc_n < 0) return fail(h, FLB_ERR_STATE, "flb_world_cloud_download: no world cloud (flb_world_cloud first, or it failed)");
+    if (n_out) *n_out = h->wc_n;
+    const int m = std::min(capacity, h->wc_n);
+    if (m > 0) {
+        FLB_CUDA(h, cudaMemcpyAsync(xyz, h->wc_xyz.p, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    }
+    return FLB_OK;
+}
+
 int flb_map_delete_boxes(flb_handle* h, const float* boxes, int nb) {
     FLB_CHECK_H(h);
     if (h->M <= 0) return fail(h, FLB_ERR_STATE, "flb_map_delete_boxes: no map uploaded");
@@ -1628,6 +1722,7 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
                       double pcl_beg_time, double pcl_end_time, const float* pts, int stride, int offset_index, int n_points,
                       float* out_xyz, double* poses_out, int* n_poses_out) {
     FLB_CHECK_H(h);
+    h->undist_n = -1;                 // flb_world_cloud's FLB_CLOUD_UNDISTORTED source is this call's output, or none
     if (!prm || !carry || !v_imu || n_imu < 1 || n_points < 0 || (n_points > 0 && (!pts || !out_xyz)) || stride < 4 ||
         offset_index < 3 || offset_index >= stride)
         return fail(h, FLB_ERR_INVALID, "flb_imu_undistort: bad arguments");
@@ -1708,6 +1803,8 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
         out_xyz[3 * (size_t)i + 1] = po_pts[4 * (size_t)i + 1];
         out_xyz[3 * (size_t)i + 2] = po_pts[4 * (size_t)i + 2];
     }
+    h->undist_pts = d_out;
+    h->undist_n = n_points;
     h->last_pass_valid = false;
     h->last_vio_valid = false;
     return FLB_OK;
@@ -1766,6 +1863,45 @@ int flb_visual_candidates(flb_handle* h, const double Rcw[9], const double Pcw[3
     return vio_inputs_release(h);
 }
 
+// pcl::VoxelGrid of n >= 1 finite points already on the device (xyz, packed): k_bbox -> k_vg_keys -> radix sort ->
+// k_vg_heads -> scan -> k_vg_centroids, enqueued on `stream`, nothing read back.  The centroids go to `out` in ascending
+// leaf index; s.box[0..5] = the box, s.box[6] = PCL's index-overflow flag, s.box[7] = the leaf count.  flb_voxel_grid
+// runs it on the scan slot's scratch, flb_vmap_select_cloud on buffers of its own.
+struct VgScratch {
+    unsigned *keys, *keys_sorted;
+    int *vals, *vals_sorted, *head, *rank, *box;
+};
+static int voxel_grid_dev(flb_handle* h, const float* xyz, int n, float leaf, const VgScratch& s, float* out) {
+    const int init[8] = {0x7fffffff, 0x7fffffff, 0x7fffffff, (int)0x80000000, (int)0x80000000, (int)0x80000000, 0, 0};
+    FLB_CUDA(h, cudaMemcpyAsync(s.box, init, sizeof(init), cudaMemcpyHostToDevice, h->stream));
+    const float inv_leaf = 1.0f / leaf;                              // inverse_leaf_size_ = Array4f::Ones() / leaf_size_
+    const int g = (n + 255) / 256;
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_bbox<<<std::min(g, 4 * std::max(h->num_sms, 1)), 256, 0, h->stream>>>(xyz, n, s.box);
+        k_vg_keys<<<g, 256, 0, h->stream>>>(xyz, n, s.box, inv_leaf, s.keys, s.vals, s.box + 6);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    size_t t1 = 0, t2 = 0;
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t1, s.keys, s.keys_sorted, s.vals, s.vals_sorted, n, 0, 31, h->stream));
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t2, s.head, s.rank, n, h->stream));
+    FLB_CUDA(h, h->cub_tmp.reserve(std::max(t1, t2)));
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, t1, s.keys, s.keys_sorted, s.vals, s.vals_sorted, n, 0, 31, h->stream));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_vg_heads<<<g, 256, 0, h->stream>>>(s.keys_sorted, n, s.head);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, t2, s.head, s.rank, n, h->stream));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_vg_centroids<<<g, 256, 0, h->stream>>>(xyz, s.keys_sorted, s.vals_sorted, s.head, s.rank, n, out, s.box + 7);
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches += 8;
+    }
+    return FLB_OK;
+}
+
 int flb_voxel_grid(flb_handle* h, const float* xyz, int n, int stride, float leaf, float* out_xyz, int capacity, int* n_out) {
     FLB_CHECK_H(h);
     if (n < 0 || (n > 0 && !xyz) || stride < 3 || !(leaf > 0) || !n_out || capacity < 0 || (capacity > 0 && !out_xyz))
@@ -1789,38 +1925,10 @@ int flb_voxel_grid(flb_handle* h, const float* xyz, int n, int stride, float lea
     FLB_CUDA(h, h->dead_before.reserve((size_t)2 * n + 2));      // head flags | ranks
     FLB_CUDA(h, h->map_comb.reserve((size_t)n * 3));             // centroids
     FLB_CUDA(h, h->bbox_dev.reserve(8));
-    int* head = h->dead_before.p;
-    int* rank = h->dead_before.p + n;
-    const int init[8] = {0x7fffffff, 0x7fffffff, 0x7fffffff, (int)0x80000000, (int)0x80000000, (int)0x80000000, 0, 0};
-    FLB_CUDA(h, cudaMemcpyAsync(h->bbox_dev.p, init, sizeof(init), cudaMemcpyHostToDevice, h->stream));
     FLB_CUDA(h, cudaMemcpyAsync(h->scan_raw.p, st, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     FLB_CUDA(h, h->st_scan.mark(h->stream));
-    const float inv_leaf = 1.0f / leaf;                              // inverse_leaf_size_ = Array4f::Ones() / leaf_size_
-    const int g = (n + 255) / 256;
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_bbox<<<std::min(g, 4 * std::max(h->num_sms, 1)), 256, 0, h->stream>>>(h->scan_raw.p, n, h->bbox_dev.p);
-        k_vg_keys<<<g, 256, 0, h->stream>>>(h->scan_raw.p, n, h->bbox_dev.p, inv_leaf, h->skeys.p, h->svals.p, h->bbox_dev.p + 6);
-        FLB_CUDA(h, cudaGetLastError());
-    }
-    size_t t1 = 0, t2 = 0;
-    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t1, h->skeys.p, h->skeys_sorted.p, h->svals.p, h->svals_sorted.p, n, 0, 31, h->stream));
-    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t2, head, rank, n, h->stream));
-    FLB_CUDA(h, h->cub_tmp.reserve(std::max(t1, t2)));
-    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, t1, h->skeys.p, h->skeys_sorted.p, h->svals.p, h->svals_sorted.p, n, 0, 31, h->stream));
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_vg_heads<<<g, 256, 0, h->stream>>>(h->skeys_sorted.p, n, head);
-        FLB_CUDA(h, cudaGetLastError());
-    }
-    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, t2, head, rank, n, h->stream));
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_vg_centroids<<<g, 256, 0, h->stream>>>(h->scan_raw.p, h->skeys_sorted.p, h->svals_sorted.p, head, rank, n, h->map_comb.p,
-                                                  h->bbox_dev.p + 7);
-        FLB_CUDA(h, cudaGetLastError());
-        h->launches += 8;
-    }
+    const VgScratch vs{h->skeys.p, h->skeys_sorted.p, h->svals.p, h->svals_sorted.p, h->dead_before.p, h->dead_before.p + n, h->bbox_dev.p};
+    { int rcv = voxel_grid_dev(h, h->scan_raw.p, n, leaf, vs, h->map_comb.p); if (rcv) return rcv; }
     int tail[2] = {0, 0};
     FLB_CUDA(h, cudaMemcpyAsync(tail, h->bbox_dev.p + 6, sizeof(tail), cudaMemcpyDeviceToHost, h->stream));
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -3224,14 +3332,15 @@ int flb_vmap_reset(flb_handle* h, const flb_vmap_params* p) {
     return FLB_OK;
 }
 
-int flb_vmap_select(flb_handle* h, const double Rcw[9], const double Pcw[3], const float* pg_down, int n, int stride, int* n_selected) {
-    FLB_CHECK_H(h);
-    { int rc = vm_check(h, "flb_vmap_select"); if (rc) return rc; }
-    if (n < 0 || (n > 0 && !pg_down) || stride < 3) return fail(h, FLB_ERR_INVALID, "flb_vmap_select: bad arguments");
+}  // extern "C"
+
+namespace {
+
+// addFromSparseMap once the pose is set: pg_down = n device points, or -- n_dev non-null -- *n_dev (on the device) of at
+// most n.  flb_vmap_select and flb_vmap_select_cloud differ only in how pg_down gets to the device.
+int vm_select_dev(flb_handle* h, const float* pg_down, int n, const int* n_dev, int* n_selected) {
     auto& vm = h->vm;
     const int L = vm.prm.length, border = (vm.prm.halfpatch + 1) * 8;
-    { int rc = vm_set_pose(h, Rcw, Pcw); if (rc) return rc; }
-    { int rc = vm_upload_points(h, pg_down, n, stride); if (rc) return rc; }
     { int rcq = vio_inputs_acquire(h); if (rcq) return rcq; }                 // the current image has landed
     size_t nkeys = 1024;
     while (nkeys < 2 * (size_t)std::max(n, 1)) nkeys <<= 1;
@@ -3248,8 +3357,8 @@ int flb_vmap_select(flb_handle* h, const double Rcw[9], const double Pcw[3], con
         k_vm_clear<<<h->num_sms * 2, 256, 0, h->stream>>>(vm.depth.p, npix, vm.keyset.p, nkeys, vm.cell_best.p, vm.cell_type.p, vm.map_value.p,
                                                           vm.cell_flag.p, L, vm.counters.p);
         if (n > 0)
-            k_vm_scan<<<(n + 255) / 256, 256, 0, h->stream>>>(h->cam, vm.pose.p, vm.pg.p, n, border, vm.keyset.p, vm.key_mask, vm.depth.p,
-                                                              vm.counters.p);
+            k_vm_scan<<<(n + 255) / 256, 256, 0, h->stream>>>(h->cam, vm.pose.p, pg_down, n, n_dev, border, vm.keyset.p, vm.key_mask,
+                                                              vm.depth.p, vm.counters.p);
         const int np = std::max(vm.pts_ub, 1);
         k_vm_candidates<<<(np + 255) / 256, 256, 0, h->stream>>>(h->cam, vm.prm, vm.pose.p, vm.pts.p, vm.counters.p, vm.keyset.p, vm.key_mask,
                                                                  border, vm.cell_best.p, vm.cell_type.p,
@@ -3276,6 +3385,60 @@ int flb_vmap_select(flb_handle* h, const double Rcw[9], const double Pcw[3], con
     return FLB_OK;
 }
 
+// The world cloud's consumers (flb_*_cloud) need one: FLB_ERR_STATE until a flb_world_cloud succeeds.
+int wc_check(flb_handle* h, const char* who) {
+    if (h->wc_n < 0) return fail(h, FLB_ERR_STATE, "%s: no world cloud (flb_world_cloud first, or it failed)", who);
+    return FLB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int flb_vmap_select(flb_handle* h, const double Rcw[9], const double Pcw[3], const float* pg_down, int n, int stride, int* n_selected) {
+    FLB_CHECK_H(h);
+    { int rc = vm_check(h, "flb_vmap_select"); if (rc) return rc; }
+    if (n < 0 || (n > 0 && !pg_down) || stride < 3) return fail(h, FLB_ERR_INVALID, "flb_vmap_select: bad arguments");
+    { int rc = vm_set_pose(h, Rcw, Pcw); if (rc) return rc; }
+    { int rc = vm_upload_points(h, pg_down, n, stride); if (rc) return rc; }
+    return vm_select_dev(h, h->vm.pg.p, n, nullptr, n_selected);
+}
+
+// LidarSelector::detect's addFromSparseMap(img, pg_down) with pg_down = downSizeFilter(pcl_wait_pub) (src/lidar_selection.cpp:
+// 351-353) on the device: flb_voxel_grid's chain on the world cloud into buffers of this call's own (the scan slot is not
+// touched), then the selection with the leaf count left on the device (k_vm_scan runs over the cloud's size as its bound).
+int flb_vmap_select_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], float leaf, int* n_selected) {
+    FLB_CHECK_H(h);
+    { int rc = vm_check(h, "flb_vmap_select_cloud"); if (rc) return rc; }
+    { int rc = wc_check(h, "flb_vmap_select_cloud"); if (rc) return rc; }
+    if (!(leaf > 0)) return fail(h, FLB_ERR_INVALID, "flb_vmap_select_cloud: bad arguments (leaf > 0)");
+    const int n = h->wc_n;
+    if (n > 0) {
+        // PCL's index-overflow test from the bounds flb_world_cloud read (k_vg_keys' float expressions on k_bbox's
+        // box, which equals them): decided here, so the leaf count never has to come back
+        const float inv_leaf = 1.0f / leaf;
+        double cells = 1.0;
+        for (int k = 0; k < 3; ++k) {
+            const float d = (h->wc_hi[k] - h->wc_lo[k]) * inv_leaf;
+            cells *= d < 9.0e18f ? (double)((long long)d + 1) : 9.2e18;
+        }
+        if (cells > 2147483647.0)
+            return fail(h, FLB_ERR_INVALID, "flb_vmap_select_cloud: leaf size too small for the cloud's extent (index overflow, as PCL warns)");
+    }
+    { int rc = vm_set_pose(h, Rcw, Pcw); if (rc) return rc; }
+    if (n == 0) return vm_select_dev(h, h->wc_down.p, 0, nullptr, n_selected);
+    FLB_CUDA(h, h->wc_down.reserve((size_t)n * 3));
+    FLB_CUDA(h, h->wc_keys.reserve(n));
+    FLB_CUDA(h, h->wc_keys_sorted.reserve(n));
+    FLB_CUDA(h, h->wc_vals.reserve(n));
+    FLB_CUDA(h, h->wc_vals_sorted.reserve(n));
+    FLB_CUDA(h, h->wc_heads.reserve((size_t)2 * n));
+    FLB_CUDA(h, h->wc_box.reserve(8));
+    const VgScratch vs{h->wc_keys.p, h->wc_keys_sorted.p, h->wc_vals.p, h->wc_vals_sorted.p, h->wc_heads.p, h->wc_heads.p + n, h->wc_box.p};
+    { int rcv = voxel_grid_dev(h, h->wc_xyz.p, n, leaf, vs, h->wc_down.p); if (rcv) return rcv; }
+    return vm_select_dev(h, h->wc_down.p, n, h->wc_box.p + 7, n_selected);
+}
+
 int flb_vmap_selected(flb_handle* h, int capacity, int* n_out, int* index, int* point, int* search_level, float* error, double* pos,
                       float* patch) {
     FLB_CHECK_H(h);
@@ -3298,15 +3461,14 @@ int flb_vmap_selected(flb_handle* h, int capacity, int* n_out, int* index, int* 
     return FLB_OK;
 }
 
-int flb_vmap_grow(flb_handle* h, const double Rcw[9], const double Pcw[3], const float* pg, int n, int stride, int frame_id) {
-    FLB_CHECK_H(h);
-    { int rc = vm_check(h, "flb_vmap_grow"); if (rc) return rc; }
-    if (n < 0 || (n > 0 && !pg) || stride < 3 || frame_id < 0) return fail(h, FLB_ERR_INVALID, "flb_vmap_grow: bad arguments");
+}  // extern "C"
+
+namespace {
+
+// addSparseMap once the capacity and the pose are set, over n device points pg (flb_vmap_grow / flb_vmap_grow_cloud).
+int vm_grow_dev(flb_handle* h, const float* pg, int n, int frame_id) {
     auto& vm = h->vm;
     const int L = vm.prm.length, border = (vm.prm.halfpatch + 1) * 8;
-    { int rc = vm_ensure_capacity(h, L, L); if (rc) return rc; }
-    { int rc = vm_set_pose(h, Rcw, Pcw); if (rc) return rc; }
-    { int rc = vm_upload_points(h, pg, n, stride); if (rc) return rc; }
     { int rcq = vio_inputs_acquire(h); if (rcq) return rcq; }
     const size_t img_bytes = (size_t)h->img_w * h->img_h;
     {
@@ -3314,10 +3476,10 @@ int flb_vmap_grow(flb_handle* h, const double Rcw[9], const double Pcw[3], const
         k_vm_store_image<<<h->num_sms, 256, 0, h->stream>>>(h->img.p, img_bytes, vm.pool.p, vm.counters.p, vm.free_slots.p, frame_id);
         k_vmap_seed<<<(L + 255) / 256, 256, 0, h->stream>>>(vm.map_value.p, L, vm.cand_key.p);
         if (n > 0)
-            k_vmap_candidates<<<(n + 127) / 128, 128, 0, h->stream>>>(h->cam, vm.pose.p, h->img.p, vm.pg.p, n, vm.prm.grid_size, vm.prm.grid_n_height,
+            k_vmap_candidates<<<(n + 127) / 128, 128, 0, h->stream>>>(h->cam, vm.pose.p, h->img.p, pg, n, vm.prm.grid_size, vm.prm.grid_n_height,
                                                                       border, vm.cand_key.p);
         k_vmap_resolve<<<(L + 255) / 256, 256, 0, h->stream>>>(vm.cand_key.p, L, vm.map_value.p, vm.winner.p);
-        k_vm_materialise<<<1, 1024, 0, h->stream>>>(h->cam, L, vm.pose.p, vm.pg.p, vm.winner.p, vm.map_value.p, vm.scan_tmp.p, vm.pts.p, vm.fts.p,
+        k_vm_materialise<<<1, 1024, 0, h->stream>>>(h->cam, L, vm.pose.p, pg, vm.winner.p, vm.map_value.p, vm.scan_tmp.p, vm.pts.p, vm.fts.p,
                                                     vm.counters.p, vm.free_slots.p, frame_id, (int)vm.pts.cap, (int)vm.fts.cap);
         FLB_CUDA(h, cudaGetLastError());
         h->launches += 4;
@@ -3326,6 +3488,33 @@ int flb_vmap_grow(flb_handle* h, const double Rcw[9], const double Pcw[3], const
     vm.fts_ub += L;
     vm.img_ub += 1;
     return vio_inputs_release(h);
+}
+
+}  // namespace
+
+extern "C" {
+
+int flb_vmap_grow(flb_handle* h, const double Rcw[9], const double Pcw[3], const float* pg, int n, int stride, int frame_id) {
+    FLB_CHECK_H(h);
+    { int rc = vm_check(h, "flb_vmap_grow"); if (rc) return rc; }
+    if (n < 0 || (n > 0 && !pg) || stride < 3 || frame_id < 0) return fail(h, FLB_ERR_INVALID, "flb_vmap_grow: bad arguments");
+    const int L = h->vm.prm.length;
+    { int rc = vm_ensure_capacity(h, L, L); if (rc) return rc; }
+    { int rc = vm_set_pose(h, Rcw, Pcw); if (rc) return rc; }
+    { int rc = vm_upload_points(h, pg, n, stride); if (rc) return rc; }
+    return vm_grow_dev(h, h->vm.pg.p, n, frame_id);
+}
+
+// addSparseMap(img, pcl_wait_pub) (src/lidar_selection.cpp:142-202) over the world cloud on the device.
+int flb_vmap_grow_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], int frame_id) {
+    FLB_CHECK_H(h);
+    { int rc = vm_check(h, "flb_vmap_grow_cloud"); if (rc) return rc; }
+    { int rc = wc_check(h, "flb_vmap_grow_cloud"); if (rc) return rc; }
+    if (frame_id < 0) return fail(h, FLB_ERR_INVALID, "flb_vmap_grow_cloud: bad arguments");
+    const int L = h->vm.prm.length;
+    { int rc = vm_ensure_capacity(h, L, L); if (rc) return rc; }
+    { int rc = vm_set_pose(h, Rcw, Pcw); if (rc) return rc; }
+    return vm_grow_dev(h, h->wc_xyz.p, h->wc_n, frame_id);
 }
 
 int flb_vmap_add_observations(flb_handle* h, const double Rcw[9], const double Pcw[3], int frame_id) {
@@ -3351,20 +3540,22 @@ int flb_vmap_add_observations(flb_handle* h, const double Rcw[9], const double P
     return vio_inputs_release(h);
 }
 
-int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, const float* world_xyz, int n,
-                 int stride, uint8_t* rgb, uint8_t* valid) {
-    FLB_CHECK_H(h);
-    if (!h->cam_set) return fail(h, FLB_ERR_STATE, "flb_colorize: flb_camera_set first");
-    const int W = h->cam.width, H = h->cam.height;
-    if (!bgr || stride_bytes < 3 * W || n < 0 || (n > 0 && (!world_xyz || !rgb || !valid)) || stride < 3)
-        return fail(h, FLB_ERR_INVALID, "flb_colorize: bad arguments");
-    if (n == 0) return FLB_OK;
+}  // extern "C"
+
+namespace {
+
+int colorize_pose(flb_handle* h, const char* who, const double* Rcw, const double* Pcw) {
     auto& vm = h->vm;
     FLB_CUDA(h, vm.pose.reserve(12));
     FLB_CUDA(h, vm.rci.reserve(12));
-    if (!(Rcw && Pcw) && !vm.on) return fail(h, FLB_ERR_STATE, "flb_colorize: no pose given and no flb_vmap_reset (extrinsics)");
-    { int rc = vm_set_pose(h, Rcw, Pcw); if (rc) return rc; }
-    { int rc = vm_upload_points(h, world_xyz, n, stride); if (rc) return rc; }
+    if (!(Rcw && Pcw) && !vm.on) return fail(h, FLB_ERR_STATE, "%s: no pose given and no flb_vmap_reset (extrinsics)", who);
+    return vm_set_pose(h, Rcw, Pcw);
+}
+
+// The colour image upload, the per-point kernel and the download of rgb / valid for n >= 1 device points xyz.
+int colorize_dev(flb_handle* h, const uint8_t* bgr, int stride_bytes, const float* xyz, int n, uint8_t* rgb, uint8_t* valid) {
+    auto& vm = h->vm;
+    const int W = h->cam.width, H = h->cam.height;
     const size_t img_bytes = (size_t)W * H * 3;
     FLB_CUDA(h, h->x_rowmask.reserve(img_bytes + (size_t)n * 4));     // colour image | rgb | valid
     unsigned char* d_img = h->x_rowmask.p;
@@ -3378,7 +3569,7 @@ int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const 
     FLB_CUDA(h, h->st_img.mark(h->stream));
     {
         LaunchScope ls(h, FAM_OTHER);
-        k_vm_colorize<<<(n + 255) / 256, 256, 0, h->stream>>>(h->cam, vm.pose.p, d_img, vm.pg.p, n, d_rgb, d_val);
+        k_vm_colorize<<<(n + 255) / 256, 256, 0, h->stream>>>(h->cam, vm.pose.p, d_img, xyz, n, d_rgb, d_val);
         FLB_CUDA(h, cudaGetLastError());
     }
     FLB_CUDA(h, h->pin_out.reserve((size_t)n * 4));
@@ -3388,6 +3579,36 @@ int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const 
     std::memcpy(valid, static_cast<unsigned char*>(h->pin_out.p) + (size_t)n * 3, n);
     h->last_pass_valid = false;                       // the row-mask export buffer was reused
     return FLB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, const float* world_xyz, int n,
+                 int stride, uint8_t* rgb, uint8_t* valid) {
+    FLB_CHECK_H(h);
+    if (!h->cam_set) return fail(h, FLB_ERR_STATE, "flb_colorize: flb_camera_set first");
+    const int W = h->cam.width;
+    if (!bgr || stride_bytes < 3 * W || n < 0 || (n > 0 && (!world_xyz || !rgb || !valid)) || stride < 3)
+        return fail(h, FLB_ERR_INVALID, "flb_colorize: bad arguments");
+    if (n == 0) return FLB_OK;
+    { int rc = colorize_pose(h, "flb_colorize", Rcw, Pcw); if (rc) return rc; }
+    { int rc = vm_upload_points(h, world_xyz, n, stride); if (rc) return rc; }
+    return colorize_dev(h, bgr, stride_bytes, h->vm.pg.p, n, rgb, valid);
+}
+
+// publish_frame_world_rgb of pcl_wait_pub (src/laserMapping.cpp:710-745) with the world cloud on the device.
+int flb_colorize_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, uint8_t* rgb,
+                       uint8_t* valid) {
+    FLB_CHECK_H(h);
+    if (!h->cam_set) return fail(h, FLB_ERR_STATE, "flb_colorize_cloud: flb_camera_set first");
+    { int rc = wc_check(h, "flb_colorize_cloud"); if (rc) return rc; }
+    const int n = h->wc_n;
+    if (!bgr || stride_bytes < 3 * h->cam.width || (n > 0 && (!rgb || !valid))) return fail(h, FLB_ERR_INVALID, "flb_colorize_cloud: bad arguments");
+    if (n == 0) return FLB_OK;
+    { int rc = colorize_pose(h, "flb_colorize_cloud", Rcw, Pcw); if (rc) return rc; }
+    return colorize_dev(h, bgr, stride_bytes, h->wc_xyz.p, n, rgb, valid);
 }
 
 int flb_vmap_counts(flb_handle* h, int* points, int* features, int* images, int* selected, int* last_added) {

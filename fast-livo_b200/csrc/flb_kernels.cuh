@@ -240,10 +240,14 @@ __global__ void k_bbox(const float* __restrict__ xyz, int n, int* __restrict__ b
 // device version sorts (existing + new) points by voxel and lets one thread replay that sequential
 // rule over each voxel's handful of points.
 // ---------------------------------------------------------------------------------------
-// map_incremental from the uploaded scan (flb_map_add_scan): one thread per point of the ordered scan writes
+// map_incremental from the uploaded scan (flb_map_add_scan) and pcl_wait_pub (flb_world_cloud, RGBpointBodyToWorld
+// has pointBodyToWorld's op order): one thread per point of the ordered scan writes
 // pointBodyToWorld of it to the caller's index in packed xyz, and the block folds its points into rec (kScanRec*: the
 // per-axis max and ~min order keys, the non-finite flag; zeroed before the launch) with one atomic maximum per word.
 // The pose is `pose`, or -- x non-null -- the device state's rot / pos with pose's extrinsic.
+// kScanOrder = false (flb_world_cloud of flb_imu_undistort's output): the source is {x, y, z, time offset} in the
+// caller's order already, so point i goes to index i.
+template <bool kScanOrder = true>
 __global__ void __launch_bounds__(256) k_map_scan_world(const float4* __restrict__ scan, int n, LioPose pose, const State18* __restrict__ x,
                                                         float* __restrict__ out, unsigned* __restrict__ rec) {
     __shared__ LioPose s_pose;
@@ -260,7 +264,8 @@ __global__ void __launch_bounds__(256) k_map_scan_world(const float4* __restrict
     unsigned v[kScanRecBad + 1] = {0, 0, 0, 0, 0, 0, 0};   // 0: the identity of the maximum for every word
     if (i < n) {
         float pw[3];
-        const int oi = map_scan_point(s_pose, scan[i], pw);
+        const int si = map_scan_point(s_pose, scan[i], pw);
+        const int oi = kScanOrder ? si : i;
 #pragma unroll
         for (int k = 0; k < 3; ++k) out[3 * (size_t)oi + k] = pw[k];
         if (finite3(pw)) {

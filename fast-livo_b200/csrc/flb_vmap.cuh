@@ -69,12 +69,13 @@ __device__ __forceinline__ unsigned vm_hash(unsigned long long k) {
 
 // First loop (:378-418): every voxel-filtered scan point marks its 0.5 m voxel and writes its depth into the pixel
 // it projects to (the LAST point of the cloud wins a pixel: maximum over {index + 1 : depth bits}).
-__global__ void k_vm_scan(CamModel cam, const double* __restrict__ pose12, const float* __restrict__ pg_down, int n, int border,
-                          unsigned long long* __restrict__ keyset, unsigned key_mask, unsigned long long* __restrict__ depth,
+// n_dev non-null (flb_vmap_select_cloud: the leaf count of the device voxel filter): *n_dev points, n is its bound.
+__global__ void k_vm_scan(CamModel cam, const double* __restrict__ pose12, const float* __restrict__ pg_down, int n, const int* __restrict__ n_dev,
+                          int border, unsigned long long* __restrict__ keyset, unsigned key_mask, unsigned long long* __restrict__ depth,
                           const int* __restrict__ counters) {
     if (counters[VM_N_POINTS] <= 0) return;                                       // :348
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+    if (i >= n || (n_dev && i >= *n_dev)) return;
     const float p[3] = {pg_down[3 * (size_t)i], pg_down[3 * (size_t)i + 1], pg_down[3 * (size_t)i + 2]};
     const unsigned long long key = vm_scan_key(p);
     unsigned slot = vm_hash(key) & key_mask;

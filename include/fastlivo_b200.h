@@ -358,6 +358,38 @@ int flb_vmap_add_observations(flb_handle* h, const double Rcw[9], const double P
  * is the input order.  Rcw / Pcw NULL: from the device state (after flb_vmap_reset).  Blocking. */
 int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, const float* world_xyz, int n,
                  int stride_floats, uint8_t* rgb, uint8_t* valid);
+
+/* ---- the frame's world cloud on the device (pcl_wait_pub) -------------------------------------------------------
+ * pcl_wait_pub (src/laserMapping.cpp:1763-1772) is the source cloud in the world frame; its three readers are the visual
+ * map's select and grow (LidarSelector::detect(img, pcl_wait_pub), :1345) and publish_frame_world_rgb (:710-745).
+ * flb_world_cloud builds it on the device and the *_cloud calls read it there: no read-back of the state, no host
+ * transform, no host voxel filter and no upload of the cloud. */
+#define FLB_CLOUD_SCAN        0   /* feats_down_body: the scan last uploaded (dense_map_en = 0) */
+#define FLB_CLOUD_UNDISTORTED 1   /* feats_undistort: the output of the last flb_imu_undistort (dense_map_en = 1) */
+/* The source cloud, in the caller's original order, transformed by RGBpointBodyToWorld (:303-315, pointBodyToWorld's op
+ * order; double math, float store) at (R, p) with prm->R_LI / prm->t_LI, or at the device state x when R == p == NULL
+ * (stream order: call it after the LIO update, after flb_map_add_scan).  IKFoM callers pass R = rot, p = pos and the
+ * offset_R_L_I / offset_T_L_I extrinsic.  The library keeps the cloud until the next call; it is a copy, so later scan
+ * uploads and flb_imu_undistort calls do not change it.  Blocking (one 32-byte read).  *n_out (may be NULL) = points.
+ * On any error no cloud is held, and every *_cloud call returns FLB_ERR_STATE until the next successful call.
+ *   FLB_ERR_STATE: no source (no scan, the scan slot used as scratch by flb_voxel_grid, no flb_imu_undistort since
+ *   creation or since a failed one), no pose given and no device state, FLB_CLOUD_SCAN after flb_comm_init /
+ *   flb_p2p_attach (each rank holds only its shard of the scan).
+ *   FLB_ERR_INVALID: prm == NULL, a bad source, exactly one of R / p NULL, a transformed point that is not finite or
+ *   whose |coordinate| exceeds 5e5 (the visual map's limit, as flb_vmap_select / flb_vmap_grow / flb_colorize check). */
+int flb_world_cloud(flb_handle* h, const struct flb_lio_params* prm, const double R[9], const double p[3], int source, int* n_out);
+/* publish_frame_world / the PCD save: up to `capacity` points of the world cloud, xyz floats (blocking). */
+int flb_world_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out);
+/* flb_vmap_select / flb_vmap_grow / flb_colorize with pg = the world cloud: the same pose, enqueue and blocking rules and
+ * byte-identical results to those calls on the host-transformed cloud.  flb_vmap_select_cloud applies downSizeFilter
+ * (pcl::VoxelGrid with `leaf`, 0.2 in the reference: src/lidar_selection.cpp:7, :351-353; flb_voxel_grid's result) on
+ * the device first, in buffers of its own (the scan slot is untouched); the leaf count stays on the device, so with
+ * n_selected == NULL it is enqueue-only.  FLB_ERR_INVALID for a leaf too small for the cloud's extent (PCL's
+ * index-overflow case, as in flb_voxel_grid).  flb_colorize_cloud writes world-cloud-size entries to rgb (x 3) / valid. */
+int flb_vmap_select_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], float leaf, int* n_selected);
+int flb_vmap_grow_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], int frame_id);
+int flb_colorize_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, uint8_t* rgb,
+                       uint8_t* valid);
 /* Gives back what the reference frees (opt-in; enqueue-only, no host synchronisation).  A Feature is owned by
  * Point::obs_ alone, so it dies when addObservation evicts it (deleteFeatureRef(getFurthestViewObs),
  * src/lidar_selection.cpp:946-950); its keyframe image (Feature::img, :183, :957) dies with the last Feature that refers
