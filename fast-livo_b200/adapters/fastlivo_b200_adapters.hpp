@@ -14,6 +14,9 @@
 //        LidarSelector::ComputeJ(cv::Mat)  src/lidar_selection.cpp:967-983
 //   flb::undistort_pcl(h, prm, carry, v_imu, pcl_beg_time, pcl_end_time, state_inout, pcl_out)   replaces
 //        ImuProcess::UndistortPcl from src/IMU_Processing.cpp:655 on (propagation + undistortion)
+//   flb::undistort_pcl_on_device(h, prm, carry, v_imu, pcl_beg_time, pcl_end_time, state_inout, pcl_in) +
+//   flb::downsample_scan(h, filter_size_surf_min)   replace UndistortPcl + downSizeFilterSurf (src/laserMapping.cpp:
+//        1398-1399) + upload_scan: feats_undistort stays on the device and becomes the scan there
 //   flb::map_incremental(h, lio_prm, filter_size_map_min)  /  flb::map_incremental(h, lio_prm, R, p, filter_size_map_min)   replace
 //        map_incremental()  src/laserMapping.cpp:692-706  (the uploaded scan into the map, no host transform)
 //
@@ -293,9 +296,11 @@ inline flb_imu_params make_imu_params(const Vec3& cov_gyr, const Vec3& cov_acc, 
     return p;
 }
 
+namespace detail {
+// out == nullptr: the compensated points stay on the device
 template <class ImuDeque, class StatesGroup, class PointCloud>
-inline void undistort_pcl(flb_handle* h, const flb_imu_params& prm, flb_imu_carry& carry, const ImuDeque& v_imu,
-                          double pcl_beg_time, double pcl_end_time, StatesGroup& state_inout, PointCloud& pcl_out) {
+inline void undistort(flb_handle* h, const flb_imu_params& prm, flb_imu_carry& carry, const ImuDeque& v_imu, double pcl_beg_time,
+                      double pcl_end_time, StatesGroup& state_inout, const PointCloud& pcl, float* out) {
     std::vector<flb_imu_sample> s;
     s.reserve(v_imu.size());
     for (const auto& m : v_imu) {
@@ -308,20 +313,44 @@ inline void undistort_pcl(flb_handle* h, const flb_imu_params& prm, flb_imu_carr
     flb_state18 x{};
     to_abi(state_inout, x);
     check(h, flb_state_upload(h, &x, &x));
-    static_assert(sizeof(pcl_out.points[0]) % sizeof(float) == 0, "point type must be float-packed");
-    const int stride = (int)(sizeof(pcl_out.points[0]) / sizeof(float));
-    const int n = (int)pcl_out.points.size();
-    const int off = n ? (int)(&pcl_out.points[0].curvature - &pcl_out.points[0].x) : 3;
-    std::vector<float> out((size_t)n * 3 + 1);
+    static_assert(sizeof(pcl.points[0]) % sizeof(float) == 0, "point type must be float-packed");
+    const int stride = (int)(sizeof(pcl.points[0]) / sizeof(float));
+    const int n = (int)pcl.points.size();
+    const int off = n ? (int)(&pcl.points[0].curvature - &pcl.points[0].x) : 3;
     check(h, flb_imu_undistort(h, &prm, &carry, s.data(), (int)s.size(), pcl_beg_time, pcl_end_time,
-                               n ? &pcl_out.points[0].x : nullptr, n ? stride : 4, off, n, out.data(), nullptr, nullptr));
+                               n ? &pcl.points[0].x : nullptr, n ? stride : 4, off, n, out, nullptr, nullptr));
+    check(h, flb_state_download(h, &x, nullptr, nullptr));
+    from_abi(x, state_inout);
+}
+}  // namespace detail
+
+template <class ImuDeque, class StatesGroup, class PointCloud>
+inline void undistort_pcl(flb_handle* h, const flb_imu_params& prm, flb_imu_carry& carry, const ImuDeque& v_imu,
+                          double pcl_beg_time, double pcl_end_time, StatesGroup& state_inout, PointCloud& pcl_out) {
+    const int n = (int)pcl_out.points.size();
+    std::vector<float> out((size_t)n * 3 + 1);
+    detail::undistort(h, prm, carry, v_imu, pcl_beg_time, pcl_end_time, state_inout, pcl_out, out.data());
     for (int i = 0; i < n; ++i) {
         pcl_out.points[i].x = out[3 * (size_t)i];
         pcl_out.points[i].y = out[3 * (size_t)i + 1];
         pcl_out.points[i].z = out[3 * (size_t)i + 2];
     }
-    check(h, flb_state_download(h, &x, nullptr, nullptr));
-    from_abi(x, state_inout);
+}
+
+// The same propagation and undistortion, with pcl_in left as it is: feats_undistort exists only on the device, where
+// downsample_scan turns it into this frame's scan (and flb_world_cloud(FLB_CLOUD_UNDISTORTED) reads it).
+template <class ImuDeque, class StatesGroup, class PointCloud>
+inline void undistort_pcl_on_device(flb_handle* h, const flb_imu_params& prm, flb_imu_carry& carry, const ImuDeque& v_imu,
+                                    double pcl_beg_time, double pcl_end_time, StatesGroup& state_inout, const PointCloud& pcl_in) {
+    detail::undistort(h, prm, carry, v_imu, pcl_beg_time, pcl_end_time, state_inout, pcl_in, nullptr);
+}
+
+// downSizeFilterSurf.setInputCloud(feats_undistort); downSizeFilterSurf.filter(*feats_down_body); then upload_scan
+// (src/laserMapping.cpp:1398-1399), all on the device.  Returns feats_down_size (:1400).
+inline int downsample_scan(flb_handle* h, float filter_size_surf_min) {
+    int n = 0;
+    check(h, flb_scan_from_undistorted(h, filter_size_surf_min, &n));
+    return n;
 }
 
 }  // namespace flb

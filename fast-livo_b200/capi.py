@@ -166,7 +166,7 @@ CLOUD_SCAN, CLOUD_UNDISTORTED = 0, 1       # flb_world_cloud sources (FLB_CLOUD_
 
 # every symbol include/fastlivo_b200.h declares (checked by the CPU-only test tier)
 SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "flb_set_stream", "flb_synchronize", "flb_host_alloc", "flb_host_free",
-           "flb_map_upload", "flb_map_add_points", "flb_map_add_scan", "flb_map_delete_boxes", "flb_map_size", "flb_map_download", "flb_scan_upload", "flb_knn", "flb_lio_pass", "flb_lio_export", "flb_lio_update", "flb_lio_update_ikfom",
+           "flb_map_upload", "flb_map_add_points", "flb_map_add_scan", "flb_map_delete_boxes", "flb_map_size", "flb_map_download", "flb_scan_upload", "flb_scan_from_undistorted", "flb_map_upload_scan", "flb_knn", "flb_lio_pass", "flb_lio_export", "flb_lio_update", "flb_lio_update_ikfom",
            "flb_image_upload", "flb_patches_upload", "flb_camera_set", "flb_vio_pass", "flb_vio_export",
            "flb_vio_update", "flb_state_upload", "flb_state_download", "flb_lio_update_enqueue",
            "flb_vio_update_enqueue", "flb_state_reset_enqueue", "flb_state_set_prior_enqueue", "flb_profile_start", "flb_profile_stop",
@@ -217,6 +217,8 @@ def lib():
         L.flb_host_free.argtypes = [vp, vp]
         L.flb_map_upload.argtypes = [vp, vp, C.c_int, C.c_int]
         L.flb_scan_upload.argtypes = [vp, vp, C.c_int, C.c_int]
+        L.flb_scan_from_undistorted.argtypes = [vp, C.c_float, C.POINTER(C.c_int)]
+        L.flb_map_upload_scan.argtypes = [vp]
         L.flb_map_add_points.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float]
         L.flb_map_add_scan.argtypes = [vp, C.POINTER(LioParams), vp, vp, C.c_float]
         L.flb_map_delete_boxes.argtypes = [vp, vp, C.c_int]
@@ -402,6 +404,19 @@ class Handle:
         a = np.ascontiguousarray(body_xyz, np.float32)
         self._ck(self.L.flb_scan_upload(self.h, _p(a), a.shape[0], a.shape[1] if a.ndim == 2 else 3))
         self.N = a.shape[0]
+
+    def scan_from_undistorted(self, leaf):
+        """flb_scan_from_undistorted: the scan = the voxel filter (leaf) of the last flb_imu_undistort output, on the
+        device; returns feats_down_size."""
+        n = C.c_int()
+        self._ck(self.L.flb_scan_from_undistorted(self.h, C.c_float(leaf), C.byref(n)))
+        self.N = n.value
+        return n.value
+
+    def map_upload_scan(self):
+        """flb_map_upload_scan: the map = the current scan's points in the caller's order (the first frame's Build)."""
+        self._ck(self.L.flb_map_upload_scan(self.h))
+        self.M = self.L.flb_map_size(self.h)
 
     def debug_set_scan_sort(self, mode):
         """0 automatic, 1 one-block ordering kernel, 2 device-wide sort (test aid)."""
@@ -700,19 +715,20 @@ class Handle:
         return out
 
     # ---- IMU propagation + undistortion (row f3)
-    def imu_undistort(self, prm: ImuParams, carry: ImuCarry, v_imu, pcl_beg_time, pcl_end_time, pts, offset_index=3):
+    def imu_undistort(self, prm: ImuParams, carry: ImuCarry, v_imu, pcl_beg_time, pcl_end_time, pts, offset_index=3, download=True):
         """flb_imu_undistort on the device state.  v_imu (K,7) [t, gyr, acc]; pts (n, stride) float32 with x,y,z
         first and the time offset (ms) at column offset_index.  Returns (xyz (n,3) float32, IMUpose (n_poses,22));
-        carry is updated in place, the device state is propagated in place."""
+        carry is updated in place, the device state is propagated in place.  download=False: out_xyz = NULL (the points
+        stay on the device for scan_from_undistorted / world_cloud) and xyz is None."""
         v = np.ascontiguousarray(v_imu, np.float64)
         pts = np.ascontiguousarray(pts, np.float32)
         n = pts.shape[0]
-        out = np.zeros((n, 3), np.float32)
+        out = np.zeros((n, 3), np.float32) if download else None
         poses = np.zeros((len(v), 22), np.float64)
         npo = C.c_int()
         self._ck(self.L.flb_imu_undistort(self.h, C.byref(prm), C.byref(carry), v.ctypes.data_as(C.c_void_p), len(v),
                                           float(pcl_beg_time), float(pcl_end_time), pts.ctypes.data_as(C.c_void_p),
-                                          pts.shape[1] if n else 4, offset_index, n, out.ctypes.data_as(C.c_void_p),
+                                          pts.shape[1] if n else 4, offset_index, n, _p(out),
                                           poses.ctypes.data_as(C.c_void_p), C.byref(npo)))
         return out, poses[:npo.value]
 

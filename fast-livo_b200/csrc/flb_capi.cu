@@ -135,6 +135,10 @@ struct NcclApi {
 NcclApi g_nccl;
 constexpr int kNcclInt32 = 2, kNcclFloat32 = 7, kNcclFloat64 = 8, kNcclSum = 0, kNcclMax = 2;  // ncclDataType_t / ncclRedOp_t values (nccl.h)
 
+// flb_scan_from_undistorted's record, read back in one copy: k_cloud_pack's record of the input, k_cloud_bounds' of the
+// centroids, voxel_grid_dev's box (box[6] PCL's overflow flag, box[7] the leaf count)
+enum { kSfRecInput = 0, kSfRecCentroids = kScanRecWords, kSfRecBox = 2 * kScanRecWords, kSfRecWords = 2 * kScanRecWords + 8 };
+
 }  // namespace
 
 struct flb_handle {
@@ -252,6 +256,11 @@ struct flb_handle {
     DevBuf<float> wc_down;
     DevBuf<unsigned> wc_keys, wc_keys_sorted;
     DevBuf<int> wc_vals, wc_vals_sorted, wc_heads, wc_box;   // heads: head flags | ranks; box: k_bbox box | overflow | count
+    // flb_scan_from_undistorted: downSizeFilterSurf of the undistortion output (packed input, centroids) and its scratch;
+    // the scan slot's scratch stays untouched.  sf_rec: input record | centroid record (kScanRec*) | VgScratch box (kSfRec*)
+    DevBuf<float> sf_xyz, sf_down;
+    DevBuf<unsigned> sf_keys, sf_keys_sorted, sf_rec;
+    DevBuf<int> sf_vals, sf_vals_sorted, sf_heads;
     DevBuf<unsigned long long> vm_key;   // flb_visual_candidates: per-cell {score, ~index}
     DevBuf<float> vm_val, vm_pts;
     DevBuf<int> vm_win;
@@ -910,7 +919,7 @@ void fill_vio_report(const VioCtrl& c, flb_vio_report* rep) {
 }  // namespace
 
 template <int kScanSortBlock, int ITEMS>
-static int launch_scan_sort_block(flb_handle* h, cudaStream_t ss, int N, const float lo[3], float inv_cell) {
+static int launch_scan_sort_block(flb_handle* h, cudaStream_t ss, const float* xyz, int N, const float lo[3], float inv_cell) {
     using Sort = cub::BlockRadixSort<unsigned, kScanSortBlock, ITEMS, int, 6>;
     const size_t smem = std::max(sizeof(typename Sort::TempStorage), (size_t)kScanSortBlock * ITEMS * sizeof(unsigned));
     bool& attr_set = h->sort_attr_set[ITEMS == 17 ? 0 : (ITEMS == 33 ? 1 : 2)];      // per handle: the attribute is per device
@@ -918,7 +927,7 @@ static int launch_scan_sort_block(flb_handle* h, cudaStream_t ss, int N, const f
         FLB_CUDA(h, cudaFuncSetAttribute(k_scan_sort_block<kScanSortBlock, ITEMS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
-    k_scan_sort_block<kScanSortBlock, ITEMS><<<1, kScanSortBlock, smem, ss>>>(h->scan_raw.p, N, lo[0], lo[1], lo[2], inv_cell, h->scan_alt.p, h->sel_alt.p,
+    k_scan_sort_block<kScanSortBlock, ITEMS><<<1, kScanSortBlock, smem, ss>>>(xyz, N, lo[0], lo[1], lo[2], inv_cell, h->scan_alt.p, h->sel_alt.p,
                                                              h->plane_ok_alt.p);
     FLB_CUDA(h, cudaGetLastError());
     return FLB_OK;
@@ -1008,6 +1017,8 @@ int flb_destroy(flb_handle* h) {
     h->add_xyz.release(); h->add_rec.release();
     h->wc_xyz.release(); h->wc_rec.release(); h->wc_down.release(); h->wc_keys.release(); h->wc_keys_sorted.release();
     h->wc_vals.release(); h->wc_vals_sorted.release(); h->wc_heads.release(); h->wc_box.release();
+    h->sf_keys.release(); h->sf_keys_sorted.release(); h->sf_rec.release(); h->sf_vals.release(); h->sf_vals_sorted.release();
+    h->sf_heads.release(); h->sf_xyz.release();
     h->cell_table.release(); h->cell_keys.release(); h->cell_keys_alt.release();
     h->map_pts_alt.release(); h->cell_start_alt.release(); h->map_raw_alt.release(); h->dead.release(); h->ins.release();
     h->dead_before.release(); h->merge_counts.release(); h->bbox_dev.release();
@@ -1022,7 +1033,7 @@ int flb_destroy(flb_handle* h) {
     for (int k = 0; k < 2; ++k) { h->pin_res[k].release(); if (h->ev_res[k]) cudaEventDestroy(h->ev_res[k]); }
     cudaStreamSynchronize(h->copy_stream);
     cudaStreamSynchronize(h->scan_stream);
-    h->scan_alt.release(); h->plane_alt.release(); h->sel_alt.release(); h->plane_ok_alt.release();
+    h->scan_alt.release(); h->plane_alt.release(); h->sel_alt.release(); h->plane_ok_alt.release(); h->sf_down.release();
     h->img_alt.release(); h->patch_pos_alt.release(); h->patch_ref_alt.release(); h->patch_level_alt.release();
     for (int k = 0; k < 2; ++k) {
         if (h->img_slot.free_ev[k]) cudaEventDestroy(h->img_slot.free_ev[k]);
@@ -1723,7 +1734,7 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
                       float* out_xyz, double* poses_out, int* n_poses_out) {
     FLB_CHECK_H(h);
     h->undist_n = -1;                 // flb_world_cloud's FLB_CLOUD_UNDISTORTED source is this call's output, or none
-    if (!prm || !carry || !v_imu || n_imu < 1 || n_points < 0 || (n_points > 0 && (!pts || !out_xyz)) || stride < 4 ||
+    if (!prm || !carry || !v_imu || n_imu < 1 || n_points < 0 || (n_points > 0 && !pts) || stride < 4 ||
         offset_index < 3 || offset_index >= stride)
         return fail(h, FLB_ERR_INVALID, "flb_imu_undistort: bad arguments");
     if (!h->state_valid) return fail(h, FLB_ERR_STATE, "flb_imu_undistort: no device state (flb_state_upload)");
@@ -1784,13 +1795,14 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
         FLB_CUDA(h, cudaGetLastError());
         h->launches += 2;
     }
-    // results: carry, aux (n_poses), poses, points
+    // results: carry, aux (n_poses), poses, points (out_xyz == NULL: the points stay on the device only, for
+    // flb_scan_from_undistorted / flb_world_cloud)
     const size_t out_bytes = (7 + 16 + (size_t)n_imu * 22) * sizeof(double) + n1 * 4 * sizeof(float);
     FLB_CUDA(h, h->pin_out.reserve(out_bytes));
     char* po = static_cast<char*>(h->pin_out.p);
     FLB_CUDA(h, cudaMemcpyAsync(po, h->imu_buf.p + off_carry, (7 + 16 + (size_t)n_imu * 22) * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     float* po_pts = reinterpret_cast<float*>(po + (7 + 16 + (size_t)n_imu * 22) * sizeof(double));
-    if (n_points > 0)
+    if (n_points > 0 && out_xyz)
         FLB_CUDA(h, cudaMemcpyAsync(po_pts, d_out, (size_t)n_points * 4 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
     std::memcpy(carry, po, sizeof(flb_imu_carry));
@@ -1798,7 +1810,7 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
     std::memcpy(&aux, po + 7 * sizeof(double), sizeof(aux));
     if (n_poses_out) *n_poses_out = aux.n_poses;
     if (poses_out) std::memcpy(poses_out, po + (7 + 16) * sizeof(double), (size_t)aux.n_poses * 22 * sizeof(double));
-    for (int i = 0; i < n_points; ++i) {
+    for (int i = 0; out_xyz && i < n_points; ++i) {
         out_xyz[3 * (size_t)i] = po_pts[4 * (size_t)i];
         out_xyz[3 * (size_t)i + 1] = po_pts[4 * (size_t)i + 1];
         out_xyz[3 * (size_t)i + 2] = po_pts[4 * (size_t)i + 2];
@@ -1945,6 +1957,93 @@ int flb_voxel_grid(flb_handle* h, const float* xyz, int n, int stride, float lea
     return FLB_OK;
 }
 
+// The device half of flb_scan_upload, shared with flb_scan_from_undistorted: N finite packed points at xyz (on the
+// device, complete before anything enqueued on `scan_stream` from here on runs), lo = their per-axis minimum.  Orders
+// them into the idle set of the double-buffered scan, resets its per-point caches and swaps it in.
+// The ordering runs on `scan_stream` into the slot that is NOT being read: updates of the previous frame still queued or
+// running on `stream` keep their scan, and -- because the persistent kernels leave one SM free and the ordering is one
+// block (k_scan_sort_block) -- this frame's upload overlaps them instead of queueing behind them.
+static int scan_install_dev(flb_handle* h, const float* xyz, int N, const float lo[3]) {
+    const size_t n1 = (size_t)std::max(N, 1);
+    const int cur = h->scan_slot, alt = cur ^ 1;
+    cudaStream_t ss = h->scan_stream;
+    FLB_CUDA(h, cudaEventRecord(h->ev_scan_free[cur], h->stream));     // all readers of the current slot are enqueued before this
+    h->scan_free_valid[cur] = true;
+    if (h->scan_free_valid[alt]) FLB_CUDA(h, cudaStreamWaitEvent(ss, h->ev_scan_free[alt], 0));
+    FLB_CUDA(h, h->scan_alt.reserve(n1));
+    FLB_CUDA(h, h->sel_alt.reserve(n1));
+    FLB_CUDA(h, h->plane_ok_alt.reserve(n1));
+    FLB_CUDA(h, h->plane_alt.reserve(n1));
+    const size_t nb = (n1 + kLioBlock - 1) / kLioBlock;
+    FLB_CUDA(h, h->partials.reserve(std::max<size_t>(nb * lio_packed(12), h->partials.cap)));
+    bool flags_done = false;
+    if (N > 0) {
+        // Morton order in the body frame (cell = twice the map grid's cell): spatially coherent warps at any pose
+        const float inv_cell = 0.5f / (float)h->cfg.cell_size;
+        // One-block ordering vs keys + device-wide radix sort + gather (identical order).  Measured on an idle H100
+        // (profiles/scan_upload_probe.py, copy included): 8 k points 42 vs 77 us, 16 k 100 vs 89, 24 k 129 vs 99 -- but the
+        // one-block kernel runs on the SM the persistent kernels leave free, so when an update is still running on
+        // `stream` (a pipelined caller) it costs nothing, while the device-wide kernels would queue behind the update.
+        // So: one block up to 16 896 points always, up to 25 600 when `stream` is busy; FLB_BLOCK_SORT=0 / 2 or
+        // flb_debug_set_scan_sort force the device-wide / one-block path.
+        static const int env_block_sort = [] { const char* e = getenv("FLB_BLOCK_SORT"); return e ? atoi(e) : 1; }();
+        const int mode = h->scan_sort_mode ? h->scan_sort_mode : (env_block_sort == 0 ? 2 : (env_block_sort == 2 ? 1 : 0));
+        bool use_block = N <= 1024 * 25 && mode != 2;
+        if (use_block && mode == 0 && N > 512 * 33) {
+            const cudaError_t q = cudaStreamQuery(h->stream);
+            (void)cudaGetLastError();
+            use_block = (q == cudaErrorNotReady);
+        }
+        if (use_block) {
+            LaunchScope ls(h, FAM_OTHER);
+            int rcs = N <= 512 * 17   ? launch_scan_sort_block<512, 17>(h, ss, xyz, N, lo, inv_cell)
+                      : N <= 512 * 33 ? launch_scan_sort_block<512, 33>(h, ss, xyz, N, lo, inv_cell)
+                                      : launch_scan_sort_block<1024, 25>(h, ss, xyz, N, lo, inv_cell);
+            if (rcs) return rcs;
+            flags_done = true;
+        } else {
+            FLB_CUDA(h, h->skeys.reserve(n1));
+            FLB_CUDA(h, h->skeys_sorted.reserve(n1));
+            FLB_CUDA(h, h->svals.reserve(n1));
+            FLB_CUDA(h, h->svals_sorted.reserve(n1));
+            const int g = (N + 255) / 256;
+            {
+                LaunchScope ls(h, FAM_OTHER);
+                k_scan_keys<<<g, 256, 0, ss>>>(xyz, N, lo[0], lo[1], lo[2], inv_cell, h->skeys.p, h->svals.p);
+                FLB_CUDA(h, cudaGetLastError());
+            }
+            size_t tmp_bytes = 0;
+            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, h->skeys.p, h->skeys_sorted.p, h->svals.p,
+                                                        h->svals_sorted.p, N, 0, 24, ss));
+            FLB_CUDA(h, h->scan_cub_tmp.reserve(tmp_bytes));
+            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->scan_cub_tmp.p, tmp_bytes, h->skeys.p, h->skeys_sorted.p, h->svals.p,
+                                                        h->svals_sorted.p, N, 0, 24, ss));
+            h->launches += 3;
+            {
+                LaunchScope ls(h, FAM_OTHER);
+                k_scan_gather<<<g, 256, 0, ss>>>(xyz, N, h->svals_sorted.p, h->scan_alt.p);
+                FLB_CUDA(h, cudaGetLastError());
+            }
+        }
+    }
+    if (!flags_done) {
+        // point_selected_surf.resize(N, true) (src/laserMapping.cpp:1469)
+        FLB_CUDA(h, cudaMemsetAsync(h->sel_alt.p, 1, n1, ss));
+        FLB_CUDA(h, cudaMemsetAsync(h->plane_ok_alt.p, 0, n1, ss));
+    }
+    FLB_CUDA(h, cudaEventRecord(h->ev_scan_ready, ss));
+    FLB_CUDA(h, cudaStreamWaitEvent(h->stream, h->ev_scan_ready, 0));
+    std::swap(h->scan, h->scan_alt);
+    std::swap(h->sel, h->sel_alt);
+    std::swap(h->plane_ok, h->plane_ok_alt);
+    std::swap(h->plane, h->plane_alt);
+    h->scan_slot = alt;
+    h->N = N;     // enqueue-only: everything later on this handle's stream is ordered after the upload
+    h->scan_valid = true;
+    h->last_pass_valid = false;
+    return FLB_OK;
+}
+
 int flb_scan_upload(flb_handle* h, const float* body_xyz, int N, int stride) {
     FLB_CHECK_H(h);
     if ((!body_xyz && N != 0) || N < 0 || stride < 3) return fail(h, FLB_ERR_INVALID, "flb_scan_upload: bad arguments");
@@ -1987,89 +2086,110 @@ int flb_scan_upload(flb_handle* h, const float* body_xyz, int N, int stride) {
         for (int j = 0; j < 24; ++j) lo[j % 3] = std::min(lo[j % 3], mn[j]);
         if (bad) return fail(h, FLB_ERR_INVALID, "flb_scan_upload: non-finite coordinate");
     }
-    // The copy and the ordering run on `scan_stream` into the slot that is NOT being read: updates of the previous frame
-    // still queued or running on `stream` keep their scan, and -- because the persistent kernels leave one SM free and
-    // the ordering is one block (k_scan_sort_block) -- this frame's upload overlaps them instead of queueing behind them.
-    const int cur = h->scan_slot, alt = cur ^ 1;
-    cudaStream_t ss = h->scan_stream;
-    FLB_CUDA(h, cudaEventRecord(h->ev_scan_free[cur], h->stream));     // all readers of the current slot are enqueued before this
-    h->scan_free_valid[cur] = true;
-    if (h->scan_free_valid[alt]) FLB_CUDA(h, cudaStreamWaitEvent(ss, h->ev_scan_free[alt], 0));
-    // (scan_raw / skeys / svals double as flb_voxel_grid's scratch on `stream`; that call ends with a stream synchronise)
+    // The copy runs on `scan_stream`, ahead of the ordering that reads it (the previous upload's ordering, which read
+    // scan_raw too, is earlier on the same stream).  scan_raw / skeys / svals double as flb_voxel_grid's scratch on
+    // `stream`; that call ends with a stream synchronise.
     FLB_CUDA(h, h->scan_raw.reserve(n1 * 3));
-    FLB_CUDA(h, h->scan_alt.reserve(n1));
-    FLB_CUDA(h, h->sel_alt.reserve(n1));
-    FLB_CUDA(h, h->plane_ok_alt.reserve(n1));
-    FLB_CUDA(h, h->plane_alt.reserve(n1));
-    const size_t nb = (n1 + kLioBlock - 1) / kLioBlock;
-    FLB_CUDA(h, h->partials.reserve(std::max<size_t>(nb * lio_packed(12), h->partials.cap)));
-    bool flags_done = false;
     if (N > 0) {
-        FLB_CUDA(h, cudaMemcpyAsync(h->scan_raw.p, st, (size_t)N * 3 * sizeof(float), cudaMemcpyHostToDevice, ss));
-        if (!direct) FLB_CUDA(h, h->st_scan.mark(ss));
-        // Morton order in the body frame (cell = twice the map grid's cell): spatially coherent warps at any pose
-        const float inv_cell = 0.5f / (float)h->cfg.cell_size;
-        // One-block ordering vs keys + device-wide radix sort + gather (identical order).  Measured on an idle H100
-        // (profiles/scan_upload_probe.py, copy included): 8 k points 42 vs 77 us, 16 k 100 vs 89, 24 k 129 vs 99 -- but the
-        // one-block kernel runs on the SM the persistent kernels leave free, so when an update is still running on
-        // `stream` (a pipelined caller) it costs nothing, while the device-wide kernels would queue behind the update.
-        // So: one block up to 16 896 points always, up to 25 600 when `stream` is busy; FLB_BLOCK_SORT=0 / 2 or
-        // flb_debug_set_scan_sort force the device-wide / one-block path.
-        static const int env_block_sort = [] { const char* e = getenv("FLB_BLOCK_SORT"); return e ? atoi(e) : 1; }();
-        const int mode = h->scan_sort_mode ? h->scan_sort_mode : (env_block_sort == 0 ? 2 : (env_block_sort == 2 ? 1 : 0));
-        bool use_block = N <= 1024 * 25 && mode != 2;
-        if (use_block && mode == 0 && N > 512 * 33) {
-            const cudaError_t q = cudaStreamQuery(h->stream);
-            (void)cudaGetLastError();
-            use_block = (q == cudaErrorNotReady);
-        }
-        if (use_block) {
+        FLB_CUDA(h, cudaMemcpyAsync(h->scan_raw.p, st, (size_t)N * 3 * sizeof(float), cudaMemcpyHostToDevice, h->scan_stream));
+        if (!direct) FLB_CUDA(h, h->st_scan.mark(h->scan_stream));
+    }
+    return scan_install_dev(h, h->scan_raw.p, N, lo);
+}
+
+// downSizeFilterSurf.setInputCloud(feats_undistort); downSizeFilterSurf.filter(*feats_down_body) (src/laserMapping.cpp:
+// 1398-1399) followed by flb_scan_upload, on the device.  The undistortion output {x, y, z, offset} is packed into sf_xyz
+// (k_cloud_pack, which also flags a non-finite point), filtered by voxel_grid_dev into sf_down in buffers of this call's
+// own, and k_cloud_bounds folds the centroids' bounds into the record; one read of the record (non-finite flags, PCL's
+// overflow flag, leaf count, the centroids' minimum = the Morton keys' origin) decides the errors, then the centroids are
+// installed exactly as flb_scan_upload installs the host copy of the same floats.
+//   Fences.  sf_down is the ordering's input on `scan_stream`.  Every install ends by making `stream` wait for its
+// ordering (ev_scan_ready), so the filter of a later call, enqueued on `stream` after that, cannot overwrite sf_down
+// under an ordering still reading it.  The other way round, the ordering of this call is enqueued on `scan_stream` only
+// after the host has waited for the record read, which `stream` runs after the filter: the centroids are complete
+// before the ordering can start, with no cross-stream wait.
+int flb_scan_from_undistorted(flb_handle* h, float leaf, int* n_out) {
+    FLB_CHECK_H(h);
+    if (n_out) *n_out = 0;
+    if (!(leaf > 0)) return fail(h, FLB_ERR_INVALID, "flb_scan_from_undistorted: bad arguments (leaf > 0)");
+    if (h->comm || h->p2p.world > 0)
+        return fail(h, FLB_ERR_STATE, "flb_scan_from_undistorted: single GPU only (each rank holds only its shard of the scan)");
+    if (h->undist_n < 0)
+        return fail(h, FLB_ERR_STATE, "flb_scan_from_undistorted: no flb_imu_undistort output (none yet, or the last call failed)");
+    const int n = h->undist_n;
+    float lo[3] = {0, 0, 0};
+    int m = 0;
+    if (n > 0) {
+        FLB_CUDA(h, h->sf_xyz.reserve((size_t)n * 3));
+        FLB_CUDA(h, h->sf_down.reserve((size_t)n * 3));
+        FLB_CUDA(h, h->sf_keys.reserve(n));
+        FLB_CUDA(h, h->sf_keys_sorted.reserve(n));
+        FLB_CUDA(h, h->sf_vals.reserve(n));
+        FLB_CUDA(h, h->sf_vals_sorted.reserve(n));
+        FLB_CUDA(h, h->sf_heads.reserve((size_t)2 * n));
+        FLB_CUDA(h, h->sf_rec.reserve(kSfRecWords));
+        FLB_CUDA(h, h->pin_out.reserve(kSfRecWords * sizeof(unsigned)));
+        unsigned* rec_in = h->sf_rec.p + kSfRecInput;
+        unsigned* rec_c = h->sf_rec.p + kSfRecCentroids;
+        int* box = reinterpret_cast<int*>(h->sf_rec.p + kSfRecBox);   // k_bbox box | overflow | leaf count
+        FLB_CUDA(h, cudaMemsetAsync(h->sf_rec.p, 0, kSfRecBox * sizeof(unsigned), h->stream));
+        {
             LaunchScope ls(h, FAM_OTHER);
-            int rcs = N <= 512 * 17   ? launch_scan_sort_block<512, 17>(h, ss, N, lo, inv_cell)
-                      : N <= 512 * 33 ? launch_scan_sort_block<512, 33>(h, ss, N, lo, inv_cell)
-                                      : launch_scan_sort_block<1024, 25>(h, ss, N, lo, inv_cell);
-            if (rcs) return rcs;
-            flags_done = true;
-        } else {
-            FLB_CUDA(h, h->skeys.reserve(n1));
-            FLB_CUDA(h, h->skeys_sorted.reserve(n1));
-            FLB_CUDA(h, h->svals.reserve(n1));
-            FLB_CUDA(h, h->svals_sorted.reserve(n1));
-            const int g = (N + 255) / 256;
-            {
-                LaunchScope ls(h, FAM_OTHER);
-                k_scan_keys<<<g, 256, 0, ss>>>(h->scan_raw.p, N, lo[0], lo[1], lo[2], inv_cell, h->skeys.p, h->svals.p);
-                FLB_CUDA(h, cudaGetLastError());
-            }
-            size_t tmp_bytes = 0;
-            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, h->skeys.p, h->skeys_sorted.p, h->svals.p,
-                                                        h->svals_sorted.p, N, 0, 24, ss));
-            FLB_CUDA(h, h->scan_cub_tmp.reserve(tmp_bytes));
-            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->scan_cub_tmp.p, tmp_bytes, h->skeys.p, h->skeys_sorted.p, h->svals.p,
-                                                        h->svals_sorted.p, N, 0, 24, ss));
-            h->launches += 3;
-            {
-                LaunchScope ls(h, FAM_OTHER);
-                k_scan_gather<<<g, 256, 0, ss>>>(h->scan_raw.p, N, h->svals_sorted.p, h->scan_alt.p);
-                FLB_CUDA(h, cudaGetLastError());
-            }
+            k_cloud_pack<false><<<(n + 255) / 256, 256, 0, h->stream>>>(h->undist_pts, n, h->sf_xyz.p, rec_in);
+            FLB_CUDA(h, cudaGetLastError());
         }
+        const VgScratch vs{h->sf_keys.p, h->sf_keys_sorted.p, h->sf_vals.p, h->sf_vals_sorted.p, h->sf_heads.p, h->sf_heads.p + n, box};
+        { int rcv = voxel_grid_dev(h, h->sf_xyz.p, n, leaf, vs, h->sf_down.p); if (rcv) return rcv; }
+        {
+            LaunchScope ls(h, FAM_OTHER);
+            k_cloud_bounds<<<(n + 255) / 256, 256, 0, h->stream>>>(h->sf_down.p, n, box + 7, rec_c);
+            FLB_CUDA(h, cudaGetLastError());
+        }
+        unsigned* rec = static_cast<unsigned*>(h->pin_out.p);
+        FLB_CUDA(h, cudaMemcpyAsync(rec, h->sf_rec.p, kSfRecWords * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+        if (rec[kSfRecInput + kScanRecBad]) return fail(h, FLB_ERR_INVALID, "flb_scan_from_undistorted: non-finite coordinate");
+        if (rec[kSfRecBox + 6])
+            return fail(h, FLB_ERR_INVALID, "flb_scan_from_undistorted: leaf size too small for the cloud's extent (index overflow, as PCL warns)");
+        if (rec[kSfRecCentroids + kScanRecBad]) return fail(h, FLB_ERR_INVALID, "flb_scan_from_undistorted: non-finite centroid");
+        m = (int)rec[kSfRecBox + 7];
+        for (int k = 0; k < 3; ++k) lo[k] = f32_from_order_key(~rec[kSfRecCentroids + kScanRecMin + k]);
     }
-    if (!flags_done) {
-        // point_selected_surf.resize(N, true) (src/laserMapping.cpp:1469)
-        FLB_CUDA(h, cudaMemsetAsync(h->sel_alt.p, 1, n1, ss));
-        FLB_CUDA(h, cudaMemsetAsync(h->plane_ok_alt.p, 0, n1, ss));
+    { int rci = scan_install_dev(h, h->sf_down.p, m, lo); if (rci) return rci; }
+    if (n_out) *n_out = m;
+    return FLB_OK;
+}
+
+// ikdtree.Build(feats_down_body->points) of the first frame (src/laserMapping.cpp:1411-1419) from the scan on the device:
+// k_cloud_pack scatters the ordered scan back to the caller's order into map_raw and folds its bounds, and the grid is
+// built as flb_map_upload builds it from the same points.
+int flb_map_upload_scan(flb_handle* h) {
+    FLB_CHECK_H(h);
+    if (h->comm || h->p2p.world > 0)
+        return fail(h, FLB_ERR_STATE, "flb_map_upload_scan: single GPU only (each rank holds only its shard of the scan)");
+    if (!h->scan_valid) return fail(h, FLB_ERR_STATE, "flb_map_upload_scan: no scan uploaded since the last flb_voxel_grid (or ever)");
+    const int M = h->N;
+    if (M < 1) return fail(h, FLB_ERR_INVALID, "flb_map_upload_scan: the scan is empty (M=%d)", M);
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    FLB_CUDA(h, h->map_raw.reserve((size_t)M * 3));
+    FLB_CUDA(h, h->add_rec.reserve(kScanRecWords));
+    FLB_CUDA(h, h->pin_out.reserve(kScanRecWords * sizeof(unsigned)));
+    FLB_CUDA(h, cudaMemsetAsync(h->add_rec.p, 0, kScanRecWords * sizeof(unsigned), h->stream));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_cloud_pack<true><<<(M + 255) / 256, 256, 0, h->stream>>>(h->scan.p, M, h->map_raw.p, h->add_rec.p);
+        FLB_CUDA(h, cudaGetLastError());
     }
-    FLB_CUDA(h, cudaEventRecord(h->ev_scan_ready, ss));
-    FLB_CUDA(h, cudaStreamWaitEvent(h->stream, h->ev_scan_ready, 0));
-    std::swap(h->scan, h->scan_alt);
-    std::swap(h->sel, h->sel_alt);
-    std::swap(h->plane_ok, h->plane_ok_alt);
-    std::swap(h->plane, h->plane_alt);
-    h->scan_slot = alt;
-    h->N = N;     // enqueue-only: everything later on this handle's stream is ordered after the upload
-    h->scan_valid = true;
-    h->last_pass_valid = false;
+    unsigned* rec = static_cast<unsigned*>(h->pin_out.p);
+    FLB_CUDA(h, cudaMemcpyAsync(rec, h->add_rec.p, kScanRecWords * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    for (int k = 0; k < 3; ++k) {                 // (both installs refuse non-finite points: the record has no bad flag set)
+        h->map_lo[k] = f32_from_order_key(~rec[kScanRecMin + k]);
+        h->map_hi[k] = f32_from_order_key(rec[kScanRecMax + k]);
+    }
+    int rc = rebuild_grid(h, M);
+    if (rc) return rc;
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
     return FLB_OK;
 }
 

@@ -292,6 +292,64 @@ __global__ void __launch_bounds__(256) k_map_scan_world(const float4* __restrict
     }
 }
 
+// Block fold of one thread's record words v (kScanRec*, 0 = identity) into rec: warp maximum, then one atomic maximum
+// per word and block.  s_red: one row per warp.
+__device__ __forceinline__ void scan_rec_fold(unsigned (&v)[kScanRecBad + 1], unsigned (*s_red)[kScanRecBad + 1], unsigned* __restrict__ rec) {
+#pragma unroll
+    for (int w = 0; w <= kScanRecBad; ++w)
+        for (int o = 16; o > 0; o >>= 1) v[w] = max(v[w], __shfl_xor_sync(0xffffffffu, v[w], o));
+    if ((threadIdx.x & 31) == 0)
+#pragma unroll
+        for (int w = 0; w <= kScanRecBad; ++w) s_red[threadIdx.x >> 5][w] = v[w];
+    __syncthreads();
+    if (threadIdx.x <= kScanRecBad) {
+        unsigned m = 0;
+        for (int wp = 0; wp < (int)(blockDim.x >> 5); ++wp) m = max(m, s_red[wp][threadIdx.x]);
+        if (m) atomicMax(rec + threadIdx.x, m);
+    }
+}
+__device__ __forceinline__ void scan_rec_point(const float* p, unsigned (&v)[kScanRecBad + 1]) {
+    if (finite3(p)) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            v[kScanRecMax + k] = f32_order_key(p[k]);
+            v[kScanRecMin + k] = ~v[kScanRecMax + k];
+        }
+    } else {
+        v[kScanRecBad] = 1;
+    }
+}
+
+// k_map_scan_world without the transform: float4 points to packed xyz, with the same bounds record (zeroed before the
+// launch).  kScanOrder = true (flb_map_upload_scan): the ordered scan, point goes to its caller's index (w).
+// kScanOrder = false (flb_scan_from_undistorted): flb_imu_undistort's {x, y, z, time offset}, point i to index i.
+template <bool kScanOrder>
+__global__ void __launch_bounds__(256) k_cloud_pack(const float4* __restrict__ src, int n, float* __restrict__ out, unsigned* __restrict__ rec) {
+    __shared__ unsigned s_red[8][kScanRecBad + 1];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned v[kScanRecBad + 1] = {0, 0, 0, 0, 0, 0, 0};
+    if (i < n) {
+        const float4 q = src[i];
+        const float p[3] = {q.x, q.y, q.z};
+        const int oi = kScanOrder ? (int)__float_as_uint(q.w) : i;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) out[3 * (size_t)oi + k] = p[k];
+        scan_rec_point(p, v);
+    }
+    scan_rec_fold(v, s_red, rec);
+}
+
+// The bounds record of packed points [0, *count), launched over n >= *count threads (the count stays on the device:
+// flb_scan_from_undistorted's leaf count, k_vg_centroids' output).
+__global__ void __launch_bounds__(256) k_cloud_bounds(const float* __restrict__ xyz, int n, const int* __restrict__ count,
+                                                      unsigned* __restrict__ rec) {
+    __shared__ unsigned s_red[8][kScanRecBad + 1];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned v[kScanRecBad + 1] = {0, 0, 0, 0, 0, 0, 0};
+    if (i < n && i < *count) scan_rec_point(xyz + 3 * (size_t)i, v);
+    scan_rec_fold(v, s_red, rec);
+}
+
 __device__ __forceinline__ unsigned long long vox_key(float x, float y, float z, float ds) {
     // floor(p / downsample_size) per axis (ikd_Tree.cpp:392-396), biased into 21 bits each
     const long long ix = (long long)floorf(x / ds) + (1ll << 20), iy = (long long)floorf(y / ds) + (1ll << 20),

@@ -137,8 +137,10 @@ int flb_map_grid_info(flb_handle* h, double* cell_size, int* sparse, int64_t* ce
  *   that survive from frame to frame (last_lidar_end_time_, acc_s_last, angvel_last), in/out.
  *   pts: n_points lidar-frame points in time order, stride_floats floats apart, x,y,z at [0..2] and the time
  *   offset in ms (PointType::curvature) at [offset_index] (pcl::PointXYZINormal: stride 12, offset_index 9).
- *   out_xyz: n_points x 3 compensated coordinates.  poses_out (optional, capacity n_imu entries of 22 doubles:
- *   offset_time, acc, gyr, vel, pos, rot) receives IMUpose; n_poses_out its length. */
+ *   out_xyz: n_points x 3 compensated coordinates, or NULL: the compensated points stay on the device only (no copy
+ *   back), for flb_scan_from_undistorted / flb_world_cloud; everything else is the same as with a buffer.
+ *   poses_out (optional, capacity n_imu entries of 22 doubles: offset_time, acc, gyr, vel, pos, rot) receives
+ *   IMUpose; n_poses_out its length. */
 typedef struct flb_imu_sample { double t; double gyr[3]; double acc[3]; } flb_imu_sample;   /* sensor_msgs::Imu */
 typedef struct flb_imu_params {
     double cov_gyr[3], cov_acc[3], cov_bias_gyr[3], cov_bias_acc[3];   /* src/IMU_Processing.cpp:15-20, :58-83 */
@@ -154,6 +156,22 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
  * feats_down_body (src/laserMapping.cpp:1398-1399): N already-downsampled points in
  * the LiDAR body frame. */
 int flb_scan_upload(flb_handle* h, const float* body_xyz, int N, int stride_floats);
+/* downSizeFilterSurf.setInputCloud(feats_undistort); downSizeFilterSurf.filter(*feats_down_body)
+ * (src/laserMapping.cpp:1398-1399) followed by flb_scan_upload, with the cloud never leaving the device.  The source is
+ * the output of the last successful flb_imu_undistort (out_xyz may be NULL there), in its point order.  The scan is
+ * then exactly what flb_scan_upload(flb_voxel_grid(out_xyz, leaf)) gives: the same points, order and per-point state,
+ * so every call that reads the scan works unchanged.  *n_out (may be NULL) = feats_down_size.  Blocking (one 96-byte
+ * read).  On any error the previous scan stays current and unchanged.
+ *   FLB_ERR_STATE: no flb_imu_undistort output (none yet, or the last call failed); after flb_comm_init /
+ *   flb_p2p_attach (each rank holds only its shard of the scan).
+ *   FLB_ERR_INVALID: !(leaf > 0), a non-finite point, a leaf too small for the cloud's extent (PCL's index-overflow
+ *   case, as in flb_voxel_grid).  Zero points give an empty scan, as flb_scan_upload(h, ..., 0, ...) does. */
+int flb_scan_from_undistorted(flb_handle* h, float leaf, int* n_out);
+/* ikdtree.Build(feats_down_body->points) of the first frame (src/laserMapping.cpp:1411-1419) from the scan on the
+ * device: replaces the map with the current scan's points in the caller's order, byte-identical to flb_map_upload of
+ * the same points.  Blocking.  FLB_ERR_STATE: no scan (or flb_voxel_grid used its slot as scratch), and after
+ * flb_comm_init / flb_p2p_attach; FLB_ERR_INVALID: an empty scan (as flb_map_upload refuses M < 1). */
+int flb_map_upload_scan(flb_handle* h);
 
 /* Exact 5-NN of nq WORLD-frame float queries, KD_TREE::Nearest_Search semantics
  * (include/ikd-Tree/ikd_Tree.cpp:350-380, 843-986, 1291-1295): float32
