@@ -19,6 +19,8 @@
 //        1398-1399) + upload_scan: feats_undistort stays on the device and becomes the scan there
 //   flb::map_incremental(h, lio_prm, filter_size_map_min)  /  flb::map_incremental(h, lio_prm, R, p, filter_size_map_min)   replace
 //        map_incremental()  src/laserMapping.cpp:692-706  (the uploaded scan into the map, no host transform)
+//   flb::lasermap_fov_segment(h, cube_len, &kdtree_delete_counter)  /  (h, cube_len, pos_lid, &kdtree_delete_counter)
+//        replace lasermap_fov_segment()  src/laserMapping.cpp:363-421  (local-map cube + box delete on the device)
 //
 // Type requirements (all met by the reference's types):
 //   Mat3  : operator()(i,j) read/write (Eigen::Matrix3d)          Vec3 : operator()(i) / [i]
@@ -30,6 +32,7 @@
 #include <cstring>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/fastlivo_b200.h"
@@ -135,6 +138,27 @@ inline void map_incremental(flb_handle* h, const flb_lio_params& lio_prm, const 
         pv[i] = p(i);
     }
     check(h, flb_map_add_scan(h, &lio_prm, Rm, pv, filter_size_map_min));
+}
+
+// ---- lasermap_fov_segment (src/laserMapping.cpp:363-421) with the cube on the device ---------------
+// Replaces lasermap_fov_segment() and its ikdtree.Delete_Point_Boxes(cub_needrm): the cube steps at the device state's
+// position (state.pos_end; call it where the reference does, :1395, after the propagation) and the points in its boxes
+// leave the device map.  kdtree_delete_counter receives the number of deleted points (:417).  DET_RANGE and
+// MOV_THRESHOLD default to the reference's constants (:83, :90).
+inline void lasermap_fov_segment(flb_handle* h, double cube_len, int* kdtree_delete_counter = nullptr, float det_range = 300.0f,
+                                 float mov_threshold = 1.5f) {
+    const flb_fov_params prm{cube_len, det_range, mov_threshold};
+    check(h, flb_map_fov_segment(h, &prm, nullptr, nullptr, nullptr, nullptr, kdtree_delete_counter));
+}
+// IKFoM callers: pos_LiD = pos_lid (Vec3 with operator()(i), :1289).  Not a pointer: lasermap_fov_segment(h, cube_len,
+// nullptr) is the overload above with no counter.
+template <class Vec3, class = typename std::enable_if<!std::is_pointer<typename std::decay<Vec3>::type>::value &&
+                                                      !std::is_same<typename std::decay<Vec3>::type, std::nullptr_t>::value>::type>
+inline void lasermap_fov_segment(flb_handle* h, double cube_len, const Vec3& pos_lid, int* kdtree_delete_counter = nullptr,
+                                 float det_range = 300.0f, float mov_threshold = 1.5f) {
+    const flb_fov_params prm{cube_len, det_range, mov_threshold};
+    const double p[3] = {pos_lid(0), pos_lid(1), pos_lid(2)};
+    check(h, flb_map_fov_segment(h, &prm, p, nullptr, nullptr, nullptr, kdtree_delete_counter));
 }
 
 // ---- IKFoM-typed measurement callback (src/laserMapping.cpp:960-1094) ------------------------

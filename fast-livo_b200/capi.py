@@ -162,6 +162,11 @@ class VioEq(C.Structure):
                 ("n_meas", C.c_int64), ("skipped", C.c_int)]
 
 
+class FovParams(C.Structure):
+    """flb_fov_params: cube_side_length, DET_RANGE, MOV_THRESHOLD of lasermap_fov_segment."""
+    _fields_ = [("cube_len", C.c_double), ("det_range", C.c_float), ("mov_threshold", C.c_float)]
+
+
 CLOUD_SCAN, CLOUD_UNDISTORTED = 0, 1       # flb_world_cloud sources (FLB_CLOUD_*)
 
 # every symbol include/fastlivo_b200.h declares (checked by the CPU-only test tier)
@@ -178,7 +183,7 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_world_cloud", "flb_world_cloud_download", "flb_vmap_select_cloud", "flb_vmap_grow_cloud", "flb_colorize_cloud",
            "flb_batch_begin", "flb_batch_set_frame", "flb_batch_state_reset_enqueue", "flb_batch_update_enqueue", "flb_batch_state_download",
            "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
-           "flb_map_grid_info", "flb_debug_set_map_index"]
+           "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset"]
 
 
 def lib_path() -> str:
@@ -222,6 +227,8 @@ def lib():
         L.flb_map_add_points.argtypes = [vp, vp, C.c_int, C.c_int, C.c_float]
         L.flb_map_add_scan.argtypes = [vp, C.POINTER(LioParams), vp, vp, C.c_float]
         L.flb_map_delete_boxes.argtypes = [vp, vp, C.c_int]
+        L.flb_map_fov_segment.argtypes = [vp, C.POINTER(FovParams), vp, C.POINTER(C.c_int), vp, vp, C.POINTER(C.c_int)]
+        L.flb_map_fov_reset.argtypes = [vp]
         L.flb_map_size.argtypes = [vp]
         L.flb_map_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
         L.flb_knn.argtypes = [vp, vp, C.c_int, vp, vp]
@@ -378,6 +385,22 @@ class Handle:
         b = np.ascontiguousarray(boxes, np.float32).reshape(-1, 6)
         self._ck(self.L.flb_map_delete_boxes(self.h, _p(b), len(b)))
         self.M = self.L.flb_map_size(self.h)
+
+    def map_fov_segment(self, cube_len, det_range=300.0, mov_threshold=1.5, pos=None):
+        """flb_map_fov_segment: lasermap_fov_segment + Delete_Point_Boxes at sensor position `pos`, or at the device state
+        when None.  Returns (boxes (n, 6) float32, local_box (6,) float32, n_deleted)."""
+        prm = FovParams(float(cube_len), float(det_range), float(mov_threshold))
+        p = None if pos is None else np.ascontiguousarray(pos, np.float64).reshape(3)
+        nb, nd = C.c_int(), C.c_int()
+        boxes = np.zeros((3, 6), np.float32)
+        local = np.zeros(6, np.float32)
+        self._ck(self.L.flb_map_fov_segment(self.h, C.byref(prm), _p(p), C.byref(nb), _p(boxes), _p(local), C.byref(nd)))
+        self.M = self.L.flb_map_size(self.h)
+        return boxes[:nb.value].copy(), local, nd.value
+
+    def map_fov_reset(self):
+        """flb_map_fov_reset: the next flb_map_fov_segment only places the cube (Localmap_Initialized = false)."""
+        self._ck(self.L.flb_map_fov_reset(self.h))
 
     def map_download(self):
         n = self.L.flb_map_size(self.h)

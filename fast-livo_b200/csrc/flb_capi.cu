@@ -189,6 +189,10 @@ struct flb_handle {
     DevBuf<int> sel_idx;
     DevBuf<float> add_xyz;                     // Add_Points: the new points on the device (packed xyz, input order)
     DevBuf<unsigned> add_rec;                  // flb_map_add_scan: bounds + non-finite record (kScanRec*)
+    // flb_map_fov_segment: two records; fov_rec[fov_cur].cube is the local-map cube (LocalMap_Points, Localmap_Initialized),
+    // a call writes the other one and makes it current once the call has succeeded.  Allocated (zeroed) by the first call.
+    DevBuf<FovRecord> fov_rec;
+    int fov_cur = 0;
 
     // scan + per-point persistent
     int N = 0;
@@ -1014,7 +1018,7 @@ int flb_destroy(flb_handle* h) {
     for (auto& ev : h->evs) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
     h->map_raw.release(); h->keys.release(); h->keys_sorted.release(); h->vals.release(); h->vals_sorted.release();
     h->map_comb.release(); h->boxes.release(); h->vkeys.release(); h->vkeys_sorted.release(); h->keep.release(); h->sel_idx.release();
-    h->add_xyz.release(); h->add_rec.release();
+    h->add_xyz.release(); h->add_rec.release(); h->fov_rec.release();
     h->wc_xyz.release(); h->wc_rec.release(); h->wc_down.release(); h->wc_keys.release(); h->wc_keys_sorted.release();
     h->wc_vals.release(); h->wc_vals_sorted.release(); h->wc_heads.release(); h->wc_box.release();
     h->sf_keys.release(); h->sf_keys_sorted.release(); h->sf_rec.release(); h->sf_vals.release(); h->sf_vals_sorted.release();
@@ -1705,6 +1709,115 @@ int flb_map_delete_boxes(flb_handle* h, const float* boxes, int nb) {
         FLB_CUDA(h, cudaGetLastError());
     }
     return compact_and_rebuild(h, h->vals.p, M);
+}
+
+// Delete the n_del (1 <= n_del < M) points flagged in h->dead[0..M) (sorted order) from the live sorted map: the merge of
+// the incremental Add_Points with no inserts.  Survivors keep their order; the grid box, the dense cell table's geometry
+// and the sparse index's anchor stay as they are (the next Add_Points that leaves the box takes the full path, which
+// re-derives it).  map_raw becomes the sorted order, as after every incremental merge, so map indices still refer to
+// flb_map_download's array.  Enqueued on `stream`; only the sparse table rebuild reads a count back.
+static int map_delete_flagged(flb_handle* h, int n_del) {
+    const int M = h->M, gm = (M + 255) / 256;
+    const GridDesc g = h->grid;
+    FLB_CUDA(h, h->dead_before.reserve((size_t)M + 1));
+    FLB_CUDA(h, h->merge_counts.reserve(2));
+    FLB_CUDA(h, h->map_pts_alt.reserve(M));
+    FLB_CUDA(h, h->map_raw_alt.reserve((size_t)M * 3));
+    if (h->sparse) FLB_CUDA(h, h->cell_keys_alt.reserve(M));
+    else FLB_CUDA(h, h->cell_start_alt.reserve((size_t)h->ncell + 1));
+    size_t tmp_bytes = 0;
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, h->dead_before.p, h->dead_before.p, M, h->stream));
+    FLB_CUDA(h, h->cub_tmp.reserve(tmp_bytes));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_dead_to_int<<<gm, 256, 0, h->stream>>>(h->dead.p, M, h->dead_before.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, tmp_bytes, h->dead_before.p, h->dead_before.p, M, h->stream));
+    h->launches += 2;
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        if (h->sparse) {
+            k_merge_counts_sparse<<<1, 32, 0, h->stream>>>(h->dead_before.p, h->dead.p, M, h->vkeys_sorted.p, 0, h->merge_counts.p);
+            k_merge_existing_sparse<<<gm, 256, 0, h->stream>>>(h->map_pts.p, h->cell_keys.p, h->dead.p, h->dead_before.p, M,
+                                                                h->vkeys_sorted.p, 0, h->map_pts_alt.p, h->map_raw_alt.p,
+                                                                h->cell_keys_alt.p);
+            h->launches += 1;
+        } else {
+            const int ncell = h->ncell;
+            k_merge_counts<<<1, 32, 0, h->stream>>>(h->dead_before.p, h->dead.p, M, h->keys_sorted.p, 0, ncell, h->merge_counts.p);
+            k_merge_cell_starts<<<(ncell + 256) / 256, 256, 0, h->stream>>>(h->cell_start.p, h->dead_before.p, h->merge_counts.p, M,
+                                                                             h->keys_sorted.p, 0, ncell, h->cell_start_alt.p);
+            k_merge_existing<<<gm, 256, 0, h->stream>>>(h->map_pts.p, h->dead.p, h->dead_before.p, M, g, h->keys_sorted.p, 0,
+                                                         h->map_pts_alt.p, h->map_raw_alt.p);
+            h->launches += 2;
+        }
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    std::swap(h->map_pts, h->map_pts_alt);
+    std::swap(h->map_raw, h->map_raw_alt);
+    h->M = M - n_del;
+    h->last_pass_valid = false;
+    if (!h->sparse) {
+        std::swap(h->cell_start, h->cell_start_alt);
+        return FLB_OK;
+    }
+    std::swap(h->cell_keys, h->cell_keys_alt);
+    return build_sparse_table(h, h->M);
+}
+
+// lasermap_fov_segment (src/laserMapping.cpp:363-421): the cube step on the device (k_fov_step), the points inside its
+// boxes flagged and counted there (k_fov_flags), one read of the record, then -- only if a point goes -- the merge above.
+// A frame whose boxes hold no map point costs two tiny kernels and the read; the map, grid and box stay untouched.
+int flb_map_fov_segment(flb_handle* h, const flb_fov_params* prm, const double pos[3], int* n_boxes, float boxes[18],
+                        float local_box[6], int* n_deleted) {
+    FLB_CHECK_H(h);
+    if (!prm || !(std::isfinite(prm->cube_len) && prm->cube_len > 0) || !(std::isfinite(prm->det_range) && prm->det_range > 0) ||
+        !(std::isfinite(prm->mov_threshold) && prm->mov_threshold > 0))
+        return fail(h, FLB_ERR_INVALID, "flb_map_fov_segment: bad arguments (prm; cube_len, det_range, mov_threshold finite and > 0)");
+    if (!pos && !h->state_valid) return fail(h, FLB_ERR_STATE, "flb_map_fov_segment: no pose given and no device state");
+    if (!pos) { int rcf = flush_state_ops(h); if (rcf) return rcf; }
+    if (!h->fov_rec.p) {
+        FLB_CUDA(h, h->fov_rec.reserve(2));
+        FLB_CUDA(h, cudaMemsetAsync(h->fov_rec.p, 0, 2 * sizeof(FovRecord), h->stream));   // Localmap_Initialized = false
+        h->fov_cur = 0;
+    }
+    FovRecord* cur = h->fov_rec.p + h->fov_cur;
+    FovRecord* next = h->fov_rec.p + (1 - h->fov_cur);
+    const int M = h->M;
+    if (M > 0) FLB_CUDA(h, h->dead.reserve(M));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_fov_step<<<1, 1, 0, h->stream>>>(cur, next, pos ? pos[0] : 0.0, pos ? pos[1] : 0.0, pos ? pos[2] : 0.0,
+                                            pos ? nullptr : &h->states.p[0], prm->cube_len, prm->det_range, prm->mov_threshold);
+        if (M > 0) {
+            k_fov_flags<<<(M + 255) / 256, 256, 0, h->stream>>>(h->map_pts.p, M, next, h->dead.p);
+            h->launches++;
+        }
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    FovRecord* rec = static_cast<FovRecord*>(h->pin_out.p);
+    FLB_CUDA(h, cudaMemcpyAsync(rec, next, sizeof(FovRecord), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    const FovRecord r = *rec;
+    if (M > 0 && r.n_deleted >= M)
+        return fail(h, FLB_ERR_STATE, "flb_map_fov_segment: the boxes hold every map point (the map would be empty)");
+    h->fov_cur = 1 - h->fov_cur;                      // the cube moves: LocalMap_Points = New_LocalMap_Points (:413)
+    if (r.n_deleted > 0) { int rcd = map_delete_flagged(h, r.n_deleted); if (rcd) return rcd; }
+    if (n_boxes) *n_boxes = r.n_boxes;
+    if (boxes) std::memcpy(boxes, r.boxes, sizeof(r.boxes));
+    if (local_box) {
+        std::memcpy(local_box, r.cube.vmin, 3 * sizeof(float));
+        std::memcpy(local_box + 3, r.cube.vmax, 3 * sizeof(float));
+    }
+    if (n_deleted) *n_deleted = r.n_deleted;
+    return FLB_OK;
+}
+
+int flb_map_fov_reset(flb_handle* h) {
+    FLB_CHECK_H(h);
+    if (h->fov_rec.p) FLB_CUDA(h, cudaMemsetAsync(h->fov_rec.p, 0, 2 * sizeof(FovRecord), h->stream));
+    return FLB_OK;
 }
 
 int flb_map_size(const flb_handle* h) { return h ? h->M : 0; }

@@ -446,6 +446,73 @@ FLB_HD unsigned f32_order_key(float f) {
 }
 FLB_HD float f32_from_order_key(unsigned k) { return u32_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
 
+// ------------------------------------------------------------------ local-map cube (lasermap_fov_segment)
+// Box q = {min xyz, max xyz} contains p: the half-open test of Delete_by_range (ikd_Tree.cpp:650), min <= p < max.
+FLB_HD bool box_contains(const float* q, float x, float y, float z) {
+    return q[0] <= x && q[3] > x && q[1] <= y && q[4] > y && q[2] <= z && q[5] > z;
+}
+
+constexpr int kFovMaxBoxes = 3;   // at most one slab per axis (:398-411)
+// LocalMap_Points (BoxPointType: float vertices) and Localmap_Initialized (src/laserMapping.cpp:361-362)
+struct FovCube {
+    float vmin[3], vmax[3];
+    int initialized, pad;
+};
+// One call of lasermap_fov_segment: the cube it leaves, cub_needrm (n_boxes of them, {min xyz, max xyz}; the unused
+// slots are the empty box, all zeros), and the number of map points inside them (the flagging kernel adds it up).
+struct FovRecord {
+    FovCube cube;
+    int n_boxes, n_deleted;
+    float boxes[6 * kFovMaxBoxes];
+};
+
+// lasermap_fov_segment (src/laserMapping.cpp:363-412) up to Delete_Point_Boxes, op for op with the reference's types:
+// pos_LiD double, the cube's vertices float, dist_to_map_edge float of fabs(double - float), the threshold the float
+// product MOV_THRESHOLD * DET_RANGE, mov_dist a double max stored as float.  `in` is the cube before the call.
+FLB_HD void fov_segment_step(const FovCube& in, const double* pos, double cube_len, float det_range, float mov_threshold,
+                             FovRecord& out) {
+    out.cube = in;
+    out.n_boxes = 0;
+    out.n_deleted = 0;
+    for (int k = 0; k < 6 * kFovMaxBoxes; ++k) out.boxes[k] = 0.0f;
+    if (!in.initialized) {                                                     // :376-384
+        for (int i = 0; i < 3; ++i) {
+            out.cube.vmin[i] = (float)(pos[i] - cube_len / 2.0);
+            out.cube.vmax[i] = (float)(pos[i] + cube_len / 2.0);
+        }
+        out.cube.initialized = 1;
+        return;
+    }
+    const float thr = mov_threshold * det_range;
+    float dist[3][2];
+    bool need_move = false;
+    for (int i = 0; i < 3; ++i) {                                              // :386-391
+        dist[i][0] = (float)fabs(pos[i] - (double)in.vmin[i]);
+        dist[i][1] = (float)fabs(pos[i] - (double)in.vmax[i]);
+        if (dist[i][0] <= thr || dist[i][1] <= thr) need_move = true;
+    }
+    if (!need_move) return;
+    const double a = (cube_len - 2.0 * (double)mov_threshold * (double)det_range) * 0.5 * 0.9;   // :396
+    const double b = (double)(det_range * (mov_threshold - 1));
+    const float mov_dist = (float)(a < b ? b : a);                             // std::max: the first unless it is less
+    for (int i = 0; i < 3; ++i) {                                              // :397-411
+        float tmp[6] = {in.vmin[0], in.vmin[1], in.vmin[2], in.vmax[0], in.vmax[1], in.vmax[2]};
+        if (dist[i][0] <= thr) {
+            out.cube.vmax[i] -= mov_dist;
+            out.cube.vmin[i] -= mov_dist;
+            tmp[i] = in.vmax[i] - mov_dist;
+        } else if (dist[i][1] <= thr) {
+            out.cube.vmax[i] += mov_dist;
+            out.cube.vmin[i] += mov_dist;
+            tmp[3 + i] = in.vmin[i] + mov_dist;
+        } else {
+            continue;
+        }
+        for (int k = 0; k < 6; ++k) out.boxes[6 * out.n_boxes + k] = tmp[k];
+        ++out.n_boxes;
+    }
+}
+
 // Row bounds, the one reader of a cell index: the points of cells [xa, xb] of row (z, y) are one contiguous run of the
 // sorted array; returns its [start, end).  Dense: two table reads (the caller clips to the grid).  Sparse: start of the
 // first occupied cell, end of the last; (0, 0) when none is occupied.

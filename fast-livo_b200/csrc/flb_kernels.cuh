@@ -435,12 +435,39 @@ __global__ void k_box_flags(const float* __restrict__ xyz, int M, const float* _
     if (i >= M) return;
     const float x = xyz[3 * (size_t)i], y = xyz[3 * (size_t)i + 1], z = xyz[3 * (size_t)i + 2];
     bool del = false;
-    for (int b = 0; b < nb; ++b) {
-        const float* q = boxes + 6 * b;
-        if (q[0] <= x && q[3] > x && q[1] <= y && q[4] > y && q[2] <= z && q[5] > z) del = true;
-    }
+    for (int b = 0; b < nb; ++b) del = del || box_contains(boxes + 6 * b, x, y, z);
     keep[i] = del ? 0 : 1;
     vals[i] = i;
+}
+
+// lasermap_fov_segment's cube step (fov_segment_step), one thread: the cube of `cur` moves at the sensor position
+// `pos`, or -- x non-null -- at the device state's pos (state.pos_end, :371), into `next`.  The caller commits `next`
+// as the new cube only once it has read the record back.
+__global__ void k_fov_step(const FovRecord* __restrict__ cur, FovRecord* __restrict__ next, double px, double py, double pz,
+                           const State18* __restrict__ x, double cube_len, float det_range, float mov_threshold) {
+    double pos[3] = {px, py, pz};
+    if (x)
+        for (int k = 0; k < 3; ++k) pos[k] = x->pos[k];
+    FovRecord r;
+    fov_segment_step(cur->cube, pos, cube_len, det_range, mov_threshold, r);
+    *next = r;
+}
+// Delete_Point_Boxes(cub_needrm) on the sorted map, first half: dead[m] = sorted point m lies in one of rec's boxes
+// (box_contains, as k_box_flags), and rec->n_deleted += their count.  Nothing to do without a box: dead is then
+// left as it was, and the caller, reading n_deleted = 0, does not look at it.
+__global__ void __launch_bounds__(256) k_fov_flags(const float4* __restrict__ pts, int M, FovRecord* __restrict__ rec,
+                                                   unsigned char* __restrict__ dead) {
+    const int nb = rec->n_boxes;
+    if (nb == 0) return;
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    bool del = false;
+    if (m < M) {
+        const float4 p = pts[m];
+        for (int b = 0; b < nb; ++b) del = del || box_contains(rec->boxes + 6 * b, p.x, p.y, p.z);
+        dead[m] = del ? 1 : 0;
+    }
+    const int c = __syncthreads_count(del);
+    if (threadIdx.x == 0 && c) atomicAdd(&rec->n_deleted, c);
 }
 
 __global__ void k_gather_xyz(const float* __restrict__ src, const int* __restrict__ idx, int n, float* __restrict__ dst) {

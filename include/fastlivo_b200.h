@@ -114,6 +114,30 @@ int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride_
 struct flb_lio_params;
 int flb_map_add_scan(flb_handle* h, const struct flb_lio_params* prm, const double R[9], const double p[3], float downsample_size);
 int flb_map_delete_boxes(flb_handle* h, const float* boxes, int nb);
+/* lasermap_fov_segment (src/laserMapping.cpp:363-421) + ikdtree.Delete_Point_Boxes(cub_needrm) in one call.  The local-
+ * map cube (LocalMap_Points, Localmap_Initialized: :361-362) lives on the device in the handle and survives map uploads.
+ *   cube_len = cube_side_length (:1118), det_range = DET_RANGE (:83, 300 in the reference), mov_threshold =
+ *   MOV_THRESHOLD (:90, 1.5).  pos = pos_LiD (:368-373): NULL = state.pos_end of the device state x as it stands in
+ *   stream order (after flb_imu_undistort that is the propagated prior, as at :1395); IKFoM callers pass pos_lid.
+ * The cube steps exactly as the reference's (float vertices, double pose; the first call after flb_create or
+ * flb_map_fov_reset only places the cube: *n_boxes = 0).  The points inside the boxes (half-open, as
+ * flb_map_delete_boxes) are removed from the live sorted map without rebuilding it: survivors keep their order, the grid
+ * box is kept.  When no point is inside, the map, its grid and its download bytes are unchanged.  Map indices still
+ * refer to flb_map_download's array.  Blocking (one small read).  Runs before any map exists (M = 0: the cube moves,
+ * nothing is deleted).  Outputs (each may be NULL): *n_boxes (0..3) = cub_needrm.size(), boxes[18] = the boxes
+ * (min xyz, max xyz; unused slots all zero), local_box[6] = the cube after the call (min xyz, max xyz), *n_deleted =
+ * kdtree_delete_counter (:417).  Bitwise the same on every rank, so multi-GPU handles may call it too.
+ *   FLB_ERR_INVALID: prm NULL, or cube_len / det_range / mov_threshold not finite or not > 0.
+ *   FLB_ERR_STATE: pos NULL without a device state; boxes that hold every map point (map and cube unchanged).
+ * flb_map_fov_reset: Localmap_Initialized = false. */
+typedef struct flb_fov_params {
+    double cube_len;       /* cube_side_length (src/laserMapping.cpp:1118) */
+    float det_range;       /* DET_RANGE (:83) */
+    float mov_threshold;   /* MOV_THRESHOLD (:90) */
+} flb_fov_params;
+int flb_map_fov_segment(flb_handle* h, const flb_fov_params* prm, const double pos[3], int* n_boxes, float boxes[18],
+                        float local_box[6], int* n_deleted);
+int flb_map_fov_reset(flb_handle* h);
 int flb_map_size(const flb_handle* h);
 int flb_map_download(flb_handle* h, float* xyz, int capacity_points, int* M_out);
 /* flb_map_grid_info: the kNN cell geometry in use.  The map's cells are indexed by a dense table over the map's box
