@@ -1334,78 +1334,143 @@ static int bits_for(long long span) {
     return b;
 }
 
-// Incremental Add_Points on the sparse index (always: there is no box to leave).  The steps of the dense incremental path
-// below, on 64-bit cell keys; the hash table is then rebuilt from the merged key array.  Nothing scales with the extent.
-static int map_add_points_sparse(flb_handle* h, const float* nxyz, int n, float ds, const float* lo, const float* hi) {
-    const int M = h->M;
-    const GridDesc g = h->grid;
-    // voxel keys relative to the new points' own box (absolute 21-bit keys if that box needs more than 62 bits)
-    const int bx = (int)std::floor(lo[0] / ds) - 1, by = (int)std::floor(lo[1] / ds) - 1, bz = (int)std::floor(lo[2] / ds) - 1;
-    const int wx = bits_for((long long)std::floor(hi[0] / ds) + 2 - bx), wy = bits_for((long long)std::floor(hi[1] / ds) + 2 - by),
-              wz = bits_for((long long)std::floor(hi[2] / ds) + 2 - bz);
-    const bool rel = wx + wy + wz <= 62;
-    const int vbits = rel ? wx + wy + wz : 63;
-    FLB_CUDA(h, h->vkeys.reserve(n));
-    FLB_CUDA(h, h->vkeys_sorted.reserve(n));
-    FLB_CUDA(h, h->vals.reserve(n));
-    FLB_CUDA(h, h->vals_sorted.reserve(n));
-    FLB_CUDA(h, h->dead.reserve(M));
-    FLB_CUDA(h, h->ins.reserve(n));
+}  // extern "C"
+
+// The merge of the incremental Add_Points and of the cube delete, once h->dead[0..M) flags the points that go (sorted
+// order) and, for n new points in nxyz, ins_keys / ins_vals hold their cell keys sorted ("no cell" for the ones not
+// inserted) and their indices.  Survivors keep their order, inserts go behind their cell's survivors, the _alt buffers
+// become the map; the dense table merges its cell_start, the sparse index rebuilds its hash table from the merged keys.
+// The grid box, the dense table's geometry and the sparse index's anchor stay as they are.  map_raw becomes the sorted
+// order, so map indices still refer to flb_map_download's array.  n = 0 (a delete): the caller knows the number of
+// flagged points, n_del, and the counts are not read back; only the sparse table rebuild reads its cell count.
+template <bool SPARSE>
+static int map_merge(flb_handle* h, const float* nxyz, int n, const CellKey<SPARSE>* ins_keys, const int* ins_vals, int n_del) {
+    const int M = h->M, ncell = h->ncell, gm = (M + 255) / 256;
     FLB_CUDA(h, h->dead_before.reserve((size_t)M + 1));
     FLB_CUDA(h, h->merge_counts.reserve(2));
     FLB_CUDA(h, h->map_pts_alt.reserve((size_t)M + n));
     FLB_CUDA(h, h->map_raw_alt.reserve(((size_t)M + n) * 3));
-    FLB_CUDA(h, h->cell_keys_alt.reserve((size_t)M + n));
+    if constexpr (SPARSE) FLB_CUDA(h, h->cell_keys_alt.reserve((size_t)M + n));
+    else FLB_CUDA(h, h->cell_start_alt.reserve((size_t)ncell + 1));
+    size_t tmp_bytes = 0;
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, h->dead_before.p, h->dead_before.p, M, h->stream));
+    FLB_CUDA(h, h->cub_tmp.reserve(tmp_bytes));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_dead_to_int<<<gm, 256, 0, h->stream>>>(h->dead.p, M, h->dead_before.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, tmp_bytes, h->dead_before.p, h->dead_before.p, M, h->stream));
+    h->launches += 2;
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        const CellKey<SPARSE>* keys_old = nullptr;
+        CellKey<SPARSE>* keys_new = nullptr;
+        if constexpr (SPARSE) {
+            keys_old = h->cell_keys.p;
+            keys_new = h->cell_keys_alt.p;
+        }
+        k_merge_counts<SPARSE><<<1, 32, 0, h->stream>>>(h->dead_before.p, h->dead.p, M, ins_keys, n, ncell, h->merge_counts.p);
+        if constexpr (!SPARSE) {
+            k_merge_cell_starts<<<(ncell + 256) / 256, 256, 0, h->stream>>>(h->cell_start.p, h->dead_before.p, h->merge_counts.p, M,
+                                                                             ins_keys, n, ncell, h->cell_start_alt.p);
+            h->launches++;
+        }
+        k_merge_existing<SPARSE><<<gm, 256, 0, h->stream>>>(h->map_pts.p, keys_old, h->dead.p, h->dead_before.p, M, h->grid, ins_keys,
+                                                            n, h->map_pts_alt.p, h->map_raw_alt.p, keys_new);
+        h->launches++;
+        if (n > 0) {
+            k_merge_inserts<SPARSE><<<(n + 255) / 256, 256, 0, h->stream>>>(nxyz, ins_keys, ins_vals, h->merge_counts.p, h->cell_start.p,
+                                                                            keys_old, h->dead_before.p, M, h->map_pts_alt.p,
+                                                                            h->map_raw_alt.p, keys_new);
+            h->launches++;
+        }
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    int counts[2] = {n_del, 0};                       // dead points, inserted points
+    if (n > 0) {
+        FLB_CUDA(h, cudaMemcpyAsync(counts, h->merge_counts.p, sizeof(counts), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    }
+    std::swap(h->map_pts, h->map_pts_alt);
+    std::swap(h->map_raw, h->map_raw_alt);
+    h->M = M - counts[0] + counts[1];
+    h->last_pass_valid = false;
+    if constexpr (SPARSE) {
+        std::swap(h->cell_keys, h->cell_keys_alt);
+        return build_sparse_table(h, h->M);
+    } else {
+        std::swap(h->cell_start, h->cell_start_alt);
+        return FLB_OK;
+    }
+}
+
+// Incremental Add_Points: the new points sorted by downsample voxel, one thread per touched voxel resolves it against
+// the live points (k_vox_resolve_incremental), the inserted points sorted by cell key, then map_merge.  The voxel keys
+// are packed into as few bits as their box needs (fewer radix passes): on the dense table the grid box, which every new
+// point lies in (else the full path runs); on the sparse index, which has no box to leave, the new points' own box,
+// with absolute 21-bit keys if that box needs more than 62 bits.  Nothing on the sparse index scales with the extent.
+template <bool SPARSE>
+static int map_add_points_inc(flb_handle* h, const float* nxyz, int n, float ds, const float* lo, const float* hi) {
+    const int M = h->M;
+    const GridDesc g = h->grid;
+    const float* klo = SPARSE ? lo : h->grid_lo;
+    const float* khi = SPARSE ? hi : h->grid_hi;
+    const int bx = (int)std::floor(klo[0] / ds) - 1, by = (int)std::floor(klo[1] / ds) - 1, bz = (int)std::floor(klo[2] / ds) - 1;
+    const int wx = bits_for((long long)std::floor(khi[0] / ds) + 2 - bx), wy = bits_for((long long)std::floor(khi[1] / ds) + 2 - by),
+              wz = bits_for((long long)std::floor(khi[2] / ds) + 2 - bz);
+    const bool rel = wx + wy + wz <= 62;
+    if (!SPARSE && !rel) return map_add_points_full(h, nxyz, n, ds);
+    const int vbits = rel ? wx + wy + wz : 63;
+    const int key_bits = SPARSE ? 64 : bits_for((long long)h->ncell);
+    FLB_CUDA(h, h->vkeys.reserve(n));
+    FLB_CUDA(h, h->vkeys_sorted.reserve(n));
+    FLB_CUDA(h, h->vals.reserve(std::max(n, M)));
+    FLB_CUDA(h, h->vals_sorted.reserve(std::max(n, M)));
+    FLB_CUDA(h, h->dead.reserve(M));
+    FLB_CUDA(h, h->ins.reserve(n));
+    // the inserts' cell keys: the sparse index's reuse the voxel-key buffers (spent by then)
+    CellKey<SPARSE>* keys;
+    CellKey<SPARSE>* keys_sorted;
+    if constexpr (SPARSE) {
+        keys = h->vkeys.p;
+        keys_sorted = h->vkeys_sorted.p;
+    } else {
+        FLB_CUDA(h, h->keys.reserve(std::max(n, M)));
+        FLB_CUDA(h, h->keys_sorted.reserve(std::max(n, M)));
+        keys = h->keys.p;
+        keys_sorted = h->keys_sorted.p;
+    }
     FLB_CUDA(h, cudaMemsetAsync(h->dead.p, 0, M, h->stream));
     FLB_CUDA(h, cudaMemsetAsync(h->ins.p, 0, n, h->stream));
-    const int gn = (n + 255) / 256, gm = (M + 255) / 256;
+    const int gn = (n + 255) / 256;
     {
         LaunchScope ls(h, FAM_OTHER);
         if (rel) k_vox_keys_rel<<<gn, 256, 0, h->stream>>>(nxyz, n, ds, bx, by, bz, wx, wx + wy, h->vkeys.p, h->vals.p);
         else k_vox_keys<<<gn, 256, 0, h->stream>>>(nxyz, n, ds, h->vkeys.p, h->vals.p);
         FLB_CUDA(h, cudaGetLastError());
     }
+    // cub_tmp also covers map_merge's scan, so that it is not reallocated under the sorts enqueued here
     size_t t1 = 0, t2 = 0, t3 = 0;
     FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t1, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, vbits, h->stream));
-    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t2, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, 64, h->stream));
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t2, keys, keys_sorted, h->vals.p, h->vals_sorted.p, n, 0, key_bits, h->stream));
     FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t3, h->dead_before.p, h->dead_before.p, M, h->stream));
     FLB_CUDA(h, h->cub_tmp.reserve(std::max(t1, std::max(t2, t3))));
     FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, t1, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, vbits, h->stream));
     {
         LaunchScope ls(h, FAM_OTHER);
-        k_vox_resolve_incremental<true><<<gn, 256, 0, h->stream>>>(h->vkeys_sorted.p, h->vals_sorted.p, nxyz, n, ds, g, cell_index(h),
-                                                                   h->map_pts.p, h->dead.p, h->ins.p);
-        // inserted points sorted by cell key (not-inserted ones carry kNoCell: behind every cell); the voxel keys are spent
-        k_insert_keys_sparse<<<gn, 256, 0, h->stream>>>(nxyz, n, h->ins.p, g, h->vkeys.p, h->vals.p);
+        k_vox_resolve_incremental<SPARSE><<<gn, 256, 0, h->stream>>>(h->vkeys_sorted.p, h->vals_sorted.p, nxyz, n, ds, g, cell_index(h),
+                                                                     h->map_pts.p, h->dead.p, h->ins.p);
+        // inserted points sorted by cell key (not-inserted ones carry "no cell": behind every cell)
+        k_insert_keys<SPARSE><<<gn, 256, 0, h->stream>>>(nxyz, n, h->ins.p, g, h->ncell, keys, h->vals.p);
         FLB_CUDA(h, cudaGetLastError());
     }
-    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, t2, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, 64, h->stream));
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_dead_to_int<<<gm, 256, 0, h->stream>>>(h->dead.p, M, h->dead_before.p);
-        FLB_CUDA(h, cudaGetLastError());
-    }
-    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, t3, h->dead_before.p, h->dead_before.p, M, h->stream));
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_merge_counts_sparse<<<1, 32, 0, h->stream>>>(h->dead_before.p, h->dead.p, M, h->vkeys_sorted.p, n, h->merge_counts.p);
-        k_merge_existing_sparse<<<gm, 256, 0, h->stream>>>(h->map_pts.p, h->cell_keys.p, h->dead.p, h->dead_before.p, M, h->vkeys_sorted.p, n,
-                                                            h->map_pts_alt.p, h->map_raw_alt.p, h->cell_keys_alt.p);
-        k_merge_inserts_sparse<<<gn, 256, 0, h->stream>>>(nxyz, h->vkeys_sorted.p, h->vals_sorted.p, h->merge_counts.p, h->cell_keys.p,
-                                                           h->dead_before.p, M, h->map_pts_alt.p, h->map_raw_alt.p, h->cell_keys_alt.p);
-        FLB_CUDA(h, cudaGetLastError());
-        h->launches += 9;
-    }
-    int counts[2] = {0, 0};
-    FLB_CUDA(h, cudaMemcpyAsync(counts, h->merge_counts.p, sizeof(counts), cudaMemcpyDeviceToHost, h->stream));
-    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    std::swap(h->map_pts, h->map_pts_alt);
-    std::swap(h->map_raw, h->map_raw_alt);
-    std::swap(h->cell_keys, h->cell_keys_alt);
-    h->M = M - counts[0] + counts[1];
-    h->last_pass_valid = false;
-    return build_sparse_table(h, h->M);
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, t2, keys, keys_sorted, h->vals.p, h->vals_sorted.p, n, 0, key_bits, h->stream));
+    h->launches += 5;                                 // the second kernel above, two launches per radix sort
+    return map_merge<SPARSE>(h, nxyz, n, keys_sorted, h->vals_sorted.p, 0);
 }
+
+extern "C" {
 
 // The voxel-key and cell-key limits of new points with bounds lo / hi (shared by both Add_Points entry points).
 static int map_add_check_bounds(flb_handle* h, const char* who, const float* lo, const float* hi, float downsample_size) {
@@ -1427,88 +1492,12 @@ static int map_add_check_bounds(flb_handle* h, const char* who, const float* lo,
 // bounds lo / hi): the map box takes them in, then the sparse-index merge, the full rebuild or the dense incremental
 // merge runs.  flb_map_add_points and flb_map_add_scan differ only in how the points get to nxyz.
 static int map_add_points_dev(flb_handle* h, const float* nxyz, int n, float downsample_size, const float* lo, const float* hi) {
-    const int M = h->M;
     bool inside = true;
     for (int k = 0; k < 3; ++k) inside = inside && lo[k] >= h->grid_lo[k] && hi[k] <= h->grid_hi[k];
     for (int k = 0; k < 3; ++k) { h->map_lo[k] = std::min(h->map_lo[k], lo[k]); h->map_hi[k] = std::max(h->map_hi[k], hi[k]); }
-    if (h->sparse) return map_add_points_sparse(h, nxyz, n, downsample_size, lo, hi);
+    if (h->sparse) return map_add_points_inc<true>(h, nxyz, n, downsample_size, lo, hi);
     if (!inside) return map_add_points_full(h, nxyz, n, downsample_size);
-
-    // ---- incremental path: every new point lies inside the box the grid covers
-    const GridDesc g = h->grid;
-    const int ncell = h->ncell;
-    const float ds = downsample_size;
-    // voxel keys relative to the grid box, packed into as few bits as the box needs (fewer radix passes)
-    const int bx = (int)std::floor(h->grid_lo[0] / ds) - 1, by = (int)std::floor(h->grid_lo[1] / ds) - 1, bz = (int)std::floor(h->grid_lo[2] / ds) - 1;
-    const int wx = bits_for((long long)std::floor(h->grid_hi[0] / ds) + 2 - bx), wy = bits_for((long long)std::floor(h->grid_hi[1] / ds) + 2 - by),
-              wz = bits_for((long long)std::floor(h->grid_hi[2] / ds) + 2 - bz);
-    if (wx + wy + wz > 62) return map_add_points_full(h, nxyz, n, downsample_size);
-    FLB_CUDA(h, h->vkeys.reserve(n));
-    FLB_CUDA(h, h->vkeys_sorted.reserve(n));
-    FLB_CUDA(h, h->vals.reserve(std::max(n, M)));
-    FLB_CUDA(h, h->vals_sorted.reserve(std::max(n, M)));
-    FLB_CUDA(h, h->keys.reserve(std::max(n, M)));
-    FLB_CUDA(h, h->keys_sorted.reserve(std::max(n, M)));
-    FLB_CUDA(h, h->dead.reserve(M));
-    FLB_CUDA(h, h->ins.reserve(n));
-    FLB_CUDA(h, h->dead_before.reserve((size_t)M + 1));
-    FLB_CUDA(h, h->merge_counts.reserve(2));
-    FLB_CUDA(h, h->map_pts_alt.reserve((size_t)M + n));
-    FLB_CUDA(h, h->map_raw_alt.reserve(((size_t)M + n) * 3));
-    FLB_CUDA(h, h->cell_start_alt.reserve((size_t)ncell + 1));
-    FLB_CUDA(h, cudaMemsetAsync(h->dead.p, 0, M, h->stream));
-    FLB_CUDA(h, cudaMemsetAsync(h->ins.p, 0, n, h->stream));
-    const int gn = (n + 255) / 256, gm = (M + 255) / 256;
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_vox_keys_rel<<<gn, 256, 0, h->stream>>>(nxyz, n, ds, bx, by, bz, wx, wx + wy, h->vkeys.p, h->vals.p);
-        FLB_CUDA(h, cudaGetLastError());
-    }
-    size_t tmp_bytes = 0, t2 = 0, t3 = 0;
-    int cell_bits = bits_for((long long)ncell);
-    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0,
-                                                wx + wy + wz, h->stream));
-    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t2, h->keys.p, h->keys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, cell_bits, h->stream));
-    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t3, h->dead_before.p, h->dead_before.p, M, h->stream));
-    FLB_CUDA(h, h->cub_tmp.reserve(std::max(tmp_bytes, std::max(t2, t3))));
-    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, tmp_bytes, h->vkeys.p, h->vkeys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0,
-                                                wx + wy + wz, h->stream));
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_vox_resolve_incremental<false><<<gn, 256, 0, h->stream>>>(h->vkeys_sorted.p, h->vals_sorted.p, nxyz, n, ds, g, h->cell_start.p, h->map_pts.p,
-                                                              h->dead.p, h->ins.p);
-        // inserted points sorted by grid cell (not-inserted ones sort behind every cell)
-        k_insert_cells<<<gn, 256, 0, h->stream>>>(nxyz, n, h->ins.p, g, ncell, h->keys.p, h->vals.p);
-        FLB_CUDA(h, cudaGetLastError());
-    }
-    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->cub_tmp.p, t2, h->keys.p, h->keys_sorted.p, h->vals.p, h->vals_sorted.p, n, 0, cell_bits, h->stream));
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_dead_to_int<<<gm, 256, 0, h->stream>>>(h->dead.p, M, h->dead_before.p);
-        FLB_CUDA(h, cudaGetLastError());
-    }
-    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, t3, h->dead_before.p, h->dead_before.p, M, h->stream));
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_merge_counts<<<1, 32, 0, h->stream>>>(h->dead_before.p, h->dead.p, M, h->keys_sorted.p, n, ncell, h->merge_counts.p);
-        k_merge_cell_starts<<<(ncell + 256) / 256, 256, 0, h->stream>>>(h->cell_start.p, h->dead_before.p, h->merge_counts.p, M, h->keys_sorted.p, n,
-                                                                         ncell, h->cell_start_alt.p);
-        k_merge_existing<<<gm, 256, 0, h->stream>>>(h->map_pts.p, h->dead.p, h->dead_before.p, M, g, h->keys_sorted.p, n, h->map_pts_alt.p,
-                                                     h->map_raw_alt.p);
-        k_merge_inserts<<<gn, 256, 0, h->stream>>>(nxyz, h->keys_sorted.p, h->vals_sorted.p, n, h->merge_counts.p, h->cell_start_alt.p,
-                                                    h->map_pts_alt.p, h->map_raw_alt.p);
-        FLB_CUDA(h, cudaGetLastError());
-        h->launches += 10;
-    }
-    int counts[2] = {0, 0};
-    FLB_CUDA(h, cudaMemcpyAsync(counts, h->merge_counts.p, sizeof(counts), cudaMemcpyDeviceToHost, h->stream));
-    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    std::swap(h->map_pts, h->map_pts_alt);
-    std::swap(h->cell_start, h->cell_start_alt);
-    std::swap(h->map_raw, h->map_raw_alt);
-    h->M = M - counts[0] + counts[1];
-    h->last_pass_valid = false;
-    return FLB_OK;
+    return map_add_points_inc<false>(h, nxyz, n, downsample_size, lo, hi);
 }
 
 int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride, float downsample_size) {
@@ -1561,6 +1550,46 @@ int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride,
     return map_add_points_dev(h, h->add_xyz.p, n, downsample_size, lo, hi);
 }
 
+// lo / hi of a bounds record (kScanRec*: the per-axis ~min and max order keys)
+static void scan_rec_bounds(const unsigned* rec, float lo[3], float hi[3]) {
+    for (int k = 0; k < 3; ++k) {
+        lo[k] = f32_from_order_key(~rec[kScanRecMin + k]);
+        hi[k] = f32_from_order_key(rec[kScanRecMax + k]);
+    }
+}
+
+// pointBodyToWorld of the n >= 1 points of src into out (k_map_scan_world; scan_order: src is the ordered scan, each
+// point goes to its caller's index; else src is in the caller's order) at (R, p), or -- R null -- at the device state x
+// once the pending state operations are flushed.  The bounds record is read back: bad = a non-finite coordinate, else
+// the points lie in lo / hi.  Ends with a stream synchronise: src may change once it returns, out is a copy.
+static int scan_to_world(flb_handle* h, const flb_lio_params* prm, const double R[9], const double p[3], const float4* src, int n,
+                         bool scan_order, DevBuf<float>& out, DevBuf<unsigned>& rec_dev, bool* bad, float lo[3], float hi[3]) {
+    if (!R) { int rcf = flush_state_ops(h); if (rcf) return rcf; }
+    LioPose pose{};
+    std::memcpy(pose.R_LI, prm->R_LI, sizeof(pose.R_LI));
+    std::memcpy(pose.t_LI, prm->t_LI, sizeof(pose.t_LI));
+    if (R) {
+        std::memcpy(pose.R, R, sizeof(pose.R));
+        std::memcpy(pose.p, p, sizeof(pose.p));
+    }
+    FLB_CUDA(h, out.reserve((size_t)n * 3));
+    FLB_CUDA(h, rec_dev.reserve(kScanRecWords));
+    FLB_CUDA(h, cudaMemsetAsync(rec_dev.p, 0, kScanRecWords * sizeof(unsigned), h->stream));
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        const State18* x = R ? nullptr : &h->states.p[0];
+        if (scan_order) k_map_scan_world<true><<<(n + 255) / 256, 256, 0, h->stream>>>(src, n, pose, x, out.p, rec_dev.p);
+        else k_map_scan_world<false><<<(n + 255) / 256, 256, 0, h->stream>>>(src, n, pose, x, out.p, rec_dev.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    unsigned* rec = static_cast<unsigned*>(h->pin_out.p);
+    FLB_CUDA(h, cudaMemcpyAsync(rec, rec_dev.p, kScanRecWords * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    *bad = rec[kScanRecBad] != 0;
+    scan_rec_bounds(rec, lo, hi);
+    return FLB_OK;
+}
+
 // map_incremental (src/laserMapping.cpp:692-706) from what is on the device: the uploaded scan, transformed at (R, p) or
 // at the device state x, enters Add_Points in the caller's order.  One kernel (transform + bounds) and one small
 // readback replace flb_map_add_points' staging, host checks and copy; the merge is the same code.
@@ -1576,34 +1605,12 @@ int flb_map_add_scan(flb_handle* h, const flb_lio_params* prm, const double R[9]
     if (!R && !h->state_valid) return fail(h, FLB_ERR_STATE, "flb_map_add_scan: no pose given and no device state");
     const int n = h->N;
     if (n == 0) return FLB_OK;
-    if (!R) { int rcf = flush_state_ops(h); if (rcf) return rcf; }
-    LioPose pose{};
-    std::memcpy(pose.R_LI, prm->R_LI, sizeof(pose.R_LI));
-    std::memcpy(pose.t_LI, prm->t_LI, sizeof(pose.t_LI));
-    if (R) {
-        std::memcpy(pose.R, R, sizeof(pose.R));
-        std::memcpy(pose.p, p, sizeof(pose.p));
-    }
-    FLB_CUDA(h, h->add_xyz.reserve((size_t)n * 3));
-    FLB_CUDA(h, h->add_rec.reserve(kScanRecWords));
-    FLB_CUDA(h, cudaMemsetAsync(h->add_rec.p, 0, kScanRecWords * sizeof(unsigned), h->stream));
-    {
-        // h->scan is the current set of the double-buffered scan.  This call ends with a stream synchronise, so a later
-        // flb_scan_upload (which fills the other set, and this one only after the next swap) cannot overwrite it under us.
-        LaunchScope ls(h, FAM_OTHER);
-        k_map_scan_world<<<(n + 255) / 256, 256, 0, h->stream>>>(h->scan.p, n, pose, R ? nullptr : &h->states.p[0], h->add_xyz.p,
-                                                                  h->add_rec.p);
-        FLB_CUDA(h, cudaGetLastError());
-    }
-    unsigned* rec = static_cast<unsigned*>(h->pin_out.p);
-    FLB_CUDA(h, cudaMemcpyAsync(rec, h->add_rec.p, kScanRecWords * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
-    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    if (rec[kScanRecBad]) return fail(h, FLB_ERR_INVALID, "flb_map_add_scan: non-finite coordinate");
+    // h->scan is the current set of the double-buffered scan.  scan_to_world ends with a stream synchronise, so a later
+    // flb_scan_upload (which fills the other set, and this one only after the next swap) cannot overwrite it under us.
+    bool bad = false;
     float lo[3], hi[3];
-    for (int k = 0; k < 3; ++k) {
-        lo[k] = f32_from_order_key(~rec[kScanRecMin + k]);
-        hi[k] = f32_from_order_key(rec[kScanRecMax + k]);
-    }
+    { int rcw = scan_to_world(h, prm, R, p, h->scan.p, n, true, h->add_xyz, h->add_rec, &bad, lo, hi); if (rcw) return rcw; }
+    if (bad) return fail(h, FLB_ERR_INVALID, "flb_map_add_scan: non-finite coordinate");
     { int rcb = map_add_check_bounds(h, "flb_map_add_scan", lo, hi, downsample_size); if (rcb) return rcb; }
     return map_add_points_dev(h, h->add_xyz.p, n, downsample_size, lo, hi);
 }
@@ -1634,38 +1641,14 @@ int flb_world_cloud(flb_handle* h, const flb_lio_params* prm, const double R[9],
     if (!R && !h->state_valid) return fail(h, FLB_ERR_STATE, "flb_world_cloud: no pose given and no device state");
     float lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0};
     if (n > 0) {
-        if (!R) { int rcf = flush_state_ops(h); if (rcf) return rcf; }
-        LioPose pose{};
-        std::memcpy(pose.R_LI, prm->R_LI, sizeof(pose.R_LI));
-        std::memcpy(pose.t_LI, prm->t_LI, sizeof(pose.t_LI));
-        if (R) {
-            std::memcpy(pose.R, R, sizeof(pose.R));
-            std::memcpy(pose.p, p, sizeof(pose.p));
-        }
-        FLB_CUDA(h, h->wc_xyz.reserve((size_t)n * 3));
-        FLB_CUDA(h, h->wc_rec.reserve(kScanRecWords));
-        FLB_CUDA(h, cudaMemsetAsync(h->wc_rec.p, 0, kScanRecWords * sizeof(unsigned), h->stream));
-        {
-            // Both sources stay put until the synchronise below: a later flb_scan_upload fills the other scan set, and
-            // flb_imu_undistort is blocking.  wc_xyz is a copy, so neither changes the cloud afterwards.
-            LaunchScope ls(h, FAM_OTHER);
-            const State18* x = R ? nullptr : &h->states.p[0];
-            if (source == FLB_CLOUD_SCAN)
-                k_map_scan_world<true><<<(n + 255) / 256, 256, 0, h->stream>>>(src, n, pose, x, h->wc_xyz.p, h->wc_rec.p);
-            else
-                k_map_scan_world<false><<<(n + 255) / 256, 256, 0, h->stream>>>(src, n, pose, x, h->wc_xyz.p, h->wc_rec.p);
-            FLB_CUDA(h, cudaGetLastError());
-        }
-        unsigned* rec = static_cast<unsigned*>(h->pin_out.p);
-        FLB_CUDA(h, cudaMemcpyAsync(rec, h->wc_rec.p, kScanRecWords * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
-        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-        if (rec[kScanRecBad]) return fail(h, FLB_ERR_INVALID, "flb_world_cloud: non-finite coordinate");
-        for (int k = 0; k < 3; ++k) {
-            lo[k] = f32_from_order_key(~rec[kScanRecMin + k]);
-            hi[k] = f32_from_order_key(rec[kScanRecMax + k]);
-            // the visual map's coordinate limit (vm_upload_points: |v| <= 5e5, 2^20 voxels of its 0.5 m key)
+        // Both sources stay put until scan_to_world's synchronise: a later flb_scan_upload fills the other scan set, and
+        // flb_imu_undistort is blocking.  wc_xyz is a copy, so neither changes the cloud afterwards.
+        bool bad = false;
+        { int rcw = scan_to_world(h, prm, R, p, src, n, source == FLB_CLOUD_SCAN, h->wc_xyz, h->wc_rec, &bad, lo, hi); if (rcw) return rcw; }
+        if (bad) return fail(h, FLB_ERR_INVALID, "flb_world_cloud: non-finite coordinate");
+        // the visual map's coordinate limit (vm_upload_points: |v| <= 5e5, 2^20 voxels of its 0.5 m key)
+        for (int k = 0; k < 3; ++k)
             if (lo[k] < -5.0e5f || hi[k] > 5.0e5f) return fail(h, FLB_ERR_INVALID, "flb_world_cloud: coordinate beyond 2^20 visual-map voxels");
-        }
     }
     std::memcpy(h->wc_lo, lo, sizeof(lo));
     std::memcpy(h->wc_hi, hi, sizeof(hi));
@@ -1711,63 +1694,9 @@ int flb_map_delete_boxes(flb_handle* h, const float* boxes, int nb) {
     return compact_and_rebuild(h, h->vals.p, M);
 }
 
-// Delete the n_del (1 <= n_del < M) points flagged in h->dead[0..M) (sorted order) from the live sorted map: the merge of
-// the incremental Add_Points with no inserts.  Survivors keep their order; the grid box, the dense cell table's geometry
-// and the sparse index's anchor stay as they are (the next Add_Points that leaves the box takes the full path, which
-// re-derives it).  map_raw becomes the sorted order, as after every incremental merge, so map indices still refer to
-// flb_map_download's array.  Enqueued on `stream`; only the sparse table rebuild reads a count back.
-static int map_delete_flagged(flb_handle* h, int n_del) {
-    const int M = h->M, gm = (M + 255) / 256;
-    const GridDesc g = h->grid;
-    FLB_CUDA(h, h->dead_before.reserve((size_t)M + 1));
-    FLB_CUDA(h, h->merge_counts.reserve(2));
-    FLB_CUDA(h, h->map_pts_alt.reserve(M));
-    FLB_CUDA(h, h->map_raw_alt.reserve((size_t)M * 3));
-    if (h->sparse) FLB_CUDA(h, h->cell_keys_alt.reserve(M));
-    else FLB_CUDA(h, h->cell_start_alt.reserve((size_t)h->ncell + 1));
-    size_t tmp_bytes = 0;
-    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, h->dead_before.p, h->dead_before.p, M, h->stream));
-    FLB_CUDA(h, h->cub_tmp.reserve(tmp_bytes));
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        k_dead_to_int<<<gm, 256, 0, h->stream>>>(h->dead.p, M, h->dead_before.p);
-        FLB_CUDA(h, cudaGetLastError());
-    }
-    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, tmp_bytes, h->dead_before.p, h->dead_before.p, M, h->stream));
-    h->launches += 2;
-    {
-        LaunchScope ls(h, FAM_OTHER);
-        if (h->sparse) {
-            k_merge_counts_sparse<<<1, 32, 0, h->stream>>>(h->dead_before.p, h->dead.p, M, h->vkeys_sorted.p, 0, h->merge_counts.p);
-            k_merge_existing_sparse<<<gm, 256, 0, h->stream>>>(h->map_pts.p, h->cell_keys.p, h->dead.p, h->dead_before.p, M,
-                                                                h->vkeys_sorted.p, 0, h->map_pts_alt.p, h->map_raw_alt.p,
-                                                                h->cell_keys_alt.p);
-            h->launches += 1;
-        } else {
-            const int ncell = h->ncell;
-            k_merge_counts<<<1, 32, 0, h->stream>>>(h->dead_before.p, h->dead.p, M, h->keys_sorted.p, 0, ncell, h->merge_counts.p);
-            k_merge_cell_starts<<<(ncell + 256) / 256, 256, 0, h->stream>>>(h->cell_start.p, h->dead_before.p, h->merge_counts.p, M,
-                                                                             h->keys_sorted.p, 0, ncell, h->cell_start_alt.p);
-            k_merge_existing<<<gm, 256, 0, h->stream>>>(h->map_pts.p, h->dead.p, h->dead_before.p, M, g, h->keys_sorted.p, 0,
-                                                         h->map_pts_alt.p, h->map_raw_alt.p);
-            h->launches += 2;
-        }
-        FLB_CUDA(h, cudaGetLastError());
-    }
-    std::swap(h->map_pts, h->map_pts_alt);
-    std::swap(h->map_raw, h->map_raw_alt);
-    h->M = M - n_del;
-    h->last_pass_valid = false;
-    if (!h->sparse) {
-        std::swap(h->cell_start, h->cell_start_alt);
-        return FLB_OK;
-    }
-    std::swap(h->cell_keys, h->cell_keys_alt);
-    return build_sparse_table(h, h->M);
-}
-
 // lasermap_fov_segment (src/laserMapping.cpp:363-421): the cube step on the device (k_fov_step), the points inside its
-// boxes flagged and counted there (k_fov_flags), one read of the record, then -- only if a point goes -- the merge above.
+// boxes flagged and counted there (k_fov_flags), one read of the record, then -- only if a point goes -- map_merge with
+// no inserts: survivors keep their order, and the grid box stays (the next Add_Points that leaves it takes the full path).
 // A frame whose boxes hold no map point costs two tiny kernels and the read; the map, grid and box stay untouched.
 int flb_map_fov_segment(flb_handle* h, const flb_fov_params* prm, const double pos[3], int* n_boxes, float boxes[18],
                         float local_box[6], int* n_deleted) {
@@ -1803,7 +1732,11 @@ int flb_map_fov_segment(flb_handle* h, const flb_fov_params* prm, const double p
     if (M > 0 && r.n_deleted >= M)
         return fail(h, FLB_ERR_STATE, "flb_map_fov_segment: the boxes hold every map point (the map would be empty)");
     h->fov_cur = 1 - h->fov_cur;                      // the cube moves: LocalMap_Points = New_LocalMap_Points (:413)
-    if (r.n_deleted > 0) { int rcd = map_delete_flagged(h, r.n_deleted); if (rcd) return rcd; }
+    if (r.n_deleted > 0) {
+        const int rcd = h->sparse ? map_merge<true>(h, nullptr, 0, nullptr, nullptr, r.n_deleted)
+                                  : map_merge<false>(h, nullptr, 0, nullptr, nullptr, r.n_deleted);
+        if (rcd) return rcd;
+    }
     if (n_boxes) *n_boxes = r.n_boxes;
     if (boxes) std::memcpy(boxes, r.boxes, sizeof(r.boxes));
     if (local_box) {
@@ -2266,7 +2199,8 @@ int flb_scan_from_undistorted(flb_handle* h, float leaf, int* n_out) {
             return fail(h, FLB_ERR_INVALID, "flb_scan_from_undistorted: leaf size too small for the cloud's extent (index overflow, as PCL warns)");
         if (rec[kSfRecCentroids + kScanRecBad]) return fail(h, FLB_ERR_INVALID, "flb_scan_from_undistorted: non-finite centroid");
         m = (int)rec[kSfRecBox + 7];
-        for (int k = 0; k < 3; ++k) lo[k] = f32_from_order_key(~rec[kSfRecCentroids + kScanRecMin + k]);
+        float hi[3];
+        scan_rec_bounds(rec + kSfRecCentroids, lo, hi);
     }
     { int rci = scan_install_dev(h, h->sf_down.p, m, lo); if (rci) return rci; }
     if (n_out) *n_out = m;
@@ -2296,10 +2230,7 @@ int flb_map_upload_scan(flb_handle* h) {
     unsigned* rec = static_cast<unsigned*>(h->pin_out.p);
     FLB_CUDA(h, cudaMemcpyAsync(rec, h->add_rec.p, kScanRecWords * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    for (int k = 0; k < 3; ++k) {                 // (both installs refuse non-finite points: the record has no bad flag set)
-        h->map_lo[k] = f32_from_order_key(~rec[kScanRecMin + k]);
-        h->map_hi[k] = f32_from_order_key(rec[kScanRecMax + k]);
-    }
+    scan_rec_bounds(rec, h->map_lo, h->map_hi);      // (both installs refuse non-finite points: the record has no bad flag set)
     int rc = rebuild_grid(h, M);
     if (rc) return rc;
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));

@@ -188,7 +188,8 @@ __global__ void k_map_gather(const float* __restrict__ xyz, int M, int stride, c
 
 // cell_start[c] = first sorted position whose cell id is >= c (c = 0 .. ncell): one binary search per cell, so long
 // runs of empty cells (a map that covers little of its bounding box) cost nothing extra.
-__device__ __forceinline__ int lower_bound_u32(const unsigned* __restrict__ a, int n, unsigned v) {
+template <class K>
+__device__ __forceinline__ int lower_bound_key(const K* __restrict__ a, int n, K v) {
     int lo = 0, hi = n;
     while (lo < hi) {
         const int mid = (lo + hi) >> 1;
@@ -199,7 +200,7 @@ __device__ __forceinline__ int lower_bound_u32(const unsigned* __restrict__ a, i
 __global__ void k_cell_starts(const unsigned* __restrict__ keys_sorted, int M, int* __restrict__ cell_start, int ncell) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c > ncell) return;
-    cell_start[c] = lower_bound_u32(keys_sorted, M, (unsigned)c);
+    cell_start[c] = lower_bound_key(keys_sorted, M, (unsigned)c);
 }
 
 // bounding box of n packed xyz points: ordered-int atomics into box[6] = {min x, y, z, max x, y, z} (as ordered bits)
@@ -240,6 +241,34 @@ __global__ void k_bbox(const float* __restrict__ xyz, int n, int* __restrict__ b
 // device version sorts (existing + new) points by voxel and lets one thread replay that sequential
 // rule over each voxel's handful of points.
 // ---------------------------------------------------------------------------------------
+// Block fold of one thread's record words v (kScanRec*, 0 = identity) into rec: warp maximum, then one atomic maximum
+// per word and block.  s_red: one row per warp.
+__device__ __forceinline__ void scan_rec_fold(unsigned (&v)[kScanRecBad + 1], unsigned (*s_red)[kScanRecBad + 1], unsigned* __restrict__ rec) {
+#pragma unroll
+    for (int w = 0; w <= kScanRecBad; ++w)
+        for (int o = 16; o > 0; o >>= 1) v[w] = max(v[w], __shfl_xor_sync(0xffffffffu, v[w], o));
+    if ((threadIdx.x & 31) == 0)
+#pragma unroll
+        for (int w = 0; w <= kScanRecBad; ++w) s_red[threadIdx.x >> 5][w] = v[w];
+    __syncthreads();
+    if (threadIdx.x <= kScanRecBad) {
+        unsigned m = 0;
+        for (int wp = 0; wp < (int)(blockDim.x >> 5); ++wp) m = max(m, s_red[wp][threadIdx.x]);
+        if (m) atomicMax(rec + threadIdx.x, m);
+    }
+}
+__device__ __forceinline__ void scan_rec_point(const float* p, unsigned (&v)[kScanRecBad + 1]) {
+    if (finite3(p)) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            v[kScanRecMax + k] = f32_order_key(p[k]);
+            v[kScanRecMin + k] = ~v[kScanRecMax + k];
+        }
+    } else {
+        v[kScanRecBad] = 1;
+    }
+}
+
 // map_incremental from the uploaded scan (flb_map_add_scan) and pcl_wait_pub (flb_world_cloud, RGBpointBodyToWorld
 // has pointBodyToWorld's op order): one thread per point of the ordered scan writes
 // pointBodyToWorld of it to the caller's index in packed xyz, and the block folds its points into rec (kScanRec*: the
@@ -268,56 +297,9 @@ __global__ void __launch_bounds__(256) k_map_scan_world(const float4* __restrict
         const int oi = kScanOrder ? si : i;
 #pragma unroll
         for (int k = 0; k < 3; ++k) out[3 * (size_t)oi + k] = pw[k];
-        if (finite3(pw)) {
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                v[kScanRecMax + k] = f32_order_key(pw[k]);
-                v[kScanRecMin + k] = ~v[kScanRecMax + k];
-            }
-        } else {
-            v[kScanRecBad] = 1;
-        }
+        scan_rec_point(pw, v);
     }
-#pragma unroll
-    for (int w = 0; w <= kScanRecBad; ++w)
-        for (int o = 16; o > 0; o >>= 1) v[w] = max(v[w], __shfl_xor_sync(0xffffffffu, v[w], o));
-    if ((threadIdx.x & 31) == 0)
-#pragma unroll
-        for (int w = 0; w <= kScanRecBad; ++w) s_red[threadIdx.x >> 5][w] = v[w];
-    __syncthreads();
-    if (threadIdx.x <= kScanRecBad) {
-        unsigned m = 0;
-        for (int wp = 0; wp < (int)(blockDim.x >> 5); ++wp) m = max(m, s_red[wp][threadIdx.x]);
-        if (m) atomicMax(rec + threadIdx.x, m);
-    }
-}
-
-// Block fold of one thread's record words v (kScanRec*, 0 = identity) into rec: warp maximum, then one atomic maximum
-// per word and block.  s_red: one row per warp.
-__device__ __forceinline__ void scan_rec_fold(unsigned (&v)[kScanRecBad + 1], unsigned (*s_red)[kScanRecBad + 1], unsigned* __restrict__ rec) {
-#pragma unroll
-    for (int w = 0; w <= kScanRecBad; ++w)
-        for (int o = 16; o > 0; o >>= 1) v[w] = max(v[w], __shfl_xor_sync(0xffffffffu, v[w], o));
-    if ((threadIdx.x & 31) == 0)
-#pragma unroll
-        for (int w = 0; w <= kScanRecBad; ++w) s_red[threadIdx.x >> 5][w] = v[w];
-    __syncthreads();
-    if (threadIdx.x <= kScanRecBad) {
-        unsigned m = 0;
-        for (int wp = 0; wp < (int)(blockDim.x >> 5); ++wp) m = max(m, s_red[wp][threadIdx.x]);
-        if (m) atomicMax(rec + threadIdx.x, m);
-    }
-}
-__device__ __forceinline__ void scan_rec_point(const float* p, unsigned (&v)[kScanRecBad + 1]) {
-    if (finite3(p)) {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            v[kScanRecMax + k] = f32_order_key(p[k]);
-            v[kScanRecMin + k] = ~v[kScanRecMax + k];
-        }
-    } else {
-        v[kScanRecBad] = 1;
-    }
+    scan_rec_fold(v, s_red, rec);
 }
 
 // k_map_scan_world without the transform: float4 points to packed xyz, with the same bounds record (zeroed before the
@@ -567,76 +549,21 @@ __global__ void k_vox_resolve_incremental(const unsigned long long* __restrict__
         }
     if (best <= -2) ins[vals[-(best + 2)]] = 1;
 }
-// cell id of every new point (ncell = "not inserted": sorts behind every real cell)
-__global__ void k_insert_cells(const float* __restrict__ nxyz, int n, const unsigned char* __restrict__ ins, GridDesc g, int ncell,
-                               unsigned* __restrict__ keys, int* __restrict__ vals) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    unsigned key = (unsigned)ncell;
-    if (ins[i]) {
-        const int cx = grid_axis_cell(nxyz[3 * (size_t)i], g.ox, g.inv_cell, g.nx), cy = grid_axis_cell(nxyz[3 * (size_t)i + 1], g.oy, g.inv_cell, g.ny),
-                  cz = grid_axis_cell(nxyz[3 * (size_t)i + 2], g.oz, g.inv_cell, g.nz);
-        key = (unsigned)((cz * g.ny + cy) * g.nx + cx);
-    }
-    keys[i] = key;
-    vals[i] = i;
-}
 __global__ void k_dead_to_int(const unsigned char* __restrict__ dead, int M, int* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < M) out[i] = dead[i];
 }
-// counts[0] = dead points, counts[1] = inserted points (needs dead_before of the last element + its flag)
-__global__ void k_merge_counts(const int* __restrict__ dead_before, const unsigned char* __restrict__ dead, int M,
-                               const unsigned* __restrict__ ins_keys_sorted, int n, int ncell, int* __restrict__ counts) {
-    if (threadIdx.x == 0 && blockIdx.x == 0) {
-        counts[0] = dead_before[M - 1] + dead[M - 1];
-        counts[1] = lower_bound_u32(ins_keys_sorted, n, (unsigned)ncell);
-    }
-}
+// dense table: the merged map's cell_start (survivors before the cell's first old point + inserts sorted before the cell)
 __global__ void k_merge_cell_starts(const int* __restrict__ cs_old, const int* __restrict__ dead_before, const int* __restrict__ counts,
                                     int M, const unsigned* __restrict__ ins_keys_sorted, int n, int ncell, int* __restrict__ cs_new) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c > ncell) return;
     const int s = cs_old[c];
     const int db = s < M ? dead_before[s] : counts[0];
-    cs_new[c] = s - db + lower_bound_u32(ins_keys_sorted, n, (unsigned)c);
-}
-__global__ void k_merge_existing(const float4* __restrict__ pts_old, const unsigned char* __restrict__ dead,
-                                 const int* __restrict__ dead_before, int M, GridDesc g, const unsigned* __restrict__ ins_keys_sorted, int n,
-                                 float4* __restrict__ pts_new, float* __restrict__ raw_new) {
-    const int m = blockIdx.x * blockDim.x + threadIdx.x;
-    if (m >= M || dead[m]) return;
-    float4 p = pts_old[m];
-    const int cx = grid_axis_cell(p.x, g.ox, g.inv_cell, g.nx), cy = grid_axis_cell(p.y, g.oy, g.inv_cell, g.ny),
-              cz = grid_axis_cell(p.z, g.oz, g.inv_cell, g.nz);
-    const unsigned cell = (unsigned)((cz * g.ny + cy) * g.nx + cx);
-    const int pos = m - dead_before[m] + lower_bound_u32(ins_keys_sorted, n, cell);
-    p.w = __int_as_float(pos);
-    pts_new[pos] = p;
-    raw_new[3 * (size_t)pos] = p.x; raw_new[3 * (size_t)pos + 1] = p.y; raw_new[3 * (size_t)pos + 2] = p.z;
-}
-__global__ void k_merge_inserts(const float* __restrict__ nxyz, const unsigned* __restrict__ ins_keys_sorted, const int* __restrict__ ins_vals_sorted,
-                                int n, const int* __restrict__ counts, const int* __restrict__ cs_new, float4* __restrict__ pts_new,
-                                float* __restrict__ raw_new) {
-    const int k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= counts[1]) return;
-    const unsigned cell = ins_keys_sorted[k];
-    const int first = lower_bound_u32(ins_keys_sorted, n, cell), last = lower_bound_u32(ins_keys_sorted, n, cell + 1u);
-    const int pos = cs_new[cell + 1] - (last - first) + (k - first);     // inserts go behind the cell's surviving points
-    const float* q = nxyz + 3 * (size_t)ins_vals_sorted[k];
-    pts_new[pos] = make_float4(q[0], q[1], q[2], __int_as_float(pos));
-    raw_new[3 * (size_t)pos] = q[0]; raw_new[3 * (size_t)pos + 1] = q[1]; raw_new[3 * (size_t)pos + 2] = q[2];
+    cs_new[c] = s - db + lower_bound_key(ins_keys_sorted, n, (unsigned)c);
 }
 
 // ---- sparse cell index (GridDesc): points sorted by 64-bit cell key, a hash table of the occupied cells
-__device__ __forceinline__ int lower_bound_u64(const unsigned long long* __restrict__ a, int n, unsigned long long v) {
-    int lo = 0, hi = n;
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (a[mid] < v) lo = mid + 1; else hi = mid;
-    }
-    return lo;
-}
 __device__ __forceinline__ unsigned long long point_cell_key(float x, float y, float z, const GridDesc& g) {
     return cell_key((int)floorf((x - g.ox) * g.inv_cell), (int)floorf((y - g.oy) * g.inv_cell), (int)floorf((z - g.oz) * g.inv_cell));
 }
@@ -660,7 +587,7 @@ __global__ void k_sparse_insert(const unsigned long long* __restrict__ keys, int
     if (i >= M) return;
     const unsigned long long k = keys[i];
     if (i > 0 && keys[i - 1] == k) return;
-    const int end = lower_bound_u64(keys + i, M - i, k + 1) + i;
+    const int end = lower_bound_key(keys + i, M - i, k + 1) + i;
     for (unsigned h = cell_hash(k) & mask;; h = (h + 1) & mask) {
         if (atomicCAS(&table[h].key, kNoCell, k) == kNoCell) {
             table[h].start = i;
@@ -669,49 +596,82 @@ __global__ void k_sparse_insert(const unsigned long long* __restrict__ keys, int
         }
     }
 }
-// Incremental Add_Points on the sparse index: as k_insert_cells / k_merge_* above, with 64-bit cell keys in place of
-// cell ids; the cell bounds come from the old sorted key array instead of a cell table.
-__global__ void k_insert_keys_sparse(const float* __restrict__ nxyz, int n, const unsigned char* __restrict__ ins, GridDesc g,
-                                     unsigned long long* __restrict__ keys, int* __restrict__ vals) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    keys[i] = ins[i] ? point_cell_key(nxyz[3 * (size_t)i], nxyz[3 * (size_t)i + 1], nxyz[3 * (size_t)i + 2], g) : kNoCell;
-    vals[i] = i;
-}
-__global__ void k_merge_counts_sparse(const int* __restrict__ dead_before, const unsigned char* __restrict__ dead, int M,
-                                      const unsigned long long* __restrict__ ins_keys_sorted, int n, int* __restrict__ counts) {
-    if (threadIdx.x == 0 && blockIdx.x == 0) {
-        counts[0] = dead_before[M - 1] + dead[M - 1];
-        counts[1] = lower_bound_u64(ins_keys_sorted, n, kNoCell);
+// ---- merge of the sorted map with its dead points and sorted inserts (incremental Add_Points; a delete is the merge
+// with no inserts), on either cell index.  The points stay sorted by cell key: the dense table's cell id, whose "no
+// cell" is ncell, or the sparse index's 64-bit key, whose "no cell" is kNoCell; both sort behind every real cell.
+// Survivors keep their order; inserts go behind their cell's survivors.  The sparse index also carries the keys
+// (keys_old -> keys_new), from which its hash table is rebuilt; the dense table's cell_start comes from
+// k_merge_cell_starts.
+template <bool SPARSE> using CellKey = std::conditional_t<SPARSE, unsigned long long, unsigned>;
+template <bool SPARSE>
+__device__ __forceinline__ CellKey<SPARSE> merge_cell_key(float x, float y, float z, const GridDesc& g) {
+    if constexpr (SPARSE) {
+        return point_cell_key(x, y, z, g);
+    } else {
+        const int cx = grid_axis_cell(x, g.ox, g.inv_cell, g.nx), cy = grid_axis_cell(y, g.oy, g.inv_cell, g.ny),
+                  cz = grid_axis_cell(z, g.oz, g.inv_cell, g.nz);
+        return (unsigned)((cz * g.ny + cy) * g.nx + cx);
     }
 }
-__global__ void k_merge_existing_sparse(const float4* __restrict__ pts_old, const unsigned long long* __restrict__ keys_old,
-                                        const unsigned char* __restrict__ dead, const int* __restrict__ dead_before, int M,
-                                        const unsigned long long* __restrict__ ins_keys_sorted, int n, float4* __restrict__ pts_new,
-                                        float* __restrict__ raw_new, unsigned long long* __restrict__ keys_new) {
+template <bool SPARSE>
+__device__ __forceinline__ CellKey<SPARSE> no_cell(int ncell) {
+    if constexpr (SPARSE) return kNoCell;
+    else return (unsigned)ncell;
+}
+// cell key of every new point ("no cell" for the ones not inserted)
+template <bool SPARSE>
+__global__ void k_insert_keys(const float* __restrict__ nxyz, int n, const unsigned char* __restrict__ ins, GridDesc g, int ncell,
+                              CellKey<SPARSE>* __restrict__ keys, int* __restrict__ vals) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    keys[i] = ins[i] ? merge_cell_key<SPARSE>(nxyz[3 * (size_t)i], nxyz[3 * (size_t)i + 1], nxyz[3 * (size_t)i + 2], g)
+                     : no_cell<SPARSE>(ncell);
+    vals[i] = i;
+}
+// counts[0] = dead points, counts[1] = inserted points (needs dead_before of the last element + its flag)
+template <bool SPARSE>
+__global__ void k_merge_counts(const int* __restrict__ dead_before, const unsigned char* __restrict__ dead, int M,
+                               const CellKey<SPARSE>* __restrict__ ins_keys_sorted, int n, int ncell, int* __restrict__ counts) {
+    if (threadIdx.x == 0 && blockIdx.x == 0) {
+        counts[0] = dead_before[M - 1] + dead[M - 1];
+        counts[1] = lower_bound_key(ins_keys_sorted, n, no_cell<SPARSE>(ncell));
+    }
+}
+// survivor m goes to m - (dead before it) + (inserts sorted before its cell)
+template <bool SPARSE>
+__global__ void k_merge_existing(const float4* __restrict__ pts_old, const CellKey<SPARSE>* __restrict__ keys_old,
+                                 const unsigned char* __restrict__ dead, const int* __restrict__ dead_before, int M, GridDesc g,
+                                 const CellKey<SPARSE>* __restrict__ ins_keys_sorted, int n, float4* __restrict__ pts_new,
+                                 float* __restrict__ raw_new, CellKey<SPARSE>* __restrict__ keys_new) {
     const int m = blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= M || dead[m]) return;
     float4 p = pts_old[m];
-    const unsigned long long key = keys_old[m];
-    const int pos = m - dead_before[m] + lower_bound_u64(ins_keys_sorted, n, key);
+    CellKey<SPARSE> key;
+    if constexpr (SPARSE) key = keys_old[m];
+    else key = merge_cell_key<false>(p.x, p.y, p.z, g);
+    const int pos = m - dead_before[m] + lower_bound_key(ins_keys_sorted, n, key);
     p.w = __int_as_float(pos);
     pts_new[pos] = p;
-    keys_new[pos] = key;
+    if constexpr (SPARSE) keys_new[pos] = key;
     raw_new[3 * (size_t)pos] = p.x; raw_new[3 * (size_t)pos + 1] = p.y; raw_new[3 * (size_t)pos + 2] = p.z;
 }
-__global__ void k_merge_inserts_sparse(const float* __restrict__ nxyz, const unsigned long long* __restrict__ ins_keys_sorted,
-                                       const int* __restrict__ ins_vals_sorted, const int* __restrict__ counts,
-                                       const unsigned long long* __restrict__ keys_old, const int* __restrict__ dead_before, int M,
-                                       float4* __restrict__ pts_new, float* __restrict__ raw_new, unsigned long long* __restrict__ keys_new) {
+// insert k goes behind its cell's survivors: s = the first old position past the cell (from the dense table's old
+// cell_start, or a search of the sparse index's old keys), minus the dead before s, plus the k inserts sorted before it
+template <bool SPARSE>
+__global__ void k_merge_inserts(const float* __restrict__ nxyz, const CellKey<SPARSE>* __restrict__ ins_keys_sorted,
+                                const int* __restrict__ ins_vals_sorted, const int* __restrict__ counts, const int* __restrict__ cell_start_old,
+                                const CellKey<SPARSE>* __restrict__ keys_old, const int* __restrict__ dead_before, int M,
+                                float4* __restrict__ pts_new, float* __restrict__ raw_new, CellKey<SPARSE>* __restrict__ keys_new) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= counts[1]) return;
-    const unsigned long long key = ins_keys_sorted[k];
-    // behind the cell's surviving points: survivors with key <= this one, then the k inserts sorted before this one
-    const int s = lower_bound_u64(keys_old, M, key + 1);
+    const CellKey<SPARSE> key = ins_keys_sorted[k];
+    int s;
+    if constexpr (SPARSE) s = lower_bound_key(keys_old, M, key + 1);
+    else s = cell_start_old[key + 1];
     const int pos = s - (s < M ? dead_before[s] : counts[0]) + k;
     const float* q = nxyz + 3 * (size_t)ins_vals_sorted[k];
     pts_new[pos] = make_float4(q[0], q[1], q[2], __int_as_float(pos));
-    keys_new[pos] = key;
+    if constexpr (SPARSE) keys_new[pos] = key;
     raw_new[3 * (size_t)pos] = q[0]; raw_new[3 * (size_t)pos + 1] = q[1]; raw_new[3 * (size_t)pos + 2] = q[2];
 }
 
