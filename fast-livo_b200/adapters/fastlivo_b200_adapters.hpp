@@ -21,6 +21,8 @@
 //        map_incremental()  src/laserMapping.cpp:692-706  (the uploaded scan into the map, no host transform)
 //   flb::lasermap_fov_segment(h, cube_len, &kdtree_delete_counter)  /  (h, cube_len, pos_lid, &kdtree_delete_counter)
 //        replace lasermap_fov_segment()  src/laserMapping.cpp:363-421  (local-map cube + box delete on the device)
+//   flb::upload_camera_frame(h, bgr, gray_rule)   replaces the resize / img_rgb / cvtColor lines of
+//        LidarSelector::detect  src/lidar_selection.cpp:1029-1037  (one BGR upload; the gray image is made on the device)
 //
 // Type requirements (all met by the reference's types):
 //   Mat3  : operator()(i,j) read/write (Eigen::Matrix3d)          Vec3 : operator()(i) / [i]
@@ -220,6 +222,16 @@ inline flb_vio_params make_vio_params(const Mat3& Rcl, const Vec3& Pcl, const Ma
     p.conv_pos_cm = 0.001f;
     p.force_all_passes = 0;
     return p;
+}
+
+// ---- the camera frame (LidarSelector::detect, src/lidar_selection.cpp:1029-1037) --------------------------------
+// Image: cv::Mat-like BGR8 frame (.data, .cols, .rows, .step) as getImageFromMsg(..., "bgr8") delivers it, at the
+// camera's size or twice it.  The device halves it when needed, keeps the colour frame for flb_colorize(_cloud) with
+// bgr = nullptr and makes the gray image every VIO / visual-map call reads.  gray_rule: FLB_GRAY_CV4 or FLB_GRAY_CV3,
+// the cvtColor of the OpenCV the caller links (CV_VERSION_MAJOR).
+template <class Image>
+inline void upload_camera_frame(flb_handle* h, const Image& bgr, int gray_rule) {
+    check(h, flb_image_upload_bgr(h, bgr.data, bgr.cols, bgr.rows, (int)bgr.step, gray_rule));
 }
 
 template <class Image, class SubMap, class StatesGroup>

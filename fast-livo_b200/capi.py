@@ -168,6 +168,7 @@ class FovParams(C.Structure):
 
 
 CLOUD_SCAN, CLOUD_UNDISTORTED = 0, 1       # flb_world_cloud sources (FLB_CLOUD_*)
+GRAY_CV4, GRAY_CV3 = 0, 1                  # flb_image_upload_bgr's cvtColor rules (FLB_GRAY_*)
 
 # every symbol include/fastlivo_b200.h declares (checked by the CPU-only test tier)
 SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "flb_set_stream", "flb_synchronize", "flb_host_alloc", "flb_host_free",
@@ -183,7 +184,8 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_world_cloud", "flb_world_cloud_download", "flb_vmap_select_cloud", "flb_vmap_grow_cloud", "flb_colorize_cloud",
            "flb_batch_begin", "flb_batch_set_frame", "flb_batch_state_reset_enqueue", "flb_batch_update_enqueue", "flb_batch_state_download",
            "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
-           "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset"]
+           "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset",
+           "flb_image_upload_bgr", "flb_image_download"]
 
 
 def lib_path() -> str:
@@ -240,6 +242,8 @@ def lib():
                                         vp, C.c_int, C.c_int, C.c_int, vp, vp, C.POINTER(C.c_int)]
         L.flb_visual_candidates.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
         L.flb_image_upload.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int]
+        L.flb_image_upload_bgr.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
+        L.flb_image_download.argtypes = [vp, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.flb_patches_upload.argtypes = [vp, vp, vp, vp, C.c_int]
         L.flb_camera_set.argtypes = [vp, C.POINTER(Camera)]
         L.flb_vio_pass.argtypes = [vp, C.POINTER(VioParams), vp, vp, C.c_int, C.POINTER(VioEq)]
@@ -459,6 +463,23 @@ class Handle:
         a = np.ascontiguousarray(gray, np.uint8)
         self._ck(self.L.flb_image_upload(self.h, _p(a), a.shape[1], a.shape[0], a.shape[1]))
 
+    def image_upload_bgr(self, bgr, gray_rule=GRAY_CV4):
+        """flb_image_upload_bgr: a (height, width, 3) uint8 BGR frame at the camera's size or twice it.  A strided view
+        (e.g. a column slice) is passed with its own row stride; its pixels must be contiguous within a row."""
+        a = np.asarray(bgr)
+        if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.strides[1:] != (3, 1) or a.strides[0] < 0:
+            a = np.ascontiguousarray(a, np.uint8)
+        self._ck(self.L.flb_image_upload_bgr(self.h, _p(a), a.shape[1], a.shape[0], a.strides[0], int(gray_rule)))
+
+    def image_download(self, gray=True, bgr=True):
+        """flb_image_download: (gray (H, W) uint8 or None, bgr (H, W, 3) uint8 or None) of the current image set."""
+        w, hgt = C.c_int(), C.c_int()
+        self._ck(self.L.flb_image_download(self.h, None, None, 0, C.byref(w), C.byref(hgt)))
+        g = np.zeros((hgt.value, w.value), np.uint8) if gray else None
+        c = np.zeros((hgt.value, w.value, 3), np.uint8) if bgr else None
+        self._ck(self.L.flb_image_download(self.h, _p(g), _p(c), w.value * hgt.value, None, None))
+        return g, c
+
     def patches_upload(self, pos, patch, level):
         pos = np.ascontiguousarray(pos, np.float64).reshape(-1, 3)
         patch = np.ascontiguousarray(patch, np.float32).reshape(len(pos), 192)
@@ -647,14 +668,15 @@ class Handle:
         R, P, pr, pp = self._pose(Rcw, Pcw)
         self._ck(self.L.flb_vmap_add_observations(self.h, pr, pp, int(frame_id)))
 
-    def colorize(self, Rcw, Pcw, bgr, world_xyz):
-        """flb_colorize: (rgb (n, 3) uint8, valid (n,) bool)."""
+    def colorize(self, Rcw, Pcw, bgr=None, world_xyz=None):
+        """flb_colorize: (rgb (n, 3) uint8, valid (n,) bool).  bgr None: the current image set's colour frame."""
         R, P, pr, pp = self._pose(Rcw, Pcw)
-        img = np.ascontiguousarray(bgr, np.uint8)
+        img = None if bgr is None else np.ascontiguousarray(bgr, np.uint8)
         pts = np.ascontiguousarray(world_xyz, np.float32).reshape(-1, 3)
         rgb = np.zeros((len(pts), 3), np.uint8)
         val = np.zeros(len(pts), np.uint8)
-        self._ck(self.L.flb_colorize(self.h, pr, pp, _p(img), img.shape[1] * 3, _p(pts), len(pts), 3, _p(rgb), _p(val)))
+        self._ck(self.L.flb_colorize(self.h, pr, pp, _p(img), 0 if img is None else img.shape[1] * 3, _p(pts), len(pts), 3, _p(rgb),
+                                     _p(val)))
         return rgb, val.astype(bool)
 
     # ---- the frame's world cloud (pcl_wait_pub) on the device
@@ -690,13 +712,14 @@ class Handle:
         R, P, pr, pp = self._pose(Rcw, Pcw)
         self._ck(self.L.flb_vmap_grow_cloud(self.h, pr, pp, int(frame_id)))
 
-    def colorize_cloud(self, Rcw, Pcw, bgr):
-        """flb_colorize_cloud: (rgb (n, 3) uint8, valid (n,) bool) of the world cloud."""
+    def colorize_cloud(self, Rcw, Pcw, bgr=None):
+        """flb_colorize_cloud: (rgb (n, 3) uint8, valid (n,) bool) of the world cloud.  bgr None: the current image
+        set's colour frame."""
         R, P, pr, pp = self._pose(Rcw, Pcw)
-        img = np.ascontiguousarray(bgr, np.uint8)
+        img = None if bgr is None else np.ascontiguousarray(bgr, np.uint8)
         rgb = np.zeros((self._wc_n, 3), np.uint8)
         val = np.zeros(self._wc_n, np.uint8)
-        self._ck(self.L.flb_colorize_cloud(self.h, pr, pp, _p(img), img.shape[1] * 3, _p(rgb), _p(val)))
+        self._ck(self.L.flb_colorize_cloud(self.h, pr, pp, _p(img), 0 if img is None else img.shape[1] * 3, _p(rgb), _p(val)))
         return rgb, val.astype(bool)
 
     def vmap_counts(self):

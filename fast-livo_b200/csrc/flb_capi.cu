@@ -287,6 +287,13 @@ struct flb_handle {
     // VIO inputs
     int img_w = 0, img_h = 0;
     DevBuf<unsigned char> img, img_alt;
+    // a set's colour frame (img_rgb, W x H x 3) beside its gray image: flb_image_upload_bgr fills both, flb_image_upload
+    // only the gray one (img_bgr_valid = false); the two swap together
+    DevBuf<unsigned char> img_bgr, img_bgr_alt;
+    bool img_bgr_valid = false;
+    // flb_image_upload_bgr's raw frame on the device.  Its H2D copy and k_image_prep, its only reader, both run on
+    // copy_stream, so the next frame's copy into it is ordered after that kernel: stream order is its reuse fence.
+    DevBuf<unsigned char> img_raw;
     int Pn = 0;
     DevBuf<double> patch_pos, patch_pos_alt;
     DevBuf<float> patch_ref, patch_ref_alt;
@@ -1030,7 +1037,7 @@ int flb_destroy(flb_handle* h) {
     h->plane_ok.release(); h->plane.release(); h->x_world.release(); h->x_nn_d2.release(); h->x_pd2.release();
     h->x_nn_idx.release(); h->x_rowmask.release(); h->x_rows.release(); h->x_meas.release(); h->partials.release();
     h->packed.release(); h->pose12.release(); h->prior.release(); h->scan_raw.release(); h->skeys.release(); h->skeys_sorted.release(); h->svals.release(); h->svals_sorted.release(); h->x_pabcd.release(); h->G_last.release(); h->states.release();
-    h->lio_ctrl.release(); h->vio_ctrl.release(); h->ik_states.release(); h->ik_ctrl.release(); h->barrier.release(); h->pkt.release(); h->arrive_lines.release(); h->trace.release(); h->dbg.release(); h->dbg_vio.release(); h->imu_buf.release(); h->imu_pts.release(); h->imu_heads.release(); h->vm_key.release(); h->vm_val.release(); h->vm_pts.release(); h->vm_win.release(); h->vm_pose.release(); h->img.release(); h->patch_pos.release(); h->patch_ref.release();
+    h->lio_ctrl.release(); h->vio_ctrl.release(); h->ik_states.release(); h->ik_ctrl.release(); h->barrier.release(); h->pkt.release(); h->arrive_lines.release(); h->trace.release(); h->dbg.release(); h->dbg_vio.release(); h->imu_buf.release(); h->imu_pts.release(); h->imu_heads.release(); h->vm_key.release(); h->vm_val.release(); h->vm_pts.release(); h->vm_win.release(); h->vm_pose.release(); h->img.release(); h->img_bgr.release(); h->img_bgr_alt.release(); h->img_raw.release(); h->patch_pos.release(); h->patch_ref.release();
     h->patch_level.release(); h->errors.release(); h->err_units.release(); h->errors_all.release(); h->x_z.release(); h->x_H.release();
     h->st_map.release(); h->st_scan.release(); h->st_img.release(); h->st_patch.release(); h->st_state.release();
     h->st_misc.release(); h->pin_out.release();
@@ -2605,10 +2612,77 @@ int flb_image_upload(flb_handle* h, const uint8_t* gray, int width, int height, 
     if (!direct) FLB_CUDA(h, h->st_img.mark(h->copy_stream));
     { int rcq = vio_copy_end(h); if (rcq) return rcq; }
     std::swap(h->img, h->img_alt);
+    std::swap(h->img_bgr, h->img_bgr_alt);
+    h->img_bgr_valid = false;
     h->img_slot.slot ^= 1;
     h->img_w = width;
     h->img_h = height;
     h->last_vio_valid = false;
+    return FLB_OK;
+}
+
+int flb_image_upload_bgr(flb_handle* h, const uint8_t* bgr, int width, int height, int stride_bytes, int gray_rule) {
+    FLB_CHECK_H(h);
+    if (!h->cam_set) return fail(h, FLB_ERR_STATE, "flb_image_upload_bgr: flb_camera_set first");
+    const int W = h->cam.width, H = h->cam.height;
+    const bool halve = (width == 2 * W && height == 2 * H);
+    if (!bgr || !(halve || (width == W && height == H)) || stride_bytes < 3 * width || (gray_rule != kGrayCv4 && gray_rule != kGrayCv3))
+        return fail(h, FLB_ERR_INVALID, "flb_image_upload_bgr: bad arguments (%dx%d, stride %d, rule %d; camera %dx%d)", width, height,
+                    stride_bytes, gray_rule, W, H);
+    const size_t row = (size_t)width * 3, raw_bytes = row * height, px = (size_t)W * H;
+    FLB_CUDA(h, h->img_raw.reserve(raw_bytes));
+    FLB_CUDA(h, h->img_alt.reserve(px));
+    FLB_CUDA(h, h->img_bgr_alt.reserve(px * 3));
+    // the raw frame goes up before the wait for the idle set's readers: only k_image_prep has to wait for them
+    if (is_pinned(bgr)) {
+        FLB_CUDA(h, cudaMemcpy2DAsync(h->img_raw.p, row, bgr, stride_bytes, row, height, cudaMemcpyHostToDevice, h->copy_stream));
+    } else {
+        void* stv = nullptr;
+        FLB_CUDA(h, h->st_img.acquire(raw_bytes, &stv));
+        unsigned char* st = static_cast<unsigned char*>(stv);
+        if ((size_t)stride_bytes == row) std::memcpy(st, bgr, raw_bytes);
+        else for (int r = 0; r < height; ++r) std::memcpy(st + (size_t)r * row, bgr + (size_t)r * stride_bytes, row);
+        FLB_CUDA(h, cudaMemcpyAsync(h->img_raw.p, st, raw_bytes, cudaMemcpyHostToDevice, h->copy_stream));
+        FLB_CUDA(h, h->st_img.mark(h->copy_stream));
+    }
+    { int rcq = vio_copy_begin(h, h->img_slot); if (rcq) return rcq; }
+    {
+        const dim3 grid((unsigned)((W + 4 * 128 - 1) / (4 * 128)), (unsigned)std::min(H, 65535));
+        const bool vec = (W % 4) == 0;
+        if (halve) {
+            if (vec) k_image_prep<true, true><<<grid, 128, 0, h->copy_stream>>>(h->img_raw.p, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
+            else k_image_prep<true, false><<<grid, 128, 0, h->copy_stream>>>(h->img_raw.p, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
+        } else {
+            if (vec) k_image_prep<false, true><<<grid, 128, 0, h->copy_stream>>>(h->img_raw.p, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
+            else k_image_prep<false, false><<<grid, 128, 0, h->copy_stream>>>(h->img_raw.p, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
+        }
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches++;
+    }
+    { int rcq = vio_copy_end(h); if (rcq) return rcq; }
+    std::swap(h->img, h->img_alt);
+    std::swap(h->img_bgr, h->img_bgr_alt);
+    h->img_bgr_valid = true;
+    h->img_slot.slot ^= 1;
+    h->img_w = W;
+    h->img_h = H;
+    h->last_vio_valid = false;
+    return FLB_OK;
+}
+
+int flb_image_download(flb_handle* h, uint8_t* gray, uint8_t* bgr, int capacity_pixels, int* width, int* height) {
+    FLB_CHECK_H(h);
+    if (h->img_w <= 0) return fail(h, FLB_ERR_STATE, "flb_image_download: no image uploaded");
+    if (bgr && !h->img_bgr_valid) return fail(h, FLB_ERR_STATE, "flb_image_download: the current image has no colour frame (flb_image_upload)");
+    const size_t px = (size_t)h->img_w * h->img_h;
+    if ((gray || bgr) && (capacity_pixels < 0 || (size_t)capacity_pixels < px))
+        return fail(h, FLB_ERR_INVALID, "flb_image_download: capacity %d < %zu pixels", capacity_pixels, px);
+    { int rcq = vio_inputs_acquire(h); if (rcq) return rcq; }
+    if (gray) FLB_CUDA(h, cudaMemcpyAsync(gray, h->img.p, px, cudaMemcpyDeviceToHost, h->stream));
+    if (bgr) FLB_CUDA(h, cudaMemcpyAsync(bgr, h->img_bgr.p, px * 3, cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (width) *width = h->img_w;
+    if (height) *height = h->img_h;
     return FLB_OK;
 }
 
@@ -3716,21 +3790,29 @@ int colorize_pose(flb_handle* h, const char* who, const double* Rcw, const doubl
     return vm_set_pose(h, Rcw, Pcw);
 }
 
-// The colour image upload, the per-point kernel and the download of rgb / valid for n >= 1 device points xyz.
+// The per-point kernel and the download of rgb / valid for n >= 1 device points xyz.  The colour image: the caller's
+// bgr, uploaded ahead of rgb / valid; bgr == NULL: the current image set's colour frame (flb_image_upload_bgr), read in
+// place once its upload has landed.
 int colorize_dev(flb_handle* h, const uint8_t* bgr, int stride_bytes, const float* xyz, int n, uint8_t* rgb, uint8_t* valid) {
     auto& vm = h->vm;
     const int W = h->cam.width, H = h->cam.height;
-    const size_t img_bytes = (size_t)W * H * 3;
-    FLB_CUDA(h, h->x_rowmask.reserve(img_bytes + (size_t)n * 4));     // colour image | rgb | valid
-    unsigned char* d_img = h->x_rowmask.p;
-    unsigned char* d_rgb = d_img + img_bytes;
+    const size_t img_bytes = bgr ? (size_t)W * H * 3 : 0;
+    FLB_CUDA(h, h->x_rowmask.reserve(img_bytes + (size_t)n * 4));     // [colour image |] rgb | valid
+    const unsigned char* d_img = h->img_bgr.p;
+    unsigned char* d_rgb = h->x_rowmask.p + img_bytes;
     unsigned char* d_val = d_rgb + (size_t)n * 3;
-    void* stv = nullptr;
-    FLB_CUDA(h, h->st_img.acquire(img_bytes, &stv));
-    unsigned char* st = static_cast<unsigned char*>(stv);
-    for (int r = 0; r < H; ++r) std::memcpy(st + (size_t)r * W * 3, bgr + (size_t)r * stride_bytes, (size_t)W * 3);
-    FLB_CUDA(h, cudaMemcpyAsync(d_img, st, img_bytes, cudaMemcpyHostToDevice, h->stream));
-    FLB_CUDA(h, h->st_img.mark(h->stream));
+    if (bgr) {
+        d_img = h->x_rowmask.p;
+        void* stv = nullptr;
+        FLB_CUDA(h, h->st_img.acquire(img_bytes, &stv));
+        unsigned char* st = static_cast<unsigned char*>(stv);
+        for (int r = 0; r < H; ++r) std::memcpy(st + (size_t)r * W * 3, bgr + (size_t)r * stride_bytes, (size_t)W * 3);
+        FLB_CUDA(h, cudaMemcpyAsync(h->x_rowmask.p, st, img_bytes, cudaMemcpyHostToDevice, h->stream));
+        FLB_CUDA(h, h->st_img.mark(h->stream));
+    } else {
+        int rcq = vio_inputs_acquire(h);
+        if (rcq) return rcq;
+    }
     {
         LaunchScope ls(h, FAM_OTHER);
         k_vm_colorize<<<(n + 255) / 256, 256, 0, h->stream>>>(h->cam, vm.pose.p, d_img, xyz, n, d_rgb, d_val);
@@ -3745,6 +3827,13 @@ int colorize_dev(flb_handle* h, const uint8_t* bgr, int stride_bytes, const floa
     return FLB_OK;
 }
 
+// bgr == NULL needs a colour frame of the camera's size in the current image set
+int colorize_frame_check(flb_handle* h, const char* who, const uint8_t* bgr) {
+    if (!bgr && !(h->img_bgr_valid && h->img_w == h->cam.width && h->img_h == h->cam.height))
+        return fail(h, FLB_ERR_STATE, "%s: bgr == NULL needs the current image from flb_image_upload_bgr at the camera's size", who);
+    return FLB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -3754,8 +3843,9 @@ int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const 
     FLB_CHECK_H(h);
     if (!h->cam_set) return fail(h, FLB_ERR_STATE, "flb_colorize: flb_camera_set first");
     const int W = h->cam.width;
-    if (!bgr || stride_bytes < 3 * W || n < 0 || (n > 0 && (!world_xyz || !rgb || !valid)) || stride < 3)
+    if ((bgr && stride_bytes < 3 * W) || n < 0 || (n > 0 && (!world_xyz || !rgb || !valid)) || stride < 3)
         return fail(h, FLB_ERR_INVALID, "flb_colorize: bad arguments");
+    { int rc = colorize_frame_check(h, "flb_colorize", bgr); if (rc) return rc; }
     if (n == 0) return FLB_OK;
     { int rc = colorize_pose(h, "flb_colorize", Rcw, Pcw); if (rc) return rc; }
     { int rc = vm_upload_points(h, world_xyz, n, stride); if (rc) return rc; }
@@ -3769,7 +3859,8 @@ int flb_colorize_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], 
     if (!h->cam_set) return fail(h, FLB_ERR_STATE, "flb_colorize_cloud: flb_camera_set first");
     { int rc = wc_check(h, "flb_colorize_cloud"); if (rc) return rc; }
     const int n = h->wc_n;
-    if (!bgr || stride_bytes < 3 * h->cam.width || (n > 0 && (!rgb || !valid))) return fail(h, FLB_ERR_INVALID, "flb_colorize_cloud: bad arguments");
+    if ((bgr && stride_bytes < 3 * h->cam.width) || (n > 0 && (!rgb || !valid))) return fail(h, FLB_ERR_INVALID, "flb_colorize_cloud: bad arguments");
+    { int rc = colorize_frame_check(h, "flb_colorize_cloud", bgr); if (rc) return rc; }
     if (n == 0) return FLB_OK;
     { int rc = colorize_pose(h, "flb_colorize_cloud", Rcw, Pcw); if (rc) return rc; }
     return colorize_dev(h, bgr, stride_bytes, h->wc_xyz.p, n, rgb, valid);

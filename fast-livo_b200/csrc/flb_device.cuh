@@ -1615,4 +1615,16 @@ FLB_HD void ikfom_boxminus(const StateIkfom& a, const StateIkfom& b, double* res
     s2_boxminus(a.grav, b.grav, res + 21);
 }
 
+// ------------------------------------------------------------------ camera frame preparation (LidarSelector::detect)
+// cv::cvtColor(img, img, CV_BGR2GRAY) on 8-bit BGR (src/lidar_selection.cpp:1037): OpenCV's fixed-point weights, with
+// the rounding shift of the OpenCV generation the caller links (FLB_GRAY_CV4 / FLB_GRAY_CV3 in the C ABI).
+enum { kGrayCv4 = 0, kGrayCv3 = 1 };
+FLB_HD unsigned bgr_to_gray(unsigned b, unsigned g, unsigned r, int rule) {
+    return rule == kGrayCv3 ? (1868u * b + 9617u * g + 4899u * r + (1u << 13)) >> 14
+                            : (3735u * b + 19235u * g + 9798u * r + (1u << 14)) >> 15;
+}
+// cv::resize(img, img, Size(), 0.5, 0.5, INTER_LINEAR) of an even-sized 8-bit frame (:1031-1034): OpenCV takes its
+// 2x2 area path there, one rounded mean per channel of each 2x2 source block.
+FLB_HD unsigned mean2x2(unsigned a, unsigned b, unsigned c, unsigned d) { return (a + b + c + d + 2u) >> 2; }
+
 }  // namespace flb

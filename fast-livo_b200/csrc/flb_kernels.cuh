@@ -3453,4 +3453,73 @@ __global__ void __launch_bounds__(BLOCK) k_lio_update_ikfom_persistent(LioArgs a
     }
 }
 
+// ---- camera frame preparation (flb_image_upload_bgr) ----------------------------------------------------------------
+// LidarSelector::detect's resize + cvtColor (src/lidar_selection.cpp:1029-1037) of one BGR8 frame held dense in `raw`
+// (W x H pixels, or 2W x 2H when HALVE) into the camera-size colour frame (img_rgb) and its gray image, both dense.
+// A thread makes 4 consecutive output pixels of a row; rows stride by gridDim.y.  VEC (W % 4 == 0, so every address
+// below is a multiple of 4): all loads and stores are 32-bit words, 3 per thread at 1x and 12 at 2x in, 4 out.
+template <bool HALVE, bool VEC>
+__global__ void __launch_bounds__(128) k_image_prep(const unsigned char* __restrict__ raw, int W, int H, int rule,
+                                                    unsigned char* __restrict__ bgr, unsigned char* __restrict__ gray) {
+    const int x0 = 4 * (blockIdx.x * blockDim.x + threadIdx.x);
+    if (x0 >= W) return;
+    const int n = min(4, W - x0);
+    auto byte = [](const unsigned* w, int j) { return (w[j >> 2] >> (8 * (j & 3))) & 0xffu; };
+    for (int y = blockIdx.y; y < H; y += gridDim.y) {
+        unsigned c[12] = {};                  // b, g, r of the 4 output pixels
+        if (HALVE) {
+            const size_t pitch = (size_t)6 * W;
+            const unsigned char* s0 = raw + (size_t)(2 * y) * pitch + (size_t)6 * x0;
+            const unsigned char* s1 = s0 + pitch;
+            if (VEC) {
+                unsigned a[6], b[6];
+#pragma unroll
+                for (int k = 0; k < 6; ++k) { a[k] = reinterpret_cast<const unsigned*>(s0)[k]; b[k] = reinterpret_cast<const unsigned*>(s1)[k]; }
+#pragma unroll
+                for (int j = 0; j < 12; ++j) {
+                    const int s = 6 * (j / 3) + j % 3;   // left source pixel of output pixel j / 3, channel j % 3
+                    c[j] = mean2x2(byte(a, s), byte(a, s + 3), byte(b, s), byte(b, s + 3));
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < 12; ++j) {
+                    const int s = 6 * (j / 3) + j % 3;
+                    if (j < 3 * n) c[j] = mean2x2(s0[s], s0[s + 3], s1[s], s1[s + 3]);
+                }
+            }
+        } else {
+            const unsigned char* s = raw + ((size_t)y * W + x0) * 3;
+            if (VEC) {
+                unsigned a[3];
+#pragma unroll
+                for (int k = 0; k < 3; ++k) a[k] = reinterpret_cast<const unsigned*>(s)[k];
+#pragma unroll
+                for (int j = 0; j < 12; ++j) c[j] = byte(a, j);
+            } else {
+#pragma unroll
+                for (int j = 0; j < 12; ++j)
+                    if (j < 3 * n) c[j] = s[j];
+            }
+        }
+        unsigned char* ob = bgr + ((size_t)y * W + x0) * 3;
+        unsigned char* og = gray + (size_t)y * W + x0;
+        if (VEC) {
+            unsigned gw = 0;
+#pragma unroll
+            for (int k = 0; k < 3; ++k)
+                reinterpret_cast<unsigned*>(ob)[k] = c[4 * k] | (c[4 * k + 1] << 8) | (c[4 * k + 2] << 16) | (c[4 * k + 3] << 24);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) gw |= bgr_to_gray(c[3 * i], c[3 * i + 1], c[3 * i + 2], rule) << (8 * i);
+            *reinterpret_cast<unsigned*>(og) = gw;
+        } else {
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+                if (i < n) {
+                    ob[3 * i] = (unsigned char)c[3 * i]; ob[3 * i + 1] = (unsigned char)c[3 * i + 1]; ob[3 * i + 2] = (unsigned char)c[3 * i + 2];
+                    og[i] = (unsigned char)bgr_to_gray(c[3 * i], c[3 * i + 1], c[3 * i + 2], rule);
+                }
+        }
+    }
+}
+
 }  // namespace flb

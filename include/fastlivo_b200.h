@@ -329,8 +329,30 @@ typedef struct flb_vio_eq {
     int     skipped;
 } flb_vio_eq;
 
-/* cv::Mat img of LidarSelector::detect (src/lidar_selection.cpp:1027-1037): gray uint8. */
+/* cv::Mat img of LidarSelector::detect (src/lidar_selection.cpp:1027-1037): gray uint8.  The image set it makes current
+ * holds no colour frame (flb_colorize / flb_colorize_cloud with bgr == NULL refuse it). */
 int flb_image_upload(flb_handle* h, const uint8_t* gray, int width, int height, int stride_bytes);
+/* The first lines of LidarSelector::detect (src/lidar_selection.cpp:1029-1037) on the device: the camera frame as the
+ * driver delivers it (getImageFromMsg(..., "bgr8"), src/laserMapping.cpp:490-493), halved by cv::resize(0.5,
+ * INTER_LINEAR) when its size differs from the camera's, kept as img_rgb and converted by cv::cvtColor(CV_BGR2GRAY).
+ * The current image set then holds the camera-size gray image, byte-identical to flb_image_upload of OpenCV's
+ * cvtColor(resize(bgr)), so every reader of the image works unchanged, and the camera-size BGR frame, which
+ * flb_colorize / flb_colorize_cloud read with bgr == NULL (publish_frame_world_rgb, :727-744).
+ *   (width, height) = the camera's (no resize), or exactly twice it (each output channel is OpenCV's 2x2 area mean
+ *   (a + b + c + d + 2) >> 2, what cv::resize does for an even-sized frame at scale 0.5).  stride_bytes >= 3 * width.
+ *   gray_rule: the fixed-point cvtColor of the OpenCV the caller links (the reference asks for OpenCV >= 3.2).
+ * The same rules as flb_image_upload: the frame fills the idle one of two device sets on the copy stream and never
+ * waits for the update that is running; a page-locked source is read in place (keep it until the next synchronise), a
+ * pageable one is free on return.  Needs flb_camera_set (FLB_ERR_STATE).  FLB_ERR_INVALID: bgr NULL, any other size,
+ * stride_bytes < 3 * width, an unknown gray_rule.  On any error the previous image set stays current and unchanged.
+ * Odd-sized frames (OpenCV's general bilinear path) and encodings other than BGR8 are not handled. */
+#define FLB_GRAY_CV4 0   /* (3735 B + 19235 G + 9798 R + 2^14) >> 15: OpenCV 4.x */
+#define FLB_GRAY_CV3 1   /* (1868 B + 9617 G + 4899 R + 2^13) >> 14: OpenCV 3.x  */
+int flb_image_upload_bgr(flb_handle* h, const uint8_t* bgr, int width, int height, int stride_bytes, int gray_rule);
+/* test / debugging aid (blocking): the current image set's gray (W*H) and colour (W*H*3) frames; either pointer may be
+ * NULL.  capacity_pixels >= W*H when either is given.  *width / *height (may be NULL) = W, H.  FLB_ERR_STATE: no image
+ * yet, or bgr != NULL for an image from flb_image_upload. */
+int flb_image_download(flb_handle* h, uint8_t* gray, uint8_t* bgr, int capacity_pixels, int* width, int* height);
 /* SubSparseMap (include/common_lib.h:263-292) flattened: pos Pn x 3 (Point::pos_),
  * patch Pn x 3 x 64 floats (warpAffine layout, src/lidar_selection.cpp:279-295),
  * search_level Pn. */
@@ -395,7 +417,9 @@ int flb_vmap_grow(flb_handle* h, const double Rcw[9], const double Pcw[3], const
 int flb_vmap_add_observations(flb_handle* h, const double Rcw[9], const double Pcw[3], int frame_id);
 /* publish_frame_world_rgb (src/laserMapping.cpp:710-745): colour every world point that projects into the current
  * frame with the bilinear BGR sample of LidarSelector::getpixel (src/lidar_selection.cpp:1007-1025).  bgr: the
- * colour frame (img_rgb), 3 bytes per pixel; rgb: n x 3 bytes (r, g, b as the reference stores them); valid[i] = 1
+ * colour frame (img_rgb), 3 bytes per pixel, uploaded by the call; or NULL: the colour frame of the current image set
+ * (flb_image_upload_bgr), read on the device with no host copy and no upload (FLB_ERR_STATE when the current image came
+ * from flb_image_upload or does not match the camera's size); rgb: n x 3 bytes (r, g, b as the reference stores them); valid[i] = 1
  * for the points the reference pushes into laserCloudWorldRGB (in front of the camera, inside the image), whose order
  * is the input order.  Rcw / Pcw NULL: from the device state (after flb_vmap_reset).  Blocking. */
 int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, const float* world_xyz, int n,
