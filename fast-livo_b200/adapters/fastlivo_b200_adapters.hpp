@@ -23,6 +23,11 @@
 //        replace lasermap_fov_segment()  src/laserMapping.cpp:363-421  (local-map cube + box delete on the device)
 //   flb::upload_camera_frame(h, bgr, gray_rule)   replaces the resize / img_rgb / cvtColor lines of
 //        LidarSelector::detect  src/lidar_selection.cpp:1029-1037  (one BGR upload; the gray image is made on the device)
+//   flb::preprocess(h, livox_msg, n_scans, blind, point_filter_num)  /  flb::preprocess(h, pc2_msg, kind, n_scans, blind,
+//        point_filter_num)   replace p_pre->process (src/preprocess.cpp:43-70) and the sort of sync_packages
+//        (src/laserMapping.cpp:551): the driver's records go up as they are; the cloud is decoded and sorted on the device
+//   flb::undistort_pcl_from_lidar(h, prm, carry, v_imu, lidar_meas, state_inout)   replaces UndistortPcl from :621 on
+//        with that device cloud as lidar_meas.lidar (the window, the LidarMeasureGroup bookkeeping, the propagation)
 //
 // Type requirements (all met by the reference's types):
 //   Mat3  : operator()(i,j) read/write (Eigen::Matrix3d)          Vec3 : operator()(i) / [i]
@@ -387,6 +392,98 @@ inline int downsample_scan(flb_handle* h, float filter_size_surf_min) {
     int n = 0;
     check(h, flb_scan_from_undistorted(h, filter_size_surf_min, &n));
     return n;
+}
+
+// ---- the driver's LiDAR message (Preprocess::process, src/preprocess.cpp:43-70, with feature_extract_enable = 0) ----
+struct LidarInfo {
+    int n_points;            // pl_surf.size(): sync_packages skips the message when it is <= 1 (src/laserMapping.cpp:538)
+    float last_offset_ms;    // points.back().curvature after the sort, for lidar_end_time (:553)
+};
+
+// livox_ros_driver::CustomMsg (.points, .point_num): avia_handler.  CustomPoint is offset_time, x, y, z, reflectivity,
+// tag, line; the offsets are taken from the type itself.
+template <class LivoxMsg>
+inline LidarInfo preprocess(flb_handle* h, const LivoxMsg& msg, int n_scans, double blind, int point_filter_num) {
+    flb_lidar_format f{};
+    f.kind = FLB_LIDAR_LIVOX;
+    f.point_step = (int)sizeof(msg.points[0]);
+    LidarInfo r{};
+    const int n = (int)msg.point_num;
+    if (n > 0) {
+        const char* p0 = reinterpret_cast<const char*>(&msg.points[0]);
+        f.off_time = (int)(reinterpret_cast<const char*>(&msg.points[0].offset_time) - p0);
+        f.off_x = (int)(reinterpret_cast<const char*>(&msg.points[0].x) - p0);
+        f.off_y = (int)(reinterpret_cast<const char*>(&msg.points[0].y) - p0);
+        f.off_z = (int)(reinterpret_cast<const char*>(&msg.points[0].z) - p0);
+        f.off_tag = (int)(reinterpret_cast<const char*>(&msg.points[0].tag) - p0);
+        f.off_line = (int)(reinterpret_cast<const char*>(&msg.points[0].line) - p0);
+    } else {
+        f.off_x = 4, f.off_y = 8, f.off_z = 12, f.off_tag = 17, f.off_line = 18;
+    }
+    f.n_scans = n_scans;
+    f.point_filter_num = point_filter_num;
+    f.blind = blind;
+    check(h, flb_lidar_upload(h, &f, n > 0 ? &msg.points[0] : nullptr, n, &r.n_points, &r.last_offset_ms));
+    return r;
+}
+
+// sensor_msgs::PointCloud2 (.fields[].name / .offset, .point_step, .width, .height, .data): oust64_handler,
+// velodyne_handler (clouds with per-point times) or xt32_handler by `kind` (FLB_LIDAR_*).  The time field is the one
+// the handler's point type names: t (Ouster), time (Velodyne), timestamp (XT32).
+template <class PointCloud2>
+inline LidarInfo preprocess(flb_handle* h, const PointCloud2& msg, int kind, int n_scans, double blind, int point_filter_num) {
+    flb_lidar_format f{};
+    f.kind = kind;
+    f.point_step = (int)msg.point_step;
+    f.off_x = f.off_y = f.off_z = f.off_time = -1;
+    const char* time_name = kind == FLB_LIDAR_OUSTER ? "t" : (kind == FLB_LIDAR_VELODYNE ? "time" : "timestamp");
+    for (const auto& fld : msg.fields) {
+        if (fld.name == "x") f.off_x = (int)fld.offset;
+        else if (fld.name == "y") f.off_y = (int)fld.offset;
+        else if (fld.name == "z") f.off_z = (int)fld.offset;
+        else if (fld.name == time_name) f.off_time = (int)fld.offset;
+    }
+    f.n_scans = n_scans;
+    f.point_filter_num = point_filter_num;
+    f.blind = blind;
+    LidarInfo r{};
+    const int n = (int)((size_t)msg.width * msg.height);
+    check(h, flb_lidar_upload(h, &f, n > 0 ? msg.data.data() : nullptr, n, &r.n_points, &r.last_offset_ms));
+    return r;
+}
+
+// ImuProcess::UndistortPcl from :621 on, with the cloud of flb::preprocess as lidar_meas.lidar.  lidar_meas needs
+// .lidar_beg_time, .last_update_time, .is_lidar_end, .lidar_scan_index_now and .measures.back().img_offset_time
+// (include/common_lib.h's LidarMeasureGroup); last_offset_ms is LidarInfo's.  Returns pcl_out.size(); the undistorted
+// points stay on the device for flb::downsample_scan / flb_world_cloud(FLB_CLOUD_UNDISTORTED).
+template <class ImuDeque, class LidarMeasureGroup, class StatesGroup>
+inline int undistort_pcl_from_lidar(flb_handle* h, const flb_imu_params& prm, flb_imu_carry& carry, const ImuDeque& v_imu,
+                                    LidarMeasureGroup& lidar_meas, float last_offset_ms, StatesGroup& state_inout) {
+    const double pcl_beg_time = lidar_meas.lidar_beg_time > lidar_meas.last_update_time ? lidar_meas.lidar_beg_time
+                                                                                        : lidar_meas.last_update_time;   // :621
+    const double pcl_end_time = lidar_meas.is_lidar_end ? lidar_meas.lidar_beg_time + last_offset_ms / double(1000)
+                                                        : lidar_meas.lidar_beg_time + lidar_meas.measures.back().img_offset_time;   // :628-630
+    const double pcl_offset_time = lidar_meas.is_lidar_end ? (pcl_end_time - lidar_meas.lidar_beg_time) * double(1000) : 0.0;   // :631-633
+    std::vector<flb_imu_sample> s;
+    s.reserve(v_imu.size());
+    for (const auto& m : v_imu) {
+        flb_imu_sample e;
+        e.t = m->header.stamp.toSec();
+        e.gyr[0] = m->angular_velocity.x; e.gyr[1] = m->angular_velocity.y; e.gyr[2] = m->angular_velocity.z;
+        e.acc[0] = m->linear_acceleration.x; e.acc[1] = m->linear_acceleration.y; e.acc[2] = m->linear_acceleration.z;
+        s.push_back(e);
+    }
+    flb_state18 x{};
+    to_abi(state_inout, x);
+    check(h, flb_state_upload(h, &x, &x));
+    int n_taken = 0;
+    check(h, flb_imu_undistort_lidar(h, &prm, &carry, s.data(), (int)s.size(), pcl_beg_time, pcl_end_time, pcl_offset_time,
+                                     lidar_meas.is_lidar_end ? 1 : 0, &n_taken, nullptr, 0, nullptr, nullptr));
+    check(h, flb_state_download(h, &x, nullptr, nullptr));
+    from_abi(x, state_inout);
+    lidar_meas.last_update_time = pcl_end_time;                                                   // :642
+    lidar_meas.lidar_scan_index_now = lidar_meas.is_lidar_end ? 0 : lidar_meas.lidar_scan_index_now + n_taken;   // :638, :643-646
+    return n_taken;
 }
 
 }  // namespace flb

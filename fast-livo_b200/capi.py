@@ -43,6 +43,13 @@ class ImuCarry(C.Structure):
     _fields_ = [("last_lidar_end_time", C.c_double), ("acc_s_last", C.c_double * 3), ("angvel_last", C.c_double * 3)]
 
 
+class LidarFormat(C.Structure):
+    """flb_lidar_format: where the fields of one driver record sit, and Preprocess's parameters."""
+    _fields_ = [("kind", C.c_int), ("point_step", C.c_int), ("off_x", C.c_int), ("off_y", C.c_int), ("off_z", C.c_int),
+                ("off_time", C.c_int), ("off_tag", C.c_int), ("off_line", C.c_int), ("n_scans", C.c_int),
+                ("point_filter_num", C.c_int), ("blind", C.c_double)]
+
+
 class State18(C.Structure):
     _fields_ = [("rot", C.c_double * 9), ("pos", C.c_double * 3), ("vel", C.c_double * 3),
                 ("bg", C.c_double * 3), ("ba", C.c_double * 3), ("grav", C.c_double * 3),
@@ -168,6 +175,7 @@ class FovParams(C.Structure):
 
 
 CLOUD_SCAN, CLOUD_UNDISTORTED = 0, 1       # flb_world_cloud sources (FLB_CLOUD_*)
+LIDAR_LIVOX, LIDAR_VELODYNE, LIDAR_OUSTER, LIDAR_XT32 = 1, 2, 3, 4    # flb_lidar_format.kind (FLB_LIDAR_*)
 GRAY_CV4, GRAY_CV3 = 0, 1                  # flb_image_upload_bgr's cvtColor rules (FLB_GRAY_*)
 
 # every symbol include/fastlivo_b200.h declares (checked by the CPU-only test tier)
@@ -185,7 +193,8 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_batch_begin", "flb_batch_set_frame", "flb_batch_state_reset_enqueue", "flb_batch_update_enqueue", "flb_batch_state_download",
            "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
            "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset",
-           "flb_image_upload_bgr", "flb_image_download"]
+           "flb_image_upload_bgr", "flb_image_download",
+           "flb_lidar_upload", "flb_lidar_download", "flb_imu_undistort_lidar"]
 
 
 def lib_path() -> str:
@@ -240,6 +249,10 @@ def lib():
         L.flb_lio_update_ikfom.argtypes = [vp, C.POINTER(IkfomParams), C.POINTER(StateIkfom), C.POINTER(IkfomReport)]
         L.flb_imu_undistort.argtypes = [vp, C.POINTER(ImuParams), C.POINTER(ImuCarry), vp, C.c_int, C.c_double, C.c_double,
                                         vp, C.c_int, C.c_int, C.c_int, vp, vp, C.POINTER(C.c_int)]
+        L.flb_lidar_upload.argtypes = [vp, C.POINTER(LidarFormat), vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_float)]
+        L.flb_lidar_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_imu_undistort_lidar.argtypes = [vp, C.POINTER(ImuParams), C.POINTER(ImuCarry), vp, C.c_int, C.c_double, C.c_double,
+                                              C.c_double, C.c_int, C.POINTER(C.c_int), vp, C.c_int, vp, C.POINTER(C.c_int)]
         L.flb_visual_candidates.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
         L.flb_image_upload.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int]
         L.flb_image_upload_bgr.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
@@ -777,6 +790,41 @@ class Handle:
                                           pts.shape[1] if n else 4, offset_index, n, _p(out),
                                           poses.ctypes.data_as(C.c_void_p), C.byref(npo)))
         return out, poses[:npo.value]
+
+    # ---- the driver's LiDAR message (Preprocess::process, the time sort, UndistortPcl's window)
+    def lidar_upload(self, fmt: LidarFormat, records, n_records=None):
+        """flb_lidar_upload: records = a uint8 array (or bytes) of n_records records of fmt.point_step bytes.  Returns
+        (pl_surf.size(), points.back().curvature after the sort)."""
+        a = np.frombuffer(records, np.uint8) if isinstance(records, (bytes, bytearray)) else records
+        if n_records is None:
+            n_records = a.size // max(fmt.point_step, 1)
+        n, last = C.c_int(), C.c_float()
+        self._ck(self.L.flb_lidar_upload(self.h, C.byref(fmt), _p(a) if a.size else None, int(n_records), C.byref(n), C.byref(last)))
+        self._lid_n = n.value
+        return n.value, np.float32(last.value)
+
+    def lidar_download(self):
+        """flb_lidar_download: the decoded, time-sorted cloud, (n, 4) float32 x, y, z, curvature."""
+        n = C.c_int()
+        self._ck(self.L.flb_lidar_download(self.h, None, 0, C.byref(n)))
+        out = np.zeros((n.value, 4), np.float32)
+        self._ck(self.L.flb_lidar_download(self.h, _p(out), n.value, None))
+        return out
+
+    def imu_undistort_lidar(self, prm: ImuParams, carry: ImuCarry, v_imu, pcl_beg_time, pcl_end_time, pcl_offset_time,
+                            is_lidar_end, download=True):
+        """flb_imu_undistort_lidar: imu_undistort on the window of the device cloud.  Returns (n_taken, xyz (n_taken, 3)
+        float32 or None, IMUpose)."""
+        v = np.ascontiguousarray(v_imu, np.float64)
+        cap = max(getattr(self, "_lid_n", 0), 1)
+        out = np.zeros((cap, 3), np.float32) if download else None
+        poses = np.zeros((len(v), 22), np.float64)
+        npo, taken = C.c_int(), C.c_int()
+        self._ck(self.L.flb_imu_undistort_lidar(self.h, C.byref(prm), C.byref(carry), v.ctypes.data_as(C.c_void_p), len(v),
+                                                float(pcl_beg_time), float(pcl_end_time), float(pcl_offset_time),
+                                                int(bool(is_lidar_end)), C.byref(taken), _p(out), cap,
+                                                poses.ctypes.data_as(C.c_void_p), C.byref(npo)))
+        return taken.value, (out[:taken.value] if download else None), poses[:npo.value]
 
     # ---- device-resident loop
     def state_upload(self, x: State18, x_prop: State18):

@@ -251,6 +251,20 @@ struct flb_handle {
     // count.  undist_n < 0: none (no call yet, or the last one failed)
     const float4* undist_pts = nullptr;
     int undist_n = -1;
+    // flb_lidar_upload: the decoded, time-sorted cloud of the current driver message (meas.lidar) as {x, y, z, curvature}.
+    // Double-buffered like the image: an upload decodes into lid_cloud_alt on copy_stream and swaps once it has
+    // succeeded.  lid_n < 0: no cloud; lid_cursor: lidar_scan_index_now.  The scratch below belongs to copy_stream,
+    // whose order fences its reuse.
+    DevBuf<float4> lid_cloud, lid_cloud_alt;
+    InSlot lid_slot;
+    int lid_n = -1, lid_cursor = 0;
+    DevBuf<unsigned char> lid_raw, lid_cub;    // the raw records; cub's scratch
+    DevBuf<float4> lid_dec, lid_sorted;        // every record decoded; the radix sort's output
+    DevBuf<int> lid_flags;                     // valid -> valid_num | kept | pos, n each; then the LidarRecord
+    DevBuf<int> lid_win;                       // flb_imu_undistort_lidar: the window's point count (on `stream`)
+    DevBuf<unsigned> lid_keys, lid_keys_sorted;
+    Staging st_lidar;
+    PinBuf pin_lidar;
     // flb_world_cloud: pcl_wait_pub (packed xyz, the caller's order) with its exact bounds; wc_n < 0: no cloud held
     DevBuf<float> wc_xyz;
     DevBuf<unsigned> wc_rec;           // bounds + non-finite record of the transform (kScanRec*)
@@ -1045,10 +1059,14 @@ int flb_destroy(flb_handle* h) {
     cudaStreamSynchronize(h->copy_stream);
     cudaStreamSynchronize(h->scan_stream);
     h->scan_alt.release(); h->plane_alt.release(); h->sel_alt.release(); h->plane_ok_alt.release(); h->sf_down.release();
+    h->lid_cloud.release(); h->lid_cloud_alt.release(); h->lid_raw.release(); h->lid_cub.release(); h->lid_dec.release();
+    h->lid_sorted.release(); h->lid_flags.release(); h->lid_win.release(); h->lid_keys.release(); h->lid_keys_sorted.release();
+    h->st_lidar.release(); h->pin_lidar.release();
     h->img_alt.release(); h->patch_pos_alt.release(); h->patch_ref_alt.release(); h->patch_level_alt.release();
     for (int k = 0; k < 2; ++k) {
         if (h->img_slot.free_ev[k]) cudaEventDestroy(h->img_slot.free_ev[k]);
         if (h->patch_slot.free_ev[k]) cudaEventDestroy(h->patch_slot.free_ev[k]);
+        if (h->lid_slot.free_ev[k]) cudaEventDestroy(h->lid_slot.free_ev[k]);
     }
     cudaEventDestroy(h->ev_scan_ready);
     cudaEventDestroy(h->ev_scan_free[0]);
@@ -1782,18 +1800,18 @@ int flb_map_download(flb_handle* h, float* xyz, int capacity, int* M_out) {
     return FLB_OK;
 }
 
-int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* carry, const flb_imu_sample* v_imu, int n_imu,
-                      double pcl_beg_time, double pcl_end_time, const float* pts, int stride, int offset_index, int n_points,
-                      float* out_xyz, double* poses_out, int* n_poses_out) {
-    FLB_CHECK_H(h);
-    h->undist_n = -1;                 // flb_world_cloud's FLB_CLOUD_UNDISTORTED source is this call's output, or none
-    if (!prm || !carry || !v_imu || n_imu < 1 || n_points < 0 || (n_points > 0 && !pts) || stride < 4 ||
-        offset_index < 3 || offset_index >= stride)
-        return fail(h, FLB_ERR_INVALID, "flb_imu_undistort: bad arguments");
-    if (!h->state_valid) return fail(h, FLB_ERR_STATE, "flb_imu_undistort: no device state (flb_state_upload)");
+namespace {
+
+// flb_imu_undistort and flb_imu_undistort_lidar from the argument checks on.  The n_points points are either the
+// caller's (pts, packed into the staging area and uploaded) or, with dev_pts, already on the device as {x, y, z, offset}
+// and read in place.
+int imu_undistort_core(flb_handle* h, const char* who, const flb_imu_params* prm, flb_imu_carry* carry, const flb_imu_sample* v_imu,
+                       int n_imu, double pcl_beg_time, double pcl_end_time, const float* pts, int stride, int offset_index,
+                       const float4* dev_pts, int n_points, float* out_xyz, double* poses_out, int* n_poses_out) {
+    if (!h->state_valid) return fail(h, FLB_ERR_STATE, "%s: no device state (flb_state_upload)", who);
     { int rcf = flush_state_ops(h); if (rcf) return rcf; }
     for (int i = 0; i + 1 < n_imu; ++i)
-        if (!(v_imu[i + 1].t >= v_imu[i].t)) return fail(h, FLB_ERR_INVALID, "flb_imu_undistort: IMU times must be non-decreasing");
+        if (!(v_imu[i + 1].t >= v_imu[i].t)) return fail(h, FLB_ERR_INVALID, "%s: IMU times must be non-decreasing", who);
     static_assert(sizeof(ImuSampleDev) == sizeof(flb_imu_sample) && sizeof(ImuCarryDev) == sizeof(flb_imu_carry), "ABI layout");
     static_assert(sizeof(ImuPose) == 22 * sizeof(double), "IMUpose layout");
     ImuParamsDev d;
@@ -1812,22 +1830,22 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
     FLB_CUDA(h, h->imu_pts.reserve(n1 * 2));
     FLB_CUDA(h, h->imu_heads.reserve(n1));
     void* stv = nullptr;
-    FLB_CUDA(h, h->st_scan.acquire(n1 * 4 * sizeof(float) + (off_aux) * sizeof(double), &stv));
+    FLB_CUDA(h, h->st_scan.acquire((dev_pts ? 0 : n1 * 4 * sizeof(float)) + (off_aux) * sizeof(double), &stv));
     double* st_d = static_cast<double*>(stv);
     std::memcpy(st_d, v_imu, (size_t)n_imu * sizeof(flb_imu_sample));
     std::memcpy(st_d + off_carry, carry, sizeof(flb_imu_carry));
     float* st_p = reinterpret_cast<float*>(st_d + off_aux);
-    for (int i = 0; i < n_points; ++i) {
+    for (int i = 0; !dev_pts && i < n_points; ++i) {
         st_p[4 * (size_t)i] = pts[(size_t)i * stride];
         st_p[4 * (size_t)i + 1] = pts[(size_t)i * stride + 1];
         st_p[4 * (size_t)i + 2] = pts[(size_t)i * stride + 2];
         st_p[4 * (size_t)i + 3] = pts[(size_t)i * stride + offset_index];
     }
     FLB_CUDA(h, cudaMemcpyAsync(h->imu_buf.p, st_d, off_aux * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    float4* d_in = h->imu_pts.p;
+    const float4* d_in = dev_pts ? dev_pts : h->imu_pts.p;
     float4* d_out = h->imu_pts.p + n1;
-    if (n_points > 0)
-        FLB_CUDA(h, cudaMemcpyAsync(d_in, st_p, (size_t)n_points * 4 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    if (n_points > 0 && !dev_pts)
+        FLB_CUDA(h, cudaMemcpyAsync(h->imu_pts.p, st_p, (size_t)n_points * 4 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     FLB_CUDA(h, h->st_scan.mark(h->stream));
     const ImuSampleDev* d_imu = reinterpret_cast<const ImuSampleDev*>(h->imu_buf.p);
     ImuCarryDev* d_carry = reinterpret_cast<ImuCarryDev*>(h->imu_buf.p + off_carry);
@@ -1872,6 +1890,181 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
     h->undist_n = n_points;
     h->last_pass_valid = false;
     h->last_vio_valid = false;
+    return FLB_OK;
+}
+
+}  // namespace
+
+int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* carry, const flb_imu_sample* v_imu, int n_imu,
+                      double pcl_beg_time, double pcl_end_time, const float* pts, int stride, int offset_index, int n_points,
+                      float* out_xyz, double* poses_out, int* n_poses_out) {
+    FLB_CHECK_H(h);
+    h->undist_n = -1;                 // flb_world_cloud's FLB_CLOUD_UNDISTORTED source is this call's output, or none
+    if (!prm || !carry || !v_imu || n_imu < 1 || n_points < 0 || (n_points > 0 && !pts) || stride < 4 ||
+        offset_index < 3 || offset_index >= stride)
+        return fail(h, FLB_ERR_INVALID, "flb_imu_undistort: bad arguments");
+    return imu_undistort_core(h, "flb_imu_undistort", prm, carry, v_imu, n_imu, pcl_beg_time, pcl_end_time, pts, stride, offset_index,
+                              nullptr, n_points, out_xyz, poses_out, n_poses_out);
+}
+
+// ---- the driver's LiDAR message on the device ----------------------------------------------------------------------
+namespace {
+
+// byte size and alignment of the time field of each kind
+int lidar_time_bytes(int kind) { return kind == kLidarXt32 ? 8 : 4; }
+
+bool lidar_field_ok(int off, int bytes, int step) { return off >= 0 && off % bytes == 0 && off + bytes <= step; }
+
+}  // namespace
+
+int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* records, int n_records, int* n_points,
+                     float* last_offset_ms) {
+    FLB_CHECK_H(h);
+    if (n_records < 0 || !fmt || (n_records > 0 && !records)) return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: bad arguments");
+    if (fmt->kind < kLidarLivox || fmt->kind > kLidarXt32) return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: unknown kind %d", fmt->kind);
+    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || !std::isfinite(fmt->blind))
+        return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: point_filter_num %d, n_scans %d, blind %g", fmt->point_filter_num,
+                    fmt->n_scans, fmt->blind);
+    const int step = fmt->point_step;
+    const bool livox = fmt->kind == kLidarLivox;
+    if (step < 1 || !lidar_field_ok(fmt->off_x, 4, step) || !lidar_field_ok(fmt->off_y, 4, step) || !lidar_field_ok(fmt->off_z, 4, step) ||
+        !lidar_field_ok(fmt->off_time, lidar_time_bytes(fmt->kind), step) ||
+        (livox && (!lidar_field_ok(fmt->off_tag, 1, step) || !lidar_field_ok(fmt->off_line, 1, step))))
+        return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: a field does not fit in point_step %d or is not aligned to its type", step);
+    LidarFmt f{};
+    f.kind = fmt->kind, f.step = step, f.off_x = fmt->off_x, f.off_y = fmt->off_y, f.off_z = fmt->off_z, f.off_time = fmt->off_time;
+    f.off_tag = livox ? fmt->off_tag : 0, f.off_line = livox ? fmt->off_line : 0;
+    f.n_scans = fmt->n_scans, f.filter_num = fmt->point_filter_num, f.blind = fmt->blind;
+    const unsigned char* rec_h = static_cast<const unsigned char*>(records);
+    if (n_records > 0 && fmt->kind == kLidarVelodyne) {
+        float t_last;                                                              // given_offset_time, :279
+        std::memcpy(&t_last, rec_h + (size_t)(n_records - 1) * step + f.off_time, sizeof(t_last));
+        if (!(t_last > 0))
+            return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: a Velodyne cloud without per-point times (last time %g): the yaw-derived "
+                        "times (src/preprocess.cpp:389-419) are a sequential per-ring walk and stay with the host", (double)t_last);
+    }
+    if (n_records > 0 && fmt->kind == kLidarXt32) std::memcpy(&f.time_head, rec_h + f.off_time, sizeof(double));   // :441
+    const size_t n = (size_t)n_records, n1 = std::max<size_t>(n, 1), raw_bytes = n * step;
+    FLB_CUDA(h, h->lid_raw.reserve(std::max<size_t>(raw_bytes, 4)));
+    FLB_CUDA(h, h->lid_cloud_alt.reserve(n1));
+    FLB_CUDA(h, h->lid_dec.reserve(n1));
+    FLB_CUDA(h, h->lid_sorted.reserve(n1));
+    FLB_CUDA(h, h->lid_keys.reserve(n1));
+    FLB_CUDA(h, h->lid_keys_sorted.reserve(n1));
+    FLB_CUDA(h, h->lid_flags.reserve(3 * n1 + 8));
+    FLB_CUDA(h, h->pin_lidar.reserve(64));
+    cudaStream_t cs = h->copy_stream;
+    int* d_vnum = h->lid_flags.p;
+    int* d_kept = d_vnum + n1;
+    int* d_pos = d_kept + n1;
+    LidarRecord* d_rec = reinterpret_cast<LidarRecord*>(d_pos + n1);
+    static_assert(sizeof(LidarRecord) == 4 * sizeof(int), "LidarRecord sits in lid_flags");
+    LidarRecord rec{};
+    // the raw records go up before the wait for the idle set's readers: only the kernels that write that set wait
+    if (n_records > 0) {
+        if (is_pinned(records)) {
+            FLB_CUDA(h, cudaMemcpyAsync(h->lid_raw.p, records, raw_bytes, cudaMemcpyHostToDevice, cs));
+        } else {
+            void* stv = nullptr;
+            FLB_CUDA(h, h->st_lidar.acquire(raw_bytes, &stv));
+            std::memcpy(stv, records, raw_bytes);
+            FLB_CUDA(h, cudaMemcpyAsync(h->lid_raw.p, stv, raw_bytes, cudaMemcpyHostToDevice, cs));
+            FLB_CUDA(h, h->st_lidar.mark(cs));
+        }
+        { int rcq = vio_copy_begin(h, h->lid_slot); if (rcq) return rcq; }
+        size_t t1 = 0, t2 = 0, t3 = 0;
+        FLB_CUDA(h, cub::DeviceScan::InclusiveSum(nullptr, t1, d_vnum, d_vnum, n_records, cs));
+        FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t2, d_kept, d_pos, n_records, cs));
+        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p, h->lid_sorted.p,
+                                                    n_records, 0, 32, cs));
+        FLB_CUDA(h, h->lid_cub.reserve(std::max(t1, std::max(t2, t3))));
+        const int g = (n_records + 255) / 256;
+        FLB_CUDA(h, cudaMemsetAsync(d_rec, 0, sizeof(LidarRecord), cs));
+        if (livox) {
+            k_lidar_valid<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum);
+            FLB_CUDA(h, cub::DeviceScan::InclusiveSum(h->lid_cub.p, t1, d_vnum, d_vnum, n_records, cs));
+            h->launches += 2;
+        }
+        k_lidar_flags<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum, h->lid_dec.p, d_kept);
+        FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t2, d_kept, d_pos, n_records, cs));
+        k_lidar_scatter<<<g, 256, 0, cs>>>(h->lid_dec.p, d_kept, d_pos, n_records, h->lid_cloud_alt.p, h->lid_keys.p, d_rec);
+        k_lidar_order<<<g, 256, 0, cs>>>(h->lid_cloud_alt.p, h->lid_keys.p, n_records, d_rec);
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches += 4;
+        FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
+        FLB_CUDA(h, cudaStreamSynchronize(cs));
+        std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
+        if (rec.bad) return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: a kept point or time is not finite");
+        if (rec.unsorted) {
+            // stable: equal times keep record order (std::sort leaves that order unspecified in the reference)
+            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p,
+                                                        h->lid_sorted.p, rec.n_kept, 0, 32, cs));
+            FLB_CUDA(h, cudaMemcpyAsync(h->lid_cloud_alt.p, h->lid_sorted.p, (size_t)rec.n_kept * sizeof(float4), cudaMemcpyDeviceToDevice, cs));
+            k_lidar_last<<<1, 1, 0, cs>>>(h->lid_cloud_alt.p, d_rec);
+            FLB_CUDA(h, cudaGetLastError());
+            h->launches += 3;
+            FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
+            FLB_CUDA(h, cudaStreamSynchronize(cs));
+            std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
+        }
+    } else {
+        int rcq = vio_copy_begin(h, h->lid_slot);
+        if (rcq) return rcq;
+    }
+    std::swap(h->lid_cloud, h->lid_cloud_alt);
+    h->lid_slot.slot ^= 1;
+    h->lid_n = rec.n_kept;
+    h->lid_cursor = 0;
+    if (n_points) *n_points = rec.n_kept;
+    if (last_offset_ms) *last_offset_ms = rec.n_kept > 0 ? rec.last : 0.f;
+    return FLB_OK;
+}
+
+int flb_lidar_download(flb_handle* h, float* xyzt, int capacity_points, int* n_out) {
+    FLB_CHECK_H(h);
+    if (h->lid_n < 0) return fail(h, FLB_ERR_STATE, "flb_lidar_download: no cloud (flb_lidar_upload)");
+    if (n_out) *n_out = h->lid_n;
+    if (!xyzt) return FLB_OK;
+    if (capacity_points < h->lid_n) return fail(h, FLB_ERR_INVALID, "flb_lidar_download: capacity %d < %d points", capacity_points, h->lid_n);
+    if (h->lid_n > 0) {
+        FLB_CUDA(h, cudaMemcpyAsync(xyzt, h->lid_cloud.p, (size_t)h->lid_n * sizeof(float4), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    }
+    return FLB_OK;
+}
+
+int flb_imu_undistort_lidar(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* carry, const flb_imu_sample* v_imu, int n_imu,
+                            double pcl_beg_time, double pcl_end_time, double pcl_offset_time, int is_lidar_end, int* n_taken,
+                            float* out_xyz, int capacity_points, double* poses_out, int* n_poses_out) {
+    FLB_CHECK_H(h);
+    h->undist_n = -1;
+    if (!prm || !carry || !v_imu || n_imu < 1 || std::isnan(pcl_offset_time))
+        return fail(h, FLB_ERR_INVALID, "flb_imu_undistort_lidar: bad arguments");
+    if (h->lid_n < 0) return fail(h, FLB_ERR_STATE, "flb_imu_undistort_lidar: no cloud (flb_lidar_upload)");
+    if (!h->state_valid) return fail(h, FLB_ERR_STATE, "flb_imu_undistort_lidar: no device state (flb_state_upload)");
+    // the window, :634-639 (the cloud is complete: flb_lidar_upload returned after its last kernel)
+    int taken = 0;
+    const int begin = h->lid_cursor;
+    if (begin < h->lid_n) {
+        FLB_CUDA(h, h->lid_win.reserve(1));
+        int* d_taken = h->lid_win.p;
+        FLB_CUDA(h, h->pin_out.reserve(64));
+        {
+            LaunchScope ls(h, FAM_OTHER);
+            k_lidar_window<<<1, 1, 0, h->stream>>>(h->lid_cloud.p, begin, h->lid_n, pcl_offset_time, d_taken);
+            FLB_CUDA(h, cudaGetLastError());
+        }
+        FLB_CUDA(h, cudaMemcpyAsync(h->pin_out.p, d_taken, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+        std::memcpy(&taken, h->pin_out.p, sizeof(int));
+    }
+    if (out_xyz && capacity_points < taken)
+        return fail(h, FLB_ERR_INVALID, "flb_imu_undistort_lidar: capacity %d < the %d points of this update", capacity_points, taken);
+    const int rc = imu_undistort_core(h, "flb_imu_undistort_lidar", prm, carry, v_imu, n_imu, pcl_beg_time, pcl_end_time, nullptr, 4, 3,
+                                      h->lid_cloud.p + begin, taken, out_xyz, poses_out, n_poses_out);
+    if (rc) return rc;
+    h->lid_cursor = is_lidar_end ? 0 : begin + taken;                             // :638, :643-646
+    if (n_taken) *n_taken = taken;
     return FLB_OK;
 }
 

@@ -1627,4 +1627,72 @@ FLB_HD unsigned bgr_to_gray(unsigned b, unsigned g, unsigned r, int rule) {
 // 2x2 area path there, one rounded mean per channel of each 2x2 source block.
 FLB_HD unsigned mean2x2(unsigned a, unsigned b, unsigned c, unsigned d) { return (a + b + c + d + 2u) >> 2; }
 
+// ------------------------------------------------------------------ LiDAR message decode (Preprocess::process)
+// The non-feature (`else`) branches of the four handlers of src/preprocess.cpp, one driver record at a time
+// (flb_lidar_upload).  A record is `step` bytes; its fields sit at the byte offsets of LidarFmt.
+enum { kLidarLivox = 1, kLidarVelodyne = 2, kLidarOuster = 3, kLidarXt32 = 4 };
+struct LidarFmt {
+    int kind, step, off_x, off_y, off_z, off_time, off_tag, off_line, n_scans, filter_num;
+    double blind;
+    double time_head;      // XT32: points[0].timestamp (:441)
+};
+struct LidarPoint { float x, y, z, t; };      // t: PointType::curvature, the offset from the scan start in ms
+
+// 32 bits of a little-endian record field.  PointCloud2 steps are arbitrary and a Livox record is 20 bytes, so a field is
+// 4-byte aligned in memory only when the record's address is.
+FLB_HD unsigned lidar_ld32(const unsigned char* p) {
+    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) return *reinterpret_cast<const unsigned*>(p);
+    return (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
+}
+FLB_HD double lidar_ld64f(const unsigned char* p) {
+    const unsigned long long u = (unsigned long long)lidar_ld32(p) | ((unsigned long long)lidar_ld32(p + 4) << 32);
+    double d;
+    memcpy(&d, &u, sizeof(d));
+    return d;
+}
+
+// x, y, z and the per-point time of record r, with each handler's own arithmetic.
+FLB_HD LidarPoint lidar_decode(const unsigned char* r, const LidarFmt& f) {
+    LidarPoint q;
+    q.x = u32_as_float(lidar_ld32(r + f.off_x));
+    q.y = u32_as_float(lidar_ld32(r + f.off_y));
+    q.z = u32_as_float(lidar_ld32(r + f.off_z));
+    if (f.kind == kLidarLivox) q.t = (float)lidar_ld32(r + f.off_time) / float(1000000);          // :149
+    else if (f.kind == kLidarOuster) q.t = (float)lidar_ld32(r + f.off_time) * 1.e-6f;            // :250
+    else if (f.kind == kLidarVelodyne) q.t = u32_as_float(lidar_ld32(r + f.off_time)) * 1.e-3f;   // :387
+    else q.t = (float)((lidar_ld64f(r + f.off_time) - f.time_head) * (double)1000.f);             // :454
+    return q;
+}
+// Livox: the record counts in valid_num (:140).  The loop starts at record 1 (:138), so record 0 never does.
+FLB_HD bool lidar_livox_valid(const unsigned char* r, int i, const LidarFmt& f) {
+    const unsigned tag = r[f.off_tag] & 0x30u;
+    return i >= 1 && (int)r[f.off_line] < f.n_scans && (tag == 0x10u || tag == 0x00u);
+}
+// Livox: record i reaches :145 when it is valid and valid_num (the count of valid records up to and including it)
+// is a multiple of point_filter_num (:143, unsigned arithmetic).
+FLB_HD bool lidar_livox_candidate(bool valid, unsigned valid_num, const LidarFmt& f) {
+    return valid && valid_num % (unsigned)f.filter_num == 0u;
+}
+// Livox, :151-154.  prev is pl_full[i-1]: record i-1's coordinates when that record was itself a candidate, otherwise
+// the zeros pl_full.resize left there (:83).  abs is the float overload; 1e-7 and blind * blind are doubles.
+FLB_HD bool lidar_livox_keep(const LidarPoint& q, float px, float py, float pz, double blind) {
+    const bool moved = (double)fabsf(q.x - px) > 1e-7 || (double)fabsf(q.y - py) > 1e-7 || (double)fabsf(q.z - pz) > 1e-7;
+    return moved && (double)(q.x * q.x + q.y * q.y + q.z * q.z) > blind * blind;
+}
+// Ouster :235-239, Velodyne :421-423, XT32 :456-458 (which compares with blind itself, not its square).
+FLB_HD bool lidar_pc2_keep(const LidarPoint& q, int i, const LidarFmt& f) {
+    if (i % f.filter_num != 0) return false;
+    const float range = q.x * q.x + q.y * q.y + q.z * q.z;
+    if (f.kind == kLidarOuster) return !((double)range < f.blind * f.blind);
+    if (f.kind == kLidarVelodyne) return (double)range > f.blind * f.blind;
+    return (double)range > f.blind;
+}
+// Order-preserving 32-bit key of a finite time for the radix sort: -0.0 and +0.0 share a key, as they compare equal in
+// time_list (include/common_lib.h), so that ties keep record order.
+FLB_HD unsigned lidar_time_key(float t) {
+    const unsigned u = float_as_u32(t == 0.f ? 0.f : t);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+FLB_HD bool lidar_finite(float v) { return (float_as_u32(v) & 0x7f800000u) != 0x7f800000u; }
+
 }  // namespace flb

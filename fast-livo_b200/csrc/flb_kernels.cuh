@@ -3522,4 +3522,94 @@ __global__ void __launch_bounds__(128) k_image_prep(const unsigned char* __restr
     }
 }
 
+// ---- LiDAR message decode (flb_lidar_upload / flb_imu_undistort_lidar) ----------------------------------------------
+// Preprocess::process (src/preprocess.cpp:43-70, the handlers' non-feature branches), the time sort of sync_packages
+// (src/laserMapping.cpp:551) and the window of UndistortPcl (src/IMU_Processing.cpp:624-646) on the raw records of one
+// driver message held in `raw`.  The per-record arithmetic is flb_device.cuh's; a thread owns one record throughout.
+struct LidarRecord {
+    int n_kept;        // pl_surf.size()
+    int unsorted;      // some kept time is below its predecessor's: the radix sort runs
+    int bad;           // a kept coordinate or time is not finite
+    float last;        // the largest kept time = points.back().curvature once sorted
+};
+
+// Livox: valid[i] = record i counts in valid_num (:140); its inclusive sum is valid_num at record i.
+__global__ void __launch_bounds__(256) k_lidar_valid(const unsigned char* __restrict__ raw, int n, LidarFmt f, int* __restrict__ valid) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) valid[i] = lidar_livox_valid(raw + (size_t)i * f.step, i, f) ? 1 : 0;
+}
+
+// dec[i] = the decoded record, kept[i] = it enters pl_surf.  Livox reads its left neighbour's record and valid_num too:
+// pl_full[i-1] holds that record only when it was a candidate itself (:145-147), otherwise zeros.
+__global__ void __launch_bounds__(256) k_lidar_flags(const unsigned char* __restrict__ raw, int n, LidarFmt f,
+                                                     const int* __restrict__ valid_num, float4* __restrict__ dec,
+                                                     int* __restrict__ kept) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned char* r = raw + (size_t)i * f.step;
+    const LidarPoint q = lidar_decode(r, f);
+    bool keep;
+    if (f.kind == kLidarLivox) {
+        const int vn = valid_num[i], vp = i > 0 ? valid_num[i - 1] : 0;
+        keep = false;
+        if (lidar_livox_candidate(vn != vp, (unsigned)vn, f)) {
+            float px = 0.f, py = 0.f, pz = 0.f;
+            const int vpp = i > 1 ? valid_num[i - 2] : 0;
+            if (i > 0 && lidar_livox_candidate(vp != vpp, (unsigned)vp, f)) {
+                const LidarPoint b = lidar_decode(r - f.step, f);
+                px = b.x, py = b.y, pz = b.z;
+            }
+            keep = lidar_livox_keep(q, px, py, pz, f.blind);
+        }
+    } else {
+        keep = lidar_pc2_keep(q, i, f);
+    }
+    dec[i] = make_float4(q.x, q.y, q.z, q.t);
+    kept[i] = keep ? 1 : 0;
+}
+
+// Stable compaction: pos = the exclusive sum of kept.  Also the sort key of every kept time, and the record's count
+// and non-finite flag (rec is zeroed before the launch).
+__global__ void __launch_bounds__(256) k_lidar_scatter(const float4* __restrict__ dec, const int* __restrict__ kept,
+                                                       const int* __restrict__ pos, int n, float4* __restrict__ cloud,
+                                                       unsigned* __restrict__ keys, LidarRecord* __restrict__ rec) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int k = kept[i], p = pos[i];
+    if (i == n - 1) rec->n_kept = p + k;
+    if (!k) return;
+    const float4 q = dec[i];
+    cloud[p] = q;
+    keys[p] = lidar_time_key(q.w);
+    if (!(lidar_finite(q.x) && lidar_finite(q.y) && lidar_finite(q.z) && lidar_finite(q.w))) rec->bad = 1;
+}
+
+// One pass over the compacted keys: are the times already non-decreasing (the common Livox case), and which is the
+// largest.  Launched over the record count; the kept count is on the device.
+__global__ void __launch_bounds__(256) k_lidar_order(const float4* __restrict__ cloud, const unsigned* __restrict__ keys, int n,
+                                                     LidarRecord* __restrict__ rec) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    const int m = rec->n_kept;
+    if (j >= m || j >= n) return;
+    if (j > 0 && keys[j] < keys[j - 1]) rec->unsorted = 1;
+    if (j == m - 1) rec->last = cloud[j].w;
+}
+
+// After the sort: points.back().curvature.
+__global__ void k_lidar_last(const float4* __restrict__ cloud, LidarRecord* __restrict__ rec) {
+    if (rec->n_kept > 0) rec->last = cloud[rec->n_kept - 1].w;
+}
+
+// UndistortPcl's window (:634-639) on the sorted cloud: the points from `begin` on while (double)curvature <=
+// pcl_offset_time.  The times do not decrease, so the loop's exit is their partition point.
+__global__ void k_lidar_window(const float4* __restrict__ cloud, int begin, int n, double pcl_offset_time, int* __restrict__ n_taken) {
+    int lo = begin, hi = n;
+    while (lo < hi) {
+        const int mid = lo + (hi - lo) / 2;
+        if ((double)cloud[mid].w <= pcl_offset_time) lo = mid + 1;
+        else hi = mid;
+    }
+    *n_taken = lo - begin;
+}
+
 }  // namespace flb

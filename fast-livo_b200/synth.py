@@ -385,6 +385,94 @@ def make_imu_frame(seed=1, n_points=24000, imu_hz=200.0, scan_s=0.1, variant="no
 
 
 # ---------------------------------------------------------------------------------------------------------
+# Raw driver messages (Preprocess::process, reference src/preprocess.cpp): flb_lidar_upload's input
+# ---------------------------------------------------------------------------------------------------------
+LIVOX_POINT = np.dtype([("offset_time", "<u4"), ("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("reflectivity", "u1"),
+                        ("tag", "u1"), ("line", "u1"), ("pad", "u1")])                    # livox_ros_driver::CustomPoint, 20 bytes
+OUSTER_POINT = np.dtype({"names": ["x", "y", "z", "intensity", "t", "reflectivity", "ring", "ambient", "range"],
+                         "formats": ["<f4", "<f4", "<f4", "<f4", "<u4", "<u2", "u1", "<u2", "<u4"],
+                         "offsets": [0, 4, 8, 16, 20, 24, 26, 28, 32], "itemsize": 48})    # ouster_ros::Point with its padding
+VELODYNE_POINT = np.dtype({"names": ["x", "y", "z", "intensity", "ring", "time"],
+                           "formats": ["<f4", "<f4", "<f4", "<f4", "<u2", "<f4"],
+                           "offsets": [0, 4, 8, 12, 16, 20], "itemsize": 24})
+XT32_POINT = np.dtype({"names": ["x", "y", "z", "intensity", "timestamp", "ring"],
+                       "formats": ["<f4", "<f4", "<f4", "<f4", "<f8", "<u2"],
+                       "offsets": [0, 4, 8, 12, 16, 24], "itemsize": 32})
+LIDAR_KINDS = {"livox": 1, "velodyne": 2, "velodyne_notime": 2, "ouster": 3, "xt32": 4}      # FLB_LIDAR_*
+
+
+def make_lidar_message(kind, seed=1, n=24000, point_filter_num=None, unsorted=None):
+    """One driver message as (records, fmt): the raw records as bytes and a dict of flb_lidar_format's fields.
+    kind: "livox" (six lines fired together, so times tie; tags over all four `& 0x30` values with other bits set; lines
+    >= n_scans; runs of repeated points; (0, 0, 0) no-return points; points inside blind; a repeated point right after a
+    record that is not taken), "ouster" (column order with staggered t, 48-byte records with padding), "velodyne",
+    "velodyne_notime" (every time 0), "xt32" (f64 timestamp).  unsorted: shuffle the firing times (default: only the
+    Ouster's stagger); point_filter_num: default 1 for Livox, 3 otherwise."""
+    rng = np.random.default_rng(1000 * LIDAR_KINDS[kind] + seed)
+    blind = {"livox": 0.5, "ouster": 0.8, "velodyne": 1.0, "velodyne_notime": 1.0, "xt32": 0.64}[kind]
+    d = rng.uniform(1.2, 60.0, n)
+    near = rng.random(n) < 0.03
+    d[near] = rng.uniform(0.05, 0.95 * blind if kind != "xt32" else 0.75, near.sum())     # inside blind (XT32: blind is unsquared)
+    az, el = rng.uniform(-np.pi, np.pi, n), rng.uniform(-0.4, 0.4, n)
+    xyz = np.stack([d * np.cos(el) * np.cos(az), d * np.cos(el) * np.sin(az), d * np.sin(el)], 1).astype(np.float32)
+    xyz[rng.random(n) < 0.03] = 0.0                                                      # no return
+    rep = np.flatnonzero(rng.random(n) < 0.04)
+    for i in rep[rep > 0]:                                                               # runs of repeated points
+        xyz[i] = xyz[i - 1]
+    idx = np.arange(n)
+    if kind == "livox":
+        a = np.zeros(n, LIVOX_POINT)
+        group = idx // 6
+        if unsorted:
+            group = rng.permutation(max(int(group.max(initial=0)) + 1, 1))[group] if n else group
+        a["offset_time"] = (group.astype(np.int64) * 25000 + 7).astype(np.uint32)         # ns; the six lines share a time
+        a["line"] = idx % 6
+        bad_line = rng.random(n) < 0.02
+        a["line"][bad_line] = rng.integers(6, 9, bad_line.sum())
+        tag = rng.choice(np.array([0x00, 0x10, 0x20, 0x30], np.uint8), n, p=[0.45, 0.4, 0.1, 0.05])
+        a["tag"] = tag | (rng.integers(0, 256, n).astype(np.uint8) & 0xCF)
+        a["reflectivity"] = rng.integers(0, 256, n)
+        for j in range(40, n - 1, 997):          # a repeated point right after a record that is not taken: compared with zero
+            xyz[j] = xyz[j - 1] = np.float32([3.0 + 0.001 * j, -2.0, 0.5])
+            a["tag"][j - 1] = 0x20 | 0x03
+            a["tag"][j] = 0x10 | 0x40
+            a["line"][j] = 2
+        fmt = dict(off_time=0, off_x=4, off_y=8, off_z=12, off_tag=17, off_line=18, n_scans=6,
+                   point_filter_num=point_filter_num or 1)
+    elif kind == "ouster":
+        a = np.zeros(n, OUSTER_POINT)
+        col, ring = idx // 64, idx % 64
+        if unsorted is False:
+            a["t"] = idx * 763
+        else:
+            a["t"] = col * 48828 + (3 - ring % 4) * 30000                                # staggered: not sorted in record order
+        a["ring"] = ring
+        a["intensity"] = rng.uniform(0, 255, n)
+        a.view(np.uint8).reshape(n, 48)[:, 12:16] = 0xAB                                 # padding is not zero
+        a.view(np.uint8).reshape(n, 48)[:, 36:48] = 0xCD
+        fmt = dict(off_x=0, off_y=4, off_z=8, off_time=20, off_tag=0, off_line=0, n_scans=64,
+                   point_filter_num=point_filter_num or 3)
+    elif kind in ("velodyne", "velodyne_notime"):
+        a = np.zeros(n, VELODYNE_POINT)
+        a["ring"] = idx % 16
+        if kind == "velodyne":
+            t = (idx // 16) * 55.296e-6 + (idx % 16) * 2.304e-6 + 1e-6                    # seconds from the scan start
+            a["time"] = rng.permutation(t) if unsorted else t
+        fmt = dict(off_x=0, off_y=4, off_z=8, off_time=20, off_tag=0, off_line=0, n_scans=16,
+                   point_filter_num=point_filter_num or 3)
+    else:
+        a = np.zeros(n, XT32_POINT)
+        t = 1.7e9 + 0.25 * seed + (idx // 32) * 55.56e-6 + (idx % 32) * 1.5e-6
+        a["timestamp"] = rng.permutation(t) if unsorted else t
+        a["ring"] = idx % 32
+        fmt = dict(off_x=0, off_y=4, off_z=8, off_time=16, off_tag=0, off_line=0, n_scans=32,
+                   point_filter_num=point_filter_num or 3)
+    a["x"], a["y"], a["z"] = xyz[:, 0], xyz[:, 1], xyz[:, 2]
+    fmt.update(kind=LIDAR_KINDS[kind], point_step=a.dtype.itemsize, blind=blind)
+    return a.tobytes(), fmt
+
+
+# ---------------------------------------------------------------------------------------------------------
 # Visual-map sequences (SURVEY.md section 8 rows f2 / f4): several frames of ONE scene along a short trajectory
 # ---------------------------------------------------------------------------------------------------------
 def voxel_centroids(xyz: np.ndarray, leaf: float) -> np.ndarray:

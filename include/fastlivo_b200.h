@@ -176,6 +176,73 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
                       double pcl_beg_time, double pcl_end_time, const float* pts, int stride_floats, int offset_index,
                       int n_points, float* out_xyz, double* poses_out, int* n_poses_out);
 
+/* ---- the driver's LiDAR message on the device ------------------------------------------------------------
+ * Preprocess::process (src/preprocess.cpp:43-70) with feature_extract_enable = 0 (every shipped config), the time sort
+ * of sync_packages (src/laserMapping.cpp:551) and the window at the top of UndistortPcl
+ * (src/IMU_Processing.cpp:621-646), from the raw records of one driver message.  Each handler's arithmetic and quirks
+ * are kept bit for bit:
+ *   FLB_LIDAR_LIVOX (avia_handler, :138-160; Avia, Mid360): the loop starts at record 1, so record 0 is never kept
+ *     (:138).  A record is valid when line < n_scans and (tag & 0x30) is 0x10 or 0x00 (:140); valid_num counts the valid
+ *     records and a record is taken when valid_num % point_filter_num == 0 (:142-143).  curvature = offset_time /
+ *     float(1000000) (:149).  It is kept when some |coordinate - pl_full[i-1]'s| > 1e-7 and x*x + y*y + z*z (float) >
+ *     blind * blind (:151-154); pl_full[i-1] holds record i-1 only when that record was taken itself, otherwise the
+ *     (0, 0, 0) of pl_full.resize (:83), so a repeated point that follows a record which was not taken is compared with
+ *     zero and kept.
+ *   FLB_LIDAR_OUSTER (oust64_handler, :233-252): i % point_filter_num == 0 (:235); skipped when the float sum of squares,
+ *     widened to double, is < blind * blind (:237-239); curvature = t * 1.e-6f (:250).
+ *   FLB_LIDAR_VELODYNE (velodyne_handler, :376-428): only clouds with per-point times, i.e. the last record's time > 0
+ *     (given_offset_time, :279).  curvature = time * 1.e-3f (:387); i % point_filter_num == 0 (:421); kept when the
+ *     float sum of squares > blind * blind (:423).  Without times the reference derives them from the yaw angle with a
+ *     sequential per-ring state (:389-419); that stays with the host and the call returns FLB_ERR_INVALID.
+ *   FLB_LIDAR_XT32 (xt32_handler, :441-461): curvature = float((timestamp - timestamp[0]) * 1000.f), computed in double
+ *     (:454); i % point_filter_num == 0 (:456); kept when the float sum of squares > blind, not its square (:458).
+ * The kept points are then sorted by curvature (time_list).  std::sort leaves the order of equal times unspecified; here
+ * it is the stable order (equal times keep record order).  Ties are real: the lines of a Livox fire together.
+ * The cloud stays on the device as {x, y, z, curvature}; intensity is not kept (no device cloud carries it).
+ *
+ * flb_lidar_upload: records = n_records records of fmt->point_step bytes (CustomMsg::points, or PointCloud2::data).
+ * *n_points = pl_surf.size(), *last_offset_ms = points.back().curvature after the sort (0 for an empty cloud); either
+ * may be NULL.  The records fill the idle one of two device sets on the copy stream and never wait for an update that is
+ * running; a page-locked source (flb_host_alloc) is read in place, a pageable one is free on return.  Blocking (one
+ * 16-byte read, a second one when the times had to be sorted).  n_records 0 or 1, or everything filtered, gives an empty
+ * cloud (sync_packages skips points.size() <= 1 itself, src/laserMapping.cpp:538).  A successful call resets the cursor
+ * (lidar_scan_index_now) to 0.  On any error the previous cloud and its cursor stay current and unchanged:
+ *   FLB_ERR_INVALID: fmt NULL, records NULL with n_records > 0, n_records < 0, an unknown kind, point_filter_num < 1,
+ *   n_scans < 1, blind not finite, a field that does not fit in point_step or is not aligned to its type, a Velodyne
+ *   cloud without times, a kept coordinate or time that is not finite. */
+#define FLB_LIDAR_LIVOX    1
+#define FLB_LIDAR_VELODYNE 2
+#define FLB_LIDAR_OUSTER   3
+#define FLB_LIDAR_XT32     4
+typedef struct flb_lidar_format {
+    int    kind;               /* FLB_LIDAR_* (LID_TYPE, include/preprocess.h:13) */
+    int    point_step;         /* bytes per record: sizeof(livox_ros_driver::CustomPoint) (20) or PointCloud2::point_step */
+    int    off_x, off_y, off_z;/* float32 fields; Livox: 4, 8, 12 */
+    int    off_time;           /* Livox offset_time (u32, 0); Ouster t (u32); Velodyne time (f32); XT32 timestamp (f64) */
+    int    off_tag, off_line;  /* Livox only (u8 at 17 and 18); ignored otherwise */
+    int    n_scans;            /* N_SCANS (scan_line); read by the Livox handler only */
+    int    point_filter_num;   /* >= 1 */
+    double blind;              /* Preprocess::blind, used per handler as above */
+} flb_lidar_format;
+int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* records, int n_records, int* n_points,
+                     float* last_offset_ms);
+/* The current cloud, x, y, z, curvature per point, for tests and for a node that publishes the raw cloud.  *n_out (may
+ * be NULL) = its size; xyzt may be NULL.  Blocking.  FLB_ERR_STATE without a cloud, FLB_ERR_INVALID when
+ * capacity_points is below its size. */
+int flb_lidar_download(flb_handle* h, float* xyzt, int capacity_points, int* n_out);
+/* UndistortPcl from :621 on with the device cloud as lidar_meas.lidar.  The window (:634-639): the points from the
+ * handle's cursor on while (double)curvature <= pcl_offset_time, read in place; *n_taken (may be NULL) = pcl_out.size().
+ * Then everything flb_imu_undistort does on those points, with the same outputs (out_xyz may be NULL; its capacity is
+ * capacity_points) and the same effect on flb_scan_from_undistorted / flb_world_cloud(FLB_CLOUD_UNDISTORTED).  The cursor
+ * advances by *n_taken, or returns to 0 when is_lidar_end (:643-646).  pcl_offset_time is the caller's (:631-633): 0.0
+ * for a camera update, (pcl_end_time - lidar_beg_time) * 1000 at the scan end.  That product can round below
+ * points.back().curvature; the last points are then left out, as in the reference, and dropped by the cursor's reset.
+ *   FLB_ERR_STATE: no cloud; no device state.  FLB_ERR_INVALID: as flb_imu_undistort, a NaN pcl_offset_time, or
+ *   capacity_points < *n_taken with out_xyz given.  On an error the cursor does not move. */
+int flb_imu_undistort_lidar(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* carry, const flb_imu_sample* v_imu,
+                            int n_imu, double pcl_beg_time, double pcl_end_time, double pcl_offset_time, int is_lidar_end,
+                            int* n_taken, float* out_xyz, int capacity_points, double* poses_out, int* n_poses_out);
+
 /* ---- scan ------------------------------------------------------------------------
  * feats_down_body (src/laserMapping.cpp:1398-1399): N already-downsampled points in
  * the LiDAR body frame. */
