@@ -26,6 +26,8 @@
 //   flb::preprocess(h, livox_msg, n_scans, blind, point_filter_num)  /  flb::preprocess(h, pc2_msg, kind, n_scans, blind,
 //        point_filter_num)   replace p_pre->process (src/preprocess.cpp:43-70) and the sort of sync_packages
 //        (src/laserMapping.cpp:551): the driver's records go up as they are; the cloud is decoded and sorted on the device
+//   flb::preprocess_velodyne(h, pc2_msg, n_scans, blind, point_filter_num)   the same for a Velodyne in any field layout,
+//        with the times derived from the yaw angle on the device when the cloud has none (src/preprocess.cpp:376-428)
 //   flb::undistort_pcl_from_lidar(h, prm, carry, v_imu, lidar_meas, state_inout)   replaces UndistortPcl from :621 on
 //        with that device cloud as lidar_meas.lidar (the window, the LidarMeasureGroup bookkeeping, the propagation)
 //
@@ -449,6 +451,39 @@ inline LidarInfo preprocess(flb_handle* h, const PointCloud2& msg, int kind, int
     LidarInfo r{};
     const int n = (int)((size_t)msg.width * msg.height);
     check(h, flb_lidar_upload(h, &f, n > 0 ? msg.data.data() : nullptr, n, &r.n_points, &r.last_offset_ms));
+    return r;
+}
+
+// sensor_msgs::PointCloud2 of any Velodyne driver: velodyne_handler with or without per-point times, fields at any
+// offset.  x, y, z (FLOAT32) and ring (UINT16) are looked up by name, time (FLOAT32) when the cloud has one; a missing
+// field or another datatype throws.  yaw_times = the times came from the yaw angle (!given_offset_time, src/preprocess.cpp:279).
+struct VelodyneInfo : LidarInfo {
+    bool yaw_times;
+};
+template <class PointCloud2>
+inline VelodyneInfo preprocess_velodyne(flb_handle* h, const PointCloud2& msg, int n_scans, double blind, int point_filter_num) {
+    enum { kUint16 = 4, kFloat32 = 7 };                  // sensor_msgs::PointField datatypes
+    flb_velodyne_format f{};
+    f.point_step = (int)msg.point_step;
+    f.off_x = f.off_y = f.off_z = f.off_time = f.off_ring = -1;
+    for (const auto& fld : msg.fields) {
+        int* off = fld.name == "x" ? &f.off_x : fld.name == "y" ? &f.off_y : fld.name == "z" ? &f.off_z
+                 : fld.name == "time" ? &f.off_time : fld.name == "ring" ? &f.off_ring : nullptr;
+        if (!off) continue;
+        if ((int)fld.datatype != (off == &f.off_ring ? kUint16 : kFloat32))
+            throw Error(FLB_ERR_INVALID, ("preprocess_velodyne: field " + std::string(fld.name) + " has the wrong datatype").c_str());
+        *off = (int)fld.offset;
+    }
+    if (f.off_x < 0 || f.off_y < 0 || f.off_z < 0 || f.off_ring < 0)
+        throw Error(FLB_ERR_INVALID, "preprocess_velodyne: the cloud lacks one of the fields x, y, z, ring");
+    f.n_scans = n_scans;
+    f.point_filter_num = point_filter_num;
+    f.blind = blind;
+    VelodyneInfo r{};
+    int yaw = 0;
+    const int n = (int)((size_t)msg.width * msg.height);
+    check(h, flb_lidar_upload_velodyne(h, &f, n > 0 ? msg.data.data() : nullptr, n, &r.n_points, &r.last_offset_ms, &yaw));
+    r.yaw_times = yaw != 0;
     return r;
 }
 

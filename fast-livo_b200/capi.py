@@ -50,6 +50,12 @@ class LidarFormat(C.Structure):
                 ("point_filter_num", C.c_int), ("blind", C.c_double)]
 
 
+class VelodyneFormat(C.Structure):
+    """flb_velodyne_format: where a Velodyne PointCloud2 record keeps x, y, z, time (-1: none) and ring, at any offset."""
+    _fields_ = [("point_step", C.c_int), ("off_x", C.c_int), ("off_y", C.c_int), ("off_z", C.c_int), ("off_time", C.c_int),
+                ("off_ring", C.c_int), ("n_scans", C.c_int), ("point_filter_num", C.c_int), ("blind", C.c_double)]
+
+
 class State18(C.Structure):
     _fields_ = [("rot", C.c_double * 9), ("pos", C.c_double * 3), ("vel", C.c_double * 3),
                 ("bg", C.c_double * 3), ("ba", C.c_double * 3), ("grav", C.c_double * 3),
@@ -194,7 +200,7 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
            "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset",
            "flb_image_upload_bgr", "flb_image_download",
-           "flb_lidar_upload", "flb_lidar_download", "flb_imu_undistort_lidar"]
+           "flb_lidar_upload", "flb_lidar_download", "flb_imu_undistort_lidar", "flb_lidar_upload_velodyne"]
 
 
 def lib_path() -> str:
@@ -251,6 +257,8 @@ def lib():
                                         vp, C.c_int, C.c_int, C.c_int, vp, vp, C.POINTER(C.c_int)]
         L.flb_lidar_upload.argtypes = [vp, C.POINTER(LidarFormat), vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_float)]
         L.flb_lidar_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_lidar_upload_velodyne.argtypes = [vp, C.POINTER(VelodyneFormat), vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_float),
+                                                C.POINTER(C.c_int)]
         L.flb_imu_undistort_lidar.argtypes = [vp, C.POINTER(ImuParams), C.POINTER(ImuCarry), vp, C.c_int, C.c_double, C.c_double,
                                               C.c_double, C.c_int, C.POINTER(C.c_int), vp, C.c_int, vp, C.POINTER(C.c_int)]
         L.flb_visual_candidates.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
@@ -802,6 +810,18 @@ class Handle:
         self._ck(self.L.flb_lidar_upload(self.h, C.byref(fmt), _p(a) if a.size else None, int(n_records), C.byref(n), C.byref(last)))
         self._lid_n = n.value
         return n.value, np.float32(last.value)
+
+    def lidar_upload_velodyne(self, fmt: VelodyneFormat, records, n_records=None):
+        """flb_lidar_upload_velodyne: records = a uint8 array (or bytes) of n_records Velodyne records of fmt.point_step
+        bytes.  Returns (pl_surf.size(), points.back().curvature after the sort, whether the times came from the yaw)."""
+        a = np.frombuffer(records, np.uint8) if isinstance(records, (bytes, bytearray)) else records
+        if n_records is None:
+            n_records = a.size // max(fmt.point_step, 1)
+        n, last, yaw = C.c_int(), C.c_float(), C.c_int()
+        self._ck(self.L.flb_lidar_upload_velodyne(self.h, C.byref(fmt), _p(a) if a.size else None, int(n_records), C.byref(n),
+                                                  C.byref(last), C.byref(yaw)))
+        self._lid_n = n.value
+        return n.value, np.float32(last.value), bool(yaw.value)
 
     def lidar_download(self):
         """flb_lidar_download: the decoded, time-sorted cloud, (n, 4) float32 x, y, z, curvature."""

@@ -263,6 +263,8 @@ struct flb_handle {
     DevBuf<int> lid_flags;                     // valid -> valid_num | kept | pos, n each; then the LidarRecord
     DevBuf<int> lid_win;                       // flb_imu_undistort_lidar: the window's point count (on `stream`)
     DevBuf<unsigned> lid_keys, lid_keys_sorted;
+    DevBuf<int> lid_idx;                       // flb_lidar_upload_velodyne's yaw route: record indices, then in ring order
+    DevBuf<VeloMap> lid_map;                   // its per-record time maps in ring order, scanned in place
     Staging st_lidar;
     PinBuf pin_lidar;
     // flb_world_cloud: pcl_wait_pub (packed xyz, the caller's order) with its exact bounds; wc_n < 0: no cloud held
@@ -1061,6 +1063,7 @@ int flb_destroy(flb_handle* h) {
     h->scan_alt.release(); h->plane_alt.release(); h->sel_alt.release(); h->plane_ok_alt.release(); h->sf_down.release();
     h->lid_cloud.release(); h->lid_cloud_alt.release(); h->lid_raw.release(); h->lid_cub.release(); h->lid_dec.release();
     h->lid_sorted.release(); h->lid_flags.release(); h->lid_win.release(); h->lid_keys.release(); h->lid_keys_sorted.release();
+    h->lid_idx.release(); h->lid_map.release();
     h->st_lidar.release(); h->pin_lidar.release();
     h->img_alt.release(); h->patch_pos_alt.release(); h->patch_ref_alt.release(); h->patch_level_alt.release();
     for (int k = 0; k < 2; ++k) {
@@ -1915,6 +1918,11 @@ int lidar_time_bytes(int kind) { return kind == kLidarXt32 ? 8 : 4; }
 
 bool lidar_field_ok(int off, int bytes, int step) { return off >= 0 && off % bytes == 0 && off + bytes <= step; }
 
+struct VeloYaw { int off_ring, n_scans; };      // flb_lidar_upload_velodyne's route without per-point times
+
+int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const void* records, int n_records, const VeloYaw* yaw,
+                      int* n_points, float* last_offset_ms);
+
 }  // namespace
 
 int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* records, int n_records, int* n_points,
@@ -1940,10 +1948,22 @@ int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* rec
         float t_last;                                                              // given_offset_time, :279
         std::memcpy(&t_last, rec_h + (size_t)(n_records - 1) * step + f.off_time, sizeof(t_last));
         if (!(t_last > 0))
-            return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: a Velodyne cloud without per-point times (last time %g): the yaw-derived "
-                        "times (src/preprocess.cpp:389-419) are a sequential per-ring walk and stay with the host", (double)t_last);
+            return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: a Velodyne cloud without per-point times (last time %g): its times "
+                        "come from the yaw angle (src/preprocess.cpp:389-419), which flb_lidar_upload_velodyne derives", (double)t_last);
     }
     if (n_records > 0 && fmt->kind == kLidarXt32) std::memcpy(&f.time_head, rec_h + f.off_time, sizeof(double));   // :441
+    return lidar_upload_core(h, "flb_lidar_upload", f, records, n_records, nullptr, n_points, last_offset_ms);
+}
+
+namespace {
+
+// flb_lidar_upload and flb_lidar_upload_velodyne from the argument checks on: decode, filter, compact and time-sort the
+// records into the idle cloud set, and swap it in.  yaw: the Velodyne route without per-point times; nullptr: the
+// handler's own per-record times.
+int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const void* records, int n_records, const VeloYaw* yaw,
+                      int* n_points, float* last_offset_ms) {
+    const int step = f.step;
+    const bool livox = f.kind == kLidarLivox;
     const size_t n = (size_t)n_records, n1 = std::max<size_t>(n, 1), raw_bytes = n * step;
     FLB_CUDA(h, h->lid_raw.reserve(std::max<size_t>(raw_bytes, 4)));
     FLB_CUDA(h, h->lid_cloud_alt.reserve(n1));
@@ -1977,24 +1997,62 @@ int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* rec
         FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t2, d_kept, d_pos, n_records, cs));
         FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p, h->lid_sorted.p,
                                                     n_records, 0, 32, cs));
-        FLB_CUDA(h, h->lid_cub.reserve(std::max(t1, std::max(t2, t3))));
+        // the yaw route: ring keys in [0, n_rings], record indices, and the ring-order maps
+        const int n_rings = yaw ? std::min(yaw->n_scans, 65536) : 0;
+        int key_bits = 1;
+        while (key_bits < 17 && (1 << key_bits) <= n_rings) ++key_bits;
+        int* d_idx = nullptr;
+        int* d_idx_sorted = nullptr;
+        int* d_bad_ring = reinterpret_cast<int*>(d_rec + 1);
+        size_t t4 = 0, t5 = 0;
+        if (yaw) {
+            FLB_CUDA(h, h->lid_idx.reserve(2 * n1));
+            FLB_CUDA(h, h->lid_map.reserve(n1));
+            d_idx = h->lid_idx.p, d_idx_sorted = h->lid_idx.p + n1;
+            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t4, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted, n_records,
+                                                        0, key_bits, cs));
+            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(nullptr, t5, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
+        }
+        FLB_CUDA(h, h->lid_cub.reserve(std::max(std::max(t1, std::max(t2, t3)), std::max(t4, t5))));
         const int g = (n_records + 255) / 256;
         FLB_CUDA(h, cudaMemsetAsync(d_rec, 0, sizeof(LidarRecord), cs));
-        if (livox) {
-            k_lidar_valid<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum);
-            FLB_CUDA(h, cub::DeviceScan::InclusiveSum(h->lid_cub.p, t1, d_vnum, d_vnum, n_records, cs));
-            h->launches += 2;
+        if (yaw) {
+            FLB_CUDA(h, cudaMemsetAsync(d_bad_ring, 0x7f, sizeof(int), cs));      // 0x7f7f7f7f: no bad ring
+            k_velo_rings<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, step, yaw->off_ring, yaw->n_scans, n_rings, h->lid_keys.p, d_idx,
+                                           d_bad_ring);
+            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t4, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted,
+                                                        n_records, 0, key_bits, cs));
+            k_velo_maps<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, n_rings, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p);
+            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t5, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
+            k_velo_flags<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, n_rings, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p,
+                                           h->lid_dec.p, d_kept);
+            h->launches += 5;
+        } else {
+            if (livox) {
+                k_lidar_valid<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum);
+                FLB_CUDA(h, cub::DeviceScan::InclusiveSum(h->lid_cub.p, t1, d_vnum, d_vnum, n_records, cs));
+                h->launches += 2;
+            }
+            k_lidar_flags<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum, h->lid_dec.p, d_kept);
+            h->launches += 1;
         }
-        k_lidar_flags<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum, h->lid_dec.p, d_kept);
         FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t2, d_kept, d_pos, n_records, cs));
         k_lidar_scatter<<<g, 256, 0, cs>>>(h->lid_dec.p, d_kept, d_pos, n_records, h->lid_cloud_alt.p, h->lid_keys.p, d_rec);
         k_lidar_order<<<g, 256, 0, cs>>>(h->lid_cloud_alt.p, h->lid_keys.p, n_records, d_rec);
         FLB_CUDA(h, cudaGetLastError());
-        h->launches += 4;
-        FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
+        h->launches += 3;
+        int bad_ring = INT_MAX;
+        FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec) + (yaw ? sizeof(int) : 0), cudaMemcpyDeviceToHost, cs));
         FLB_CUDA(h, cudaStreamSynchronize(cs));
         std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
-        if (rec.bad) return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: a kept point or time is not finite");
+        if (yaw) std::memcpy(&bad_ring, static_cast<const char*>(h->pin_lidar.p) + sizeof(rec), sizeof(int));
+        if (bad_ring < n_records) {
+            uint16_t ring;
+            std::memcpy(&ring, static_cast<const unsigned char*>(records) + (size_t)bad_ring * step + yaw->off_ring, sizeof(ring));
+            return fail(h, FLB_ERR_INVALID, "%s: record %d has ring %u >= n_scans %d (the per-ring yaw state has no such ring)", who,
+                        bad_ring, (unsigned)ring, yaw->n_scans);
+        }
+        if (rec.bad) return fail(h, FLB_ERR_INVALID, "%s: a kept point or time is not finite", who);
         if (rec.unsorted) {
             // stable: equal times keep record order (std::sort leaves that order unspecified in the reference)
             FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p,
@@ -2017,6 +2075,40 @@ int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* rec
     h->lid_cursor = 0;
     if (n_points) *n_points = rec.n_kept;
     if (last_offset_ms) *last_offset_ms = rec.n_kept > 0 ? rec.last : 0.f;
+    return FLB_OK;
+}
+
+bool velo_field_ok(int off, int bytes, int step) { return off >= 0 && off <= step - bytes; }
+
+}  // namespace
+
+int flb_lidar_upload_velodyne(flb_handle* h, const flb_velodyne_format* fmt, const void* records, int n_records, int* n_points,
+                              float* last_offset_ms, int* yaw_times) {
+    FLB_CHECK_H(h);
+    const char* who = "flb_lidar_upload_velodyne";
+    if (n_records < 0 || !fmt || (n_records > 0 && !records)) return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
+    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || !std::isfinite(fmt->blind))
+        return fail(h, FLB_ERR_INVALID, "%s: point_filter_num %d, n_scans %d, blind %g", who, fmt->point_filter_num, fmt->n_scans,
+                    fmt->blind);
+    const int step = fmt->point_step;
+    if (step < 1 || !velo_field_ok(fmt->off_x, 4, step) || !velo_field_ok(fmt->off_y, 4, step) || !velo_field_ok(fmt->off_z, 4, step) ||
+        !velo_field_ok(fmt->off_ring, 2, step) || (fmt->off_time != -1 && !velo_field_ok(fmt->off_time, 4, step)))
+        return fail(h, FLB_ERR_INVALID, "%s: a field does not fit in point_step %d", who, step);
+    LidarFmt f{};
+    f.kind = kLidarVelodyne, f.step = step, f.off_x = fmt->off_x, f.off_y = fmt->off_y, f.off_z = fmt->off_z;
+    f.off_time = fmt->off_time >= 0 ? fmt->off_time : 0;
+    f.n_scans = fmt->n_scans, f.filter_num = fmt->point_filter_num, f.blind = fmt->blind;
+    // given_offset_time (:279): the last record's time > 0.  Without a time field the reference reads 0.
+    bool given = n_records == 0;
+    if (n_records > 0 && fmt->off_time >= 0) {
+        float t_last;
+        std::memcpy(&t_last, static_cast<const unsigned char*>(records) + (size_t)(n_records - 1) * step + fmt->off_time, sizeof(t_last));
+        given = t_last > 0;
+    }
+    VeloYaw yaw{fmt->off_ring, fmt->n_scans};
+    const int rc = lidar_upload_core(h, who, f, records, n_records, given ? nullptr : &yaw, n_points, last_offset_ms);
+    if (rc) return rc;
+    if (yaw_times) *yaw_times = given ? 0 : 1;
     return FLB_OK;
 }
 

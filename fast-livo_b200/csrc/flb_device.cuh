@@ -1695,4 +1695,48 @@ FLB_HD unsigned lidar_time_key(float t) {
 }
 FLB_HD bool lidar_finite(float v) { return (float_as_u32(v) & 0x7f800000u) != 0x7f800000u; }
 
+// ------------------------------------------------------------------ Velodyne times from the yaw angle
+// velodyne_handler's non-feature branch without per-point times (src/preprocess.cpp:376-428, flb_lidar_upload_velodyne).
+// Per ring, the first record sets yaw_fp and time_last = 0 and is never kept; every later record j gets
+//   base_j = float((yaw_fp - yaw_j [+ 360]) / omega_l),  t_j = base_j < time_last ? float(base_j + 360 / omega_l) : base_j,
+// and time_last = t_j.  Each step is the map x -> x > c ? a : b on time_last; such maps compose into one of the same form,
+// so the walk over a ring is an inclusive scan of VeloMap under velo_compose.
+
+// 16 bits of a little-endian record field at any offset (the ring)
+FLB_HD unsigned lidar_ld16(const unsigned char* p) { return (unsigned)p[0] | ((unsigned)p[1] << 8); }
+
+// omega_l (:272) and 360.0 / omega_l (:415), in the reference's double arithmetic
+FLB_HD double velo_omega() { return 0.361 * 10; }
+FLB_HD double velo_wrap() { return 360.0 / velo_omega(); }
+
+// The yaw of :392 in degrees.  The reference calls atan2 on two floats, which resolves to the float overload and so to
+// the libm it links; the project defines the angle as the double atan2 rounded to float (DESIGN §2).  The widening to
+// double before the multiply is the reference's.
+FLB_HD double velo_yaw(float x, float y) { return (double)(float)atan2((double)y, (double)x) * 57.2957; }
+
+struct VeloMap { float c, a, b; };    // x -> (x > c) ? a : b
+
+FLB_HD float velo_apply(const VeloMap& m, float x) { return x > m.c ? m.a : m.b; }
+// `first` then `then`: x > first.c selects first.a or first.b, which `then` maps on.  Exact for every input, NaN
+// included (a NaN compares false), so the operator is associative.
+FLB_HD VeloMap velo_compose(const VeloMap& first, const VeloMap& then) {
+    VeloMap m;
+    m.c = first.c;
+    m.a = velo_apply(then, first.a);
+    m.b = velo_apply(then, first.b);
+    return m;
+}
+// The first record of a ring: time_last = 0 whatever came before (:394-403).  A constant map, so a scan in ring order
+// needs no segment boundaries: the head absorbs the prefix of the rings before it.
+FLB_HD VeloMap velo_head() { VeloMap m; m.c = 0.f; m.a = 0.f; m.b = 0.f; return m; }
+// Every later record of the ring (:406-417).  A NaN yaw gives a NaN base, so the next record cannot wrap.
+FLB_HD VeloMap velo_step(double yaw, double yaw_fp) {
+    const float base = yaw <= yaw_fp ? (float)((yaw_fp - yaw) / velo_omega()) : (float)((yaw_fp - yaw + 360.0) / velo_omega());
+    VeloMap m;
+    m.c = base;
+    m.a = (float)((double)base + velo_wrap());
+    m.b = base;
+    return m;
+}
+
 }  // namespace flb

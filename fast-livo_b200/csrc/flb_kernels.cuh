@@ -3612,4 +3612,77 @@ __global__ void k_lidar_window(const float4* __restrict__ cloud, int begin, int 
     *n_taken = lo - begin;
 }
 
+// ---- Velodyne times from the yaw angle (flb_lidar_upload_velodyne) ---------------------------------------------------
+// velodyne_handler without per-point times (src/preprocess.cpp:376-428).  A stable radix sort puts the record indices in
+// ring order; the rings' walks are then one inclusive scan of velo_step maps (flb_device.cuh), and k_velo_flags writes
+// the times back in record order as k_lidar_flags's dec / kept, from which flb_lidar_upload's compaction and time sort
+// go on.  A thread owns one record (k_velo_rings) or one position in ring order (k_velo_maps, k_velo_flags).
+
+struct VeloComposeOp {
+    __device__ __forceinline__ VeloMap operator()(const VeloMap& first, const VeloMap& then) const { return velo_compose(first, then); }
+};
+
+// key[i] = record i's ring, or n_rings for a ring >= n_scans, whose first record goes to *bad_ring (preset to 0x7f7f7f7f,
+// above every record index); idx[i] = i, the radix sort's values.
+__global__ void __launch_bounds__(256) k_velo_rings(const unsigned char* __restrict__ raw, int n, int step, int off_ring, int n_scans,
+                                                    int n_rings, unsigned* __restrict__ key, int* __restrict__ idx, int* __restrict__ bad_ring) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned ring = lidar_ld16(raw + (size_t)i * step + off_ring);
+    const bool ok = (int)ring < n_scans;
+    key[i] = ok ? ring : (unsigned)n_rings;
+    idx[i] = i;
+    if (!ok) atomicMin(bad_ring, i);
+}
+
+// First position of ring k in the sorted keys: the ring's first record in record order (the sort is stable).
+__device__ __forceinline__ int velo_head_pos(const unsigned* __restrict__ key, int p, unsigned k) {
+    int lo = 0, hi = p;
+    while (lo < hi) {
+        const int mid = lo + (hi - lo) / 2;
+        if (key[mid] < k) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// map[p] = the step of the record at ring-order position p: velo_head for a ring's first record (and for a bad ring,
+// which fails the upload), else velo_step against the yaw of the ring's first record (the head gather).
+__global__ void __launch_bounds__(256) k_velo_maps(const unsigned char* __restrict__ raw, int n, LidarFmt f, int n_rings,
+                                                   const unsigned* __restrict__ key, const int* __restrict__ idx, VeloMap* __restrict__ map) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    const unsigned k = key[p];
+    const int hp = k < (unsigned)n_rings ? velo_head_pos(key, p, k) : p;
+    VeloMap m = velo_head();
+    if (hp != p) {
+        const unsigned char* r = raw + (size_t)idx[p] * f.step;
+        const unsigned char* h = raw + (size_t)idx[hp] * f.step;
+        const double yaw = velo_yaw(u32_as_float(lidar_ld32(r + f.off_x)), u32_as_float(lidar_ld32(r + f.off_y)));
+        const double yaw_fp = velo_yaw(u32_as_float(lidar_ld32(h + f.off_x)), u32_as_float(lidar_ld32(h + f.off_y)));
+        m = velo_step(yaw, yaw_fp);
+    }
+    map[p] = m;
+}
+
+// After the scan: t = the scanned map applied to time_last = 0.  dec / kept in record order as k_lidar_flags writes them;
+// a ring's first record is never kept (the `continue` of :403), a later one by :421-423.
+__global__ void __launch_bounds__(256) k_velo_flags(const unsigned char* __restrict__ raw, int n, LidarFmt f, int n_rings,
+                                                    const unsigned* __restrict__ key, const int* __restrict__ idx,
+                                                    const VeloMap* __restrict__ scanned, float4* __restrict__ dec, int* __restrict__ kept) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    const int i = idx[p];
+    const unsigned k = key[p];
+    const bool head = p == 0 || key[p - 1] != k;
+    const unsigned char* r = raw + (size_t)i * f.step;
+    LidarPoint q;
+    q.x = u32_as_float(lidar_ld32(r + f.off_x));
+    q.y = u32_as_float(lidar_ld32(r + f.off_y));
+    q.z = u32_as_float(lidar_ld32(r + f.off_z));
+    q.t = head ? 0.f : velo_apply(scanned[p], 0.f);
+    dec[i] = make_float4(q.x, q.y, q.z, q.t);
+    kept[i] = (k < (unsigned)n_rings && !head && lidar_pc2_keep(q, i, f)) ? 1 : 0;
+}
+
 }  // namespace flb

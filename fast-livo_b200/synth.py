@@ -472,6 +472,69 @@ def make_lidar_message(kind, seed=1, n=24000, point_filter_num=None, unsorted=No
     return a.tobytes(), fmt
 
 
+# Velodyne PointCloud2 layouts (flb_lidar_upload_velodyne's input): XYZIRT (velodyne_pointcloud with times), a packed
+# 22-byte XYZIRT with the float time at 18, and a 32-byte XYZIR (pcl::PointXYZIR's padded layout) without a time field.
+VELODYNE_LAYOUTS = {
+    "xyzirt": (np.dtype({"names": ["x", "y", "z", "intensity", "ring", "time"], "formats": ["<f4", "<f4", "<f4", "<f4", "<u2", "<f4"],
+                         "offsets": [0, 4, 8, 12, 16, 20], "itemsize": 24}), 20),
+    "packed22": (np.dtype({"names": ["x", "y", "z", "intensity", "ring", "time"], "formats": ["<f4", "<f4", "<f4", "<f4", "<u2", "<f4"],
+                           "offsets": [0, 4, 8, 12, 16, 18], "itemsize": 22}), 18),
+    "xyzir32": (np.dtype({"names": ["x", "y", "z", "intensity", "ring"], "formats": ["<f4", "<f4", "<f4", "<f4", "<u2"],
+                          "offsets": [0, 4, 8, 16, 20], "itemsize": 32}), -1),
+}
+
+
+def make_velodyne_spin(layout="xyzirt", seed=1, n_scans=16, n_cols=1800, point_filter_num=1, timed=False, blind=1.0):
+    """One spin of a rotating Velodyne as (records, fmt): the raw PointCloud2 data and a dict of flb_velodyne_format's
+    fields.  Column by column, the rings fire in an interleaved order; the yaw turns clockwise from a random start through
+    a little over 360 degrees, so it crosses +-180 and each ring's time_last wraps near the end; azimuth jitter makes some
+    later records turn back, which the reference's walk takes for a spurious wrap.  Also: NaN no-return records (never a
+    ring's first record, which would make the whole ring's times NaN), -0.0 coordinates (atan2 gives +-pi), points inside
+    blind, an empty ring (ring 1 never fires) and a one-record ring (ring n_scans - 1 fires once).  layout: a key of
+    VELODYNE_LAYOUTS.  timed: per-point times in seconds (a layout without a time field ignores it); otherwise every time
+    is 0 and the times come from the yaw."""
+    dt, off_time = VELODYNE_LAYOUTS[layout]
+    rng = np.random.default_rng(7919 * seed + n_scans)
+    order = np.concatenate([np.arange(0, n_scans, 2), np.arange(1, n_scans, 2)])          # interleaved firing order
+    order = order[order != 1]                                                            # the empty ring
+    lone = n_scans - 1
+    ring = np.tile(order, n_cols)
+    col = np.repeat(np.arange(n_cols), len(order))
+    keep = (ring != lone) | (col == n_cols // 3)                                         # the one-record ring
+    ring, col = ring[keep], col[keep]
+    n = len(ring)
+    pos = np.zeros(n_scans, np.int64)
+    pos[order] = np.arange(len(order))
+    slot = pos[ring]                                                                     # position in the firing order
+    spin = 360.0 + rng.uniform(2.0, 8.0)                                                 # a little over one turn
+    az = rng.uniform(-180.0, 180.0) - spin * (col + slot / len(order)) / n_cols          # clockwise
+    az += rng.normal(0.0, 0.1, n)                                                        # azimuth jitter
+    el = np.deg2rad(-15.0 + 30.0 * ring / max(n_scans - 1, 1))
+    d = rng.uniform(1.2, 60.0, n)
+    near = rng.random(n) < 0.03
+    d[near] = rng.uniform(0.05, 0.95 * blind, near.sum())
+    a_rad = np.deg2rad(az)
+    xyz = np.stack([d * np.cos(el) * np.cos(a_rad), d * np.cos(el) * np.sin(a_rad), d * np.sin(el)], 1).astype(np.float32)
+    first = np.zeros(n, bool)
+    first[np.unique(ring, return_index=True)[1]] = True
+    nan = (rng.random(n) < 0.03) & ~first
+    xyz[nan] = np.nan
+    neg = np.flatnonzero(~first & ~nan)
+    z0 = rng.choice(neg, min(len(neg), 24), replace=False)
+    xyz[z0[:8], 1] = -0.0                                                                # y = -0.0: atan2 gives -pi or -0
+    xyz[z0[8:16], 0] = -0.0                                                              # x = -0.0: +-pi/2
+    xyz[z0[16:], :2] = np.float32([-0.0, -0.0]) * rng.choice([1, -1], (len(z0[16:]), 2))   # both zero: +-0 or +-pi
+    a = np.zeros(n, dt)
+    a["x"], a["y"], a["z"] = xyz[:, 0], xyz[:, 1], xyz[:, 2]
+    a["intensity"] = rng.uniform(0, 255, n)
+    a["ring"] = ring
+    if off_time >= 0 and timed:
+        a["time"] = col * 55.296e-6 + slot * 2.304e-6 + 1e-6
+    fmt = dict(point_step=dt.itemsize, off_x=0, off_y=4, off_z=8, off_time=off_time, off_ring=dt.fields["ring"][1], n_scans=n_scans,
+               point_filter_num=point_filter_num, blind=blind)
+    return a.tobytes(), fmt
+
+
 # ---------------------------------------------------------------------------------------------------------
 # Visual-map sequences (SURVEY.md section 8 rows f2 / f4): several frames of ONE scene along a short trajectory
 # ---------------------------------------------------------------------------------------------------------

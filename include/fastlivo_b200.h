@@ -243,6 +243,47 @@ int flb_imu_undistort_lidar(flb_handle* h, const flb_imu_params* prm, flb_imu_ca
                             int n_imu, double pcl_beg_time, double pcl_end_time, double pcl_offset_time, int is_lidar_end,
                             int* n_taken, float* out_xyz, int capacity_points, double* poses_out, int* n_poses_out);
 
+/* ---- a Velodyne message in any field layout, with or without per-point times ------------------------------
+ * velodyne_handler (src/preprocess.cpp:259-297, and its non-feature branch :376-428) on the PointCloud2 data of any
+ * Velodyne driver: XYZIRT, XYZIR without a time field, a time of 0 everywhere, and float fields at any byte offset
+ * (a packed 22-byte record puts the time at 18).  The result goes where flb_lidar_upload's goes, so flb_lidar_download
+ * and flb_imu_undistort_lidar work on it unchanged.
+ *   With times (the last record's time > 0, given_offset_time, :279): exactly flb_lidar_upload(FLB_LIDAR_VELODYNE) on
+ *     the same records wherever that call accepts the layout; the ring is not read.  *yaw_times = 0.
+ *   Without times: the times come from the yaw angle, per ring (layer = ring, :391), in record order:
+ *     yaw = atan2(y, x) * 57.2957 (:392).  The reference's arguments are floats, so its atan2 is the float overload of
+ *       the libm it links; here the yaw is defined as (float)atan2((double)y, (double)x), widened to double before the
+ *       multiply.  The two agree except near float rounding midpoints; DESIGN §2 gives the effect (a few 1e-6 ms).
+ *     The first record of a ring sets yaw_fp = yaw and time_last = 0 and is never kept (the `continue` of :403), whatever
+ *       i % point_filter_num is; it still uses up its index i.
+ *     Every later record: base = float((yaw_fp - yaw) / omega_l) when yaw <= yaw_fp, else float((yaw_fp - yaw + 360.0)
+ *       / omega_l), with omega_l = 0.361 * 10 (:272, :406-413); t = float(base + 360.0 / omega_l) when base < time_last,
+ *       else base (:415); time_last = t.  A NaN yaw (a no-return record) gives a NaN time_last, so the next record of
+ *       the ring cannot wrap.  *yaw_times = 1.
+ *     A record is kept when i % point_filter_num == 0 and the float x*x + y*y + z*z > blind * blind (:421-423).
+ *   The kept points are then sorted by time, stably, as by flb_lidar_upload.  The rings are walked as one parallel scan
+ *   (DESIGN §4.9), not a loop.  n_records 0 gives an empty cloud and *yaw_times = 0.
+ * fmt: off_x, off_y, off_z float32 and off_ring uint16 at any byte offset within point_step; off_time float32 seconds at
+ * any offset, or -1 for a cloud without a time field (the reference then reads 0: the yaw route).  n_points,
+ * last_offset_ms and yaw_times may be NULL.  Everything else is flb_lidar_upload's: the idle set on the copy stream, a
+ * page-locked source read in place, the swap on success only, the cursor reset to 0.  On any error the previous cloud
+ * and its cursor stay current and unchanged:
+ *   FLB_ERR_INVALID: fmt NULL, records NULL with n_records > 0, n_records < 0, point_filter_num < 1, n_scans < 1, blind
+ *   not finite, a field that does not fit in point_step, a ring >= n_scans on the yaw route (the reference indexes past
+ *   its per-ring vectors there; the message names the ring and the record), a kept coordinate or time that is not
+ *   finite (a ring whose first record has no return makes every time of that ring NaN). */
+typedef struct flb_velodyne_format {
+    int    point_step;         /* PointCloud2::point_step */
+    int    off_x, off_y, off_z;/* float32, any alignment */
+    int    off_time;           /* float32 seconds, any alignment; -1: no time field */
+    int    off_ring;           /* uint16, any alignment */
+    int    n_scans;            /* N_SCANS (scan_line) */
+    int    point_filter_num;   /* >= 1 */
+    double blind;              /* Preprocess::blind */
+} flb_velodyne_format;
+int flb_lidar_upload_velodyne(flb_handle* h, const flb_velodyne_format* fmt, const void* records, int n_records, int* n_points,
+                              float* last_offset_ms, int* yaw_times);
+
 /* ---- scan ------------------------------------------------------------------------
  * feats_down_body (src/laserMapping.cpp:1398-1399): N already-downsampled points in
  * the LiDAR body frame. */
