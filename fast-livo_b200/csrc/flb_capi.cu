@@ -2166,6 +2166,7 @@ int flb_visual_candidates(flb_handle* h, const double Rcw[9], const double Pcw[3
     if (!Rcw || !Pcw || n < 0 || (n > 0 && !world_xyz) || stride < 3 || grid_size < 1 || border < 0 || !map_value || !winner)
         return fail(h, FLB_ERR_INVALID, "flb_visual_candidates: bad arguments");
     if (!h->cam_set || h->img_w <= 0) return fail(h, FLB_ERR_STATE, "flb_visual_candidates: camera and image must be set first");
+    if (h->cam.width != h->img_w || h->cam.height != h->img_h) return fail(h, FLB_ERR_STATE, "camera / image size mismatch");
     const int gw = h->img_w / grid_size, gh = h->img_h / grid_size, ncell = gw * gh;      // :55-57
     if (ncell < 1) return fail(h, FLB_ERR_INVALID, "flb_visual_candidates: grid_size larger than the image");
     { int rcq = vio_inputs_acquire(h); if (rcq) return rcq; }                           // the image upload has landed
@@ -3528,6 +3529,7 @@ int flb_batch_update_enqueue(flb_handle* h, const flb_lio_params* lprm, const fl
     const bool vio = vprm != nullptr && h->Pn > 0 && vprm->max_iteration > 0;
     if (vio) {
         if (!h->cam_set || h->img_w <= 0) return fail(h, FLB_ERR_STATE, "flb_batch_update_enqueue: camera and image must be set first");
+        if (h->cam.width != h->img_w || h->cam.height != h->img_h) return fail(h, FLB_ERR_STATE, "camera / image size mismatch");
         if (h->pn_on_device) { int rc = resolve_pn(h); if (rc) return rc; }
     }
     const int nb_lio = (b.n_max + kLioBlock - 1) / kLioBlock;

@@ -476,7 +476,8 @@ int flb_camera_set(flb_handle* h, const flb_camera* cam);
  *   map_value (grid_n_width*grid_n_height floats, grid_n_* = image size / grid_size, :55-56): in = the values
  *   addFromSparseMap left there (:447-455), out = updated.  winner: per cell the index into world_xyz of the
  *   point that took the cell in this call (the reference's add_voxel_points_[cell] / TYPE_POINTCLOUD), -1
- *   otherwise.  Creating the Point / Feature objects for the winners (:174-195) stays with the caller. */
+ *   otherwise.  Creating the Point / Feature objects for the winners (:174-195) stays with the caller.
+ *   FLB_ERR_STATE: no camera or no image, or a camera whose size differs from the uploaded image's. */
 int flb_visual_candidates(flb_handle* h, const double Rcw[9], const double Pcw[3], const float* world_xyz, int n,
                           int stride_floats, int grid_size, int border, float* map_value, int* winner);
 
@@ -658,7 +659,9 @@ int flb_batch_begin(flb_handle* h, int B, int max_points_per_frame);
 int flb_batch_set_frame(flb_handle* h, int frame, const float* body_xyz, int N, int stride_floats, const flb_state18* x,
                         const flb_state18* x_prop);
 int flb_batch_state_reset_enqueue(flb_handle* h);
-/* LIO update of every frame, then (vprm != NULL) VIO update with the LIO posterior as prior.  Enqueue-only. */
+/* LIO update of every frame, then (vprm != NULL) VIO update with the LIO posterior as prior.  Enqueue-only.
+ * FLB_ERR_STATE, before anything is enqueued: no batch, a frame not set, and, when the VIO step runs (vprm != NULL,
+ * patches uploaded, max_iteration > 0), no camera or no image, or a camera whose size differs from the image's. */
 int flb_batch_update_enqueue(flb_handle* h, const flb_lio_params* lprm, const flb_vio_params* vprm);
 int flb_batch_state_download(flb_handle* h, int frame, flb_state18* x, flb_lio_report* lio, flb_vio_report* vio);
 
