@@ -28,6 +28,9 @@
 //        (src/laserMapping.cpp:551): the driver's records go up as they are; the cloud is decoded and sorted on the device
 //   flb::preprocess_velodyne(h, pc2_msg, n_scans, blind, point_filter_num)   the same for a Velodyne in any field layout,
 //        with the times derived from the yaw angle on the device when the cloud has none (src/preprocess.cpp:376-428)
+//   flb::preprocess_features(h, livox_msg, n_scans, blind, point_filter_num)  /  flb::preprocess_features(h, pc2_msg,
+//        FLB_LIDAR_OUSTER or FLB_LIDAR_VELODYNE, n_scans, blind, point_filter_num)   the same with feature_extract_enable = 1:
+//        the handlers' feature branches and give_feature (src/preprocess.cpp:94-135, :174-227, :299-373, :466-936)
 //   flb::undistort_pcl_from_lidar(h, prm, carry, v_imu, lidar_meas, state_inout)   replaces UndistortPcl from :621 on
 //        with that device cloud as lidar_meas.lidar (the window, the LidarMeasureGroup bookkeeping, the propagation)
 //
@@ -484,6 +487,91 @@ inline VelodyneInfo preprocess_velodyne(flb_handle* h, const PointCloud2& msg, i
     const int n = (int)((size_t)msg.width * msg.height);
     check(h, flb_lidar_upload_velodyne(h, &f, n > 0 ? msg.data.data() : nullptr, n, &r.n_points, &r.last_offset_ms, &yaw));
     r.yaw_times = yaw != 0;
+    return r;
+}
+
+// ---- feature_extract_enable = 1: the feature branches and give_feature, pl_surf on the device --------------------
+// Preprocess::disB is never assigned by the reference's constructor (src/preprocess.cpp:12-13 assign disA twice), so a
+// node runs with whatever its heap held.  p_pre is allocated once during static initialisation (src/laserMapping.cpp:208),
+// from memory the process has not used before, which the OS hands out zeroed: 0 is the value such a node sees, and
+// the adapters pass it.  A caller who wants another value calls flb_lidar_upload_features directly.
+constexpr double kFeatureDisB = 0.0;
+
+// livox_ros_driver::CustomMsg: avia_handler's feature branch (:94-135).  Offsets from the type, as flb::preprocess.
+template <class LivoxMsg>
+inline LidarInfo preprocess_features(flb_handle* h, const LivoxMsg& msg, int n_scans, double blind, int point_filter_num) {
+    flb_lidar_format f{};
+    f.kind = FLB_LIDAR_LIVOX;
+    f.point_step = (int)sizeof(msg.points[0]);
+    LidarInfo r{};
+    const int n = (int)msg.point_num;
+    if (n > 0) {
+        const char* p0 = reinterpret_cast<const char*>(&msg.points[0]);
+        f.off_time = (int)(reinterpret_cast<const char*>(&msg.points[0].offset_time) - p0);
+        f.off_x = (int)(reinterpret_cast<const char*>(&msg.points[0].x) - p0);
+        f.off_y = (int)(reinterpret_cast<const char*>(&msg.points[0].y) - p0);
+        f.off_z = (int)(reinterpret_cast<const char*>(&msg.points[0].z) - p0);
+        f.off_tag = (int)(reinterpret_cast<const char*>(&msg.points[0].tag) - p0);
+        f.off_line = (int)(reinterpret_cast<const char*>(&msg.points[0].line) - p0);
+    } else {
+        f.off_x = 4, f.off_y = 8, f.off_z = 12, f.off_tag = 17, f.off_line = 18;
+    }
+    f.n_scans = n_scans;
+    f.point_filter_num = point_filter_num;
+    f.blind = blind;
+    check(h, flb_lidar_upload_features(h, &f, kFeatureDisB, n > 0 ? &msg.points[0] : nullptr, n, &r.n_points, &r.last_offset_ms));
+    return r;
+}
+
+// sensor_msgs::PointCloud2 of an Ouster (kind FLB_LIDAR_OUSTER: oust64_handler's feature branch, :174-227) or a Velodyne
+// (FLB_LIDAR_VELODYNE: velodyne_handler's, :299-373, with or without per-point times).  Fields are looked up by name and
+// their datatypes checked: x, y, z FLOAT32 and, for the Ouster, t UINT32 and ring UINT8; for the Velodyne ring UINT16 and
+// time FLOAT32 when the cloud has one.  A missing field, another datatype or another kind throws before any upload.
+template <class PointCloud2>
+inline VelodyneInfo preprocess_features(flb_handle* h, const PointCloud2& msg, int kind, int n_scans, double blind,
+                                        int point_filter_num) {
+    enum { kUint8 = 2, kUint16 = 4, kUint32 = 6, kFloat32 = 7 };          // sensor_msgs::PointField datatypes
+    if (kind != FLB_LIDAR_OUSTER && kind != FLB_LIDAR_VELODYNE)
+        throw Error(FLB_ERR_INVALID, "preprocess_features: kind must be FLB_LIDAR_OUSTER or FLB_LIDAR_VELODYNE (the XT32 has no "
+                                     "feature branch: flb::preprocess serves it)");
+    const bool ouster = kind == FLB_LIDAR_OUSTER;
+    int off_x = -1, off_y = -1, off_z = -1, off_time = -1, off_ring = -1;
+    for (const auto& fld : msg.fields) {
+        int* off = fld.name == "x" ? &off_x : fld.name == "y" ? &off_y : fld.name == "z" ? &off_z
+                 : fld.name == (ouster ? "t" : "time") ? &off_time : fld.name == "ring" ? &off_ring : nullptr;
+        if (!off) continue;
+        const int want = off == &off_ring ? (ouster ? kUint8 : kUint16) : (off == &off_time && ouster) ? kUint32 : kFloat32;
+        if ((int)fld.datatype != want)
+            throw Error(FLB_ERR_INVALID, ("preprocess_features: field " + std::string(fld.name) + " has the wrong datatype").c_str());
+        *off = (int)fld.offset;
+    }
+    if (off_x < 0 || off_y < 0 || off_z < 0 || off_ring < 0 || (ouster && off_time < 0))
+        throw Error(FLB_ERR_INVALID, ouster ? "preprocess_features: the cloud lacks one of the fields x, y, z, t, ring"
+                                            : "preprocess_features: the cloud lacks one of the fields x, y, z, ring");
+    VelodyneInfo r{};
+    const int n = (int)((size_t)msg.width * msg.height);
+    const void* data = n > 0 ? msg.data.data() : nullptr;
+    if (ouster) {
+        flb_lidar_format f{};
+        f.kind = FLB_LIDAR_OUSTER;
+        f.point_step = (int)msg.point_step;
+        f.off_x = off_x, f.off_y = off_y, f.off_z = off_z, f.off_time = off_time, f.off_line = off_ring;
+        f.n_scans = n_scans;
+        f.point_filter_num = point_filter_num;
+        f.blind = blind;
+        check(h, flb_lidar_upload_features(h, &f, kFeatureDisB, data, n, &r.n_points, &r.last_offset_ms));
+        r.yaw_times = false;
+    } else {
+        flb_velodyne_format f{};
+        f.point_step = (int)msg.point_step;
+        f.off_x = off_x, f.off_y = off_y, f.off_z = off_z, f.off_time = off_time, f.off_ring = off_ring;
+        f.n_scans = n_scans;
+        f.point_filter_num = point_filter_num;
+        f.blind = blind;
+        int yaw = 0;
+        check(h, flb_lidar_upload_velodyne_features(h, &f, kFeatureDisB, data, n, &r.n_points, &r.last_offset_ms, &yaw));
+        r.yaw_times = yaw != 0;
+    }
     return r;
 }
 

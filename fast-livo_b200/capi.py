@@ -200,7 +200,8 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
            "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset",
            "flb_image_upload_bgr", "flb_image_download",
-           "flb_lidar_upload", "flb_lidar_download", "flb_imu_undistort_lidar", "flb_lidar_upload_velodyne"]
+           "flb_lidar_upload", "flb_lidar_download", "flb_imu_undistort_lidar", "flb_lidar_upload_velodyne",
+           "flb_lidar_upload_features", "flb_lidar_upload_velodyne_features"]
 
 
 def lib_path() -> str:
@@ -259,6 +260,10 @@ def lib():
         L.flb_lidar_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
         L.flb_lidar_upload_velodyne.argtypes = [vp, C.POINTER(VelodyneFormat), vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_float),
                                                 C.POINTER(C.c_int)]
+        L.flb_lidar_upload_features.argtypes = [vp, C.POINTER(LidarFormat), C.c_double, vp, C.c_int, C.POINTER(C.c_int),
+                                                C.POINTER(C.c_float)]
+        L.flb_lidar_upload_velodyne_features.argtypes = [vp, C.POINTER(VelodyneFormat), C.c_double, vp, C.c_int, C.POINTER(C.c_int),
+                                                         C.POINTER(C.c_float), C.POINTER(C.c_int)]
         L.flb_imu_undistort_lidar.argtypes = [vp, C.POINTER(ImuParams), C.POINTER(ImuCarry), vp, C.c_int, C.c_double, C.c_double,
                                               C.c_double, C.c_int, C.POINTER(C.c_int), vp, C.c_int, vp, C.POINTER(C.c_int)]
         L.flb_visual_candidates.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
@@ -820,6 +825,30 @@ class Handle:
         n, last, yaw = C.c_int(), C.c_float(), C.c_int()
         self._ck(self.L.flb_lidar_upload_velodyne(self.h, C.byref(fmt), _p(a) if a.size else None, int(n_records), C.byref(n),
                                                   C.byref(last), C.byref(yaw)))
+        self._lid_n = n.value
+        return n.value, np.float32(last.value), bool(yaw.value)
+
+    def lidar_upload_features(self, fmt: LidarFormat, records, dis_b=0.0, n_records=None):
+        """flb_lidar_upload_features (feature_extract_enable: 1) for a Livox or Ouster message; fmt.off_line is the Livox
+        line or the Ouster's u8 ring.  Returns (pl_surf.size(), points.back().curvature after the sort)."""
+        a = np.frombuffer(records, np.uint8) if isinstance(records, (bytes, bytearray)) else records
+        if n_records is None:
+            n_records = a.size // max(fmt.point_step, 1)
+        n, last = C.c_int(), C.c_float()
+        self._ck(self.L.flb_lidar_upload_features(self.h, C.byref(fmt), float(dis_b), _p(a) if a.size else None, int(n_records),
+                                                  C.byref(n), C.byref(last)))
+        self._lid_n = n.value
+        return n.value, np.float32(last.value)
+
+    def lidar_upload_velodyne_features(self, fmt: VelodyneFormat, records, dis_b=0.0, n_records=None):
+        """flb_lidar_upload_velodyne_features (feature_extract_enable: 1).  Returns (pl_surf.size(),
+        points.back().curvature after the sort, whether the times came from the yaw)."""
+        a = np.frombuffer(records, np.uint8) if isinstance(records, (bytes, bytearray)) else records
+        if n_records is None:
+            n_records = a.size // max(fmt.point_step, 1)
+        n, last, yaw = C.c_int(), C.c_float(), C.c_int()
+        self._ck(self.L.flb_lidar_upload_velodyne_features(self.h, C.byref(fmt), float(dis_b), _p(a) if a.size else None,
+                                                           int(n_records), C.byref(n), C.byref(last), C.byref(yaw)))
         self._lid_n = n.value
         return n.value, np.float32(last.value), bool(yaw.value)
 

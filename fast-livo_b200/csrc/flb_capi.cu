@@ -265,6 +265,13 @@ struct flb_handle {
     DevBuf<unsigned> lid_keys, lid_keys_sorted;
     DevBuf<int> lid_idx;                       // flb_lidar_upload_velodyne's yaw route: record indices, then in ring order
     DevBuf<VeloMap> lid_map;                   // its per-record time maps in ring order, scanned in place
+    // flb_lidar_upload_features: the line-major points, their per-point ints (line, jump levels, scans), doubles
+    // (range, dista, intersect), plane_judge results and byte flags (visited, small-plane condition)
+    DevBuf<float4> feat_pts;
+    DevBuf<int> feat_i;
+    DevBuf<double> feat_d;
+    DevBuf<FeatStep> feat_st;
+    DevBuf<unsigned char> feat_u8;
     Staging st_lidar;
     PinBuf pin_lidar;
     // flb_world_cloud: pcl_wait_pub (packed xyz, the caller's order) with its exact bounds; wc_n < 0: no cloud held
@@ -2107,6 +2114,231 @@ int flb_lidar_upload_velodyne(flb_handle* h, const flb_velodyne_format* fmt, con
     }
     VeloYaw yaw{fmt->off_ring, fmt->n_scans};
     const int rc = lidar_upload_core(h, who, f, records, n_records, given ? nullptr : &yaw, n_points, last_offset_ms);
+    if (rc) return rc;
+    if (yaw_times) *yaw_times = given ? 0 : 1;
+    return FLB_OK;
+}
+
+// ---- the feature branches: give_feature's pl_surf ------------------------------------------------------------------
+namespace {
+
+// Preprocess's constants (:9-30): the four thresholds are the constructor's std::cos values, computed here on the host
+// because the device cos may differ from libm in the last ulp.
+FeatConst feat_const(const LidarFmt& f, double dis_b) {
+    FeatConst c;
+    c.blind = f.blind, c.dis_b = dis_b, c.avia = f.kind == kLidarLivox ? 1 : 0;
+    c.jump_up = std::cos(170.0 / 180 * M_PI);
+    c.jump_down = std::cos(8.0 / 180 * M_PI);
+    c.cos160 = std::cos(160.0 / 180 * M_PI);
+    c.smallp_intersect = std::cos(172.5 / 180 * M_PI);
+    return c;
+}
+
+// flb_lidar_upload_features and flb_lidar_upload_velodyne_features from the argument checks on.  f.off_line: the
+// Livox line, the Ouster's u8 ring or the Velodyne's u16 ring.  yaw: Velodyne times from the yaw angle.
+int lidar_features_core(flb_handle* h, const char* who, const LidarFmt& f, double dis_b, const void* records, int n_records,
+                        bool yaw, int* n_points, float* last_offset_ms) {
+    const FeatConst c = feat_const(f, dis_b);
+    const int min_size = f.kind == kLidarLivox ? 6 : f.kind == kLidarVelodyne ? 2 : 1;   // :117, :357; the Ouster: any
+    const int step = f.step;
+    const size_t n = (size_t)n_records, n1 = std::max<size_t>(n, 1), raw_bytes = n * step;
+    const int ns = f.n_scans;
+    int levels = 1;                                      // 2^levels > any chain length (<= the point count)
+    while (levels < 31 && ((size_t)1 << levels) <= n1) ++levels;
+    FLB_CUDA(h, h->lid_raw.reserve(std::max<size_t>(raw_bytes, 4)));
+    FLB_CUDA(h, h->lid_cloud_alt.reserve(n1));
+    FLB_CUDA(h, h->lid_dec.reserve(n1));
+    FLB_CUDA(h, h->lid_sorted.reserve(n1));
+    FLB_CUDA(h, h->lid_keys.reserve(n1));
+    FLB_CUDA(h, h->lid_keys_sorted.reserve(n1));
+    FLB_CUDA(h, h->lid_idx.reserve(2 * n1));
+    FLB_CUDA(h, h->lid_map.reserve(n1));
+    FLB_CUDA(h, h->lid_flags.reserve(3 * n1 + 8));
+    FLB_CUDA(h, h->feat_pts.reserve(n1));
+    FLB_CUDA(h, h->feat_i.reserve((size_t)(levels + 8) * n1 + 3 * (size_t)ns + 1));
+    FLB_CUDA(h, h->feat_d.reserve(3 * n1));
+    FLB_CUDA(h, h->feat_st.reserve(n1));
+    FLB_CUDA(h, h->feat_u8.reserve(2 * n1));
+    FLB_CUDA(h, h->pin_lidar.reserve(64));
+    cudaStream_t cs = h->copy_stream;
+    int* d_take = h->lid_flags.p;
+    int* d_kept = d_take + n1;
+    int* d_pos = d_kept + n1;
+    LidarRecord* d_rec = reinterpret_cast<LidarRecord*>(d_pos + n1);
+    int* d_count = reinterpret_cast<int*>(d_rec + 1);
+    int* d_idx = h->lid_idx.p;
+    int* d_idx_sorted = h->lid_idx.p + n1;
+    // per-point ints: lkey | pv | rs | rs2 | seed | ft | fin | J[levels] | lbeg | lend | lhead
+    int* d_lkey = h->feat_i.p;
+    int* d_pv = d_lkey + n1;
+    int* d_rs = d_pv + n1;
+    int* d_rs2 = d_rs + n1;
+    int* d_seed = d_rs2 + n1;
+    int* d_ft = d_seed + n1;
+    int* d_fin = d_ft + n1;
+    int* d_J = d_fin + n1;
+    int* d_lbeg = d_J + (size_t)levels * n1;
+    int* d_lend = d_lbeg + ns;
+    int* d_lhead = d_lend + ns;
+    double* d_rng = h->feat_d.p;
+    double* d_dista = d_rng + n1;
+    double* d_isect = d_dista + n1;
+    unsigned char* d_vis = h->feat_u8.p;
+    unsigned char* d_small = d_vis + n1;
+    LidarRecord rec{};
+    if (n_records > 0) {
+        if (is_pinned(records)) {
+            FLB_CUDA(h, cudaMemcpyAsync(h->lid_raw.p, records, raw_bytes, cudaMemcpyHostToDevice, cs));
+        } else {
+            void* stv = nullptr;
+            FLB_CUDA(h, h->st_lidar.acquire(raw_bytes, &stv));
+            std::memcpy(stv, records, raw_bytes);
+            FLB_CUDA(h, cudaMemcpyAsync(h->lid_raw.p, stv, raw_bytes, cudaMemcpyHostToDevice, cs));
+            FLB_CUDA(h, h->st_lidar.mark(cs));
+        }
+        { int rcq = vio_copy_begin(h, h->lid_slot); if (rcq) return rcq; }
+        const int g = (n_records + 255) / 256;
+        size_t t1 = 0, t2 = 0, t3 = 0, t4 = 0, t5 = 0;
+        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t1, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted, n_records,
+                                                    0, 8, cs));
+        FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t2, d_take, d_pos, n_records, cs));
+        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p, h->lid_sorted.p,
+                                                    n_records, 0, 32, cs));
+        FLB_CUDA(h, cub::DeviceScan::InclusiveScan(nullptr, t4, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
+        FLB_CUDA(h, cub::DeviceScan::InclusiveScan(nullptr, t5, d_seed, d_rs, FeatMaxOp(), n_records, cs));
+        size_t t6 = 0;
+        FLB_CUDA(h, cub::DeviceScan::ExclusiveScan(nullptr, t6, d_seed, d_pv, FeatMaxOp(), -1, n_records, cs));
+        FLB_CUDA(h, h->lid_cub.reserve(std::max(std::max(std::max(t1, t2), std::max(t3, t4)), std::max(t5, t6))));
+        // the records into line order
+        k_feat_keys<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, h->lid_keys.p, d_idx);
+        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t1, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted,
+                                                    n_records, 0, 8, cs));
+        if (yaw) {
+            k_velo_maps<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, ns, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p);
+            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t4, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
+            h->launches += 2;
+        }
+        k_feat_take<<<g, 256, 0, cs>>>(h->lid_keys_sorted.p, n_records, ns, yaw ? 1 : 0, d_take);
+        FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t2, d_take, d_pos, n_records, cs));
+        k_feat_gather<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, yaw ? 1 : 0, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p,
+                                         d_take, d_pos, h->feat_pts.p, d_lkey, d_count);
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches += 6;
+        int M = 0;
+        FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_count, sizeof(int), cudaMemcpyDeviceToHost, cs));
+        FLB_CUDA(h, cudaStreamSynchronize(cs));
+        std::memcpy(&M, h->pin_lidar.p, sizeof(int));
+        FLB_CUDA(h, cudaMemsetAsync(d_rec, 0, sizeof(LidarRecord), cs));
+        if (M > 0) {
+            const int gm = (M + 255) / 256;
+            int lv = 1;
+            while (lv < levels && (1 << lv) <= M) ++lv;
+            FLB_CUDA(h, cudaMemsetAsync(d_lbeg, 0, 2 * ns * sizeof(int), cs));
+            FLB_CUDA(h, cudaMemsetAsync(d_lhead, 0x7f, ns * sizeof(int), cs));      // 0x7f7f7f7f: no head
+            k_feat_range<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_lkey, M, c.avia, c.blind, d_rng, d_dista, d_lbeg, d_lend, d_lhead);
+            k_feat_steps<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_rng, d_dista, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, c,
+                                             h->feat_st.p, d_J, d_vis);
+            for (int l = 0; l + 1 < lv; ++l) k_feat_jump<<<gm, 256, 0, cs>>>(d_J + (size_t)l * n1, M, d_J + (size_t)(l + 1) * n1);
+            for (int l = lv - 1; l >= 0; --l) k_feat_mark<<<gm, 256, 0, cs>>>(d_J + (size_t)l * n1, M, d_vis);
+            k_feat_vis_index<<<gm, 256, 0, cs>>>(d_vis, M, d_seed);
+            FLB_CUDA(h, cub::DeviceScan::ExclusiveScan(h->lid_cub.p, t6, d_seed, d_pv, FeatMaxOp(), -1, M, cs));
+            k_feat_types<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_rng, d_dista, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, c,
+                                             h->feat_st.p, d_vis, d_pv, d_ft, d_isect);
+            k_feat_small<<<gm, 256, 0, cs>>>(d_rng, d_dista, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, c, d_ft, d_isect, d_small);
+            k_feat_small_seed<<<gm, 256, 0, cs>>>(d_small, M, d_seed);
+            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t5, d_seed, d_rs, FeatMaxOp(), M, cs));
+            k_feat_final<<<gm, 256, 0, cs>>>(d_ft, d_small, d_rs, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, d_fin, d_seed);
+            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t5, d_seed, d_rs2, FeatMaxOp(), M, cs));
+            k_feat_emit<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_fin, d_rs2, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, f.filter_num,
+                                            h->lid_dec.p, d_kept);
+            // flb_lidar_upload's compaction and time sort
+            FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t2, d_kept, d_pos, M, cs));
+            k_lidar_scatter<<<gm, 256, 0, cs>>>(h->lid_dec.p, d_kept, d_pos, M, h->lid_cloud_alt.p, h->lid_keys.p, d_rec);
+            k_lidar_order<<<gm, 256, 0, cs>>>(h->lid_cloud_alt.p, h->lid_keys.p, M, d_rec);
+            FLB_CUDA(h, cudaGetLastError());
+            h->launches += 15 + 2 * lv;
+        }
+        FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
+        FLB_CUDA(h, cudaStreamSynchronize(cs));
+        std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
+        if (rec.bad) return fail(h, FLB_ERR_INVALID, "%s: a point of pl_surf or its time is not finite", who);
+        if (rec.unsorted) {
+            // stable: equal times keep pl_surf's line-major order
+            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p,
+                                                        h->lid_sorted.p, rec.n_kept, 0, 32, cs));
+            FLB_CUDA(h, cudaMemcpyAsync(h->lid_cloud_alt.p, h->lid_sorted.p, (size_t)rec.n_kept * sizeof(float4), cudaMemcpyDeviceToDevice, cs));
+            k_lidar_last<<<1, 1, 0, cs>>>(h->lid_cloud_alt.p, d_rec);
+            FLB_CUDA(h, cudaGetLastError());
+            h->launches += 3;
+            FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
+            FLB_CUDA(h, cudaStreamSynchronize(cs));
+            std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
+        }
+    } else {
+        int rcq = vio_copy_begin(h, h->lid_slot);
+        if (rcq) return rcq;
+    }
+    std::swap(h->lid_cloud, h->lid_cloud_alt);
+    h->lid_slot.slot ^= 1;
+    h->lid_n = rec.n_kept;
+    h->lid_cursor = 0;
+    if (n_points) *n_points = rec.n_kept;
+    if (last_offset_ms) *last_offset_ms = rec.n_kept > 0 ? rec.last : 0.f;
+    return FLB_OK;
+}
+
+}  // namespace
+
+int flb_lidar_upload_features(flb_handle* h, const flb_lidar_format* fmt, double dis_b, const void* records, int n_records,
+                              int* n_points, float* last_offset_ms) {
+    FLB_CHECK_H(h);
+    const char* who = "flb_lidar_upload_features";
+    if (n_records < 0 || !fmt || (n_records > 0 && !records) || !std::isfinite(dis_b))
+        return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
+    if (fmt->kind == kLidarVelodyne || fmt->kind == kLidarXt32)
+        return fail(h, FLB_ERR_INVALID, "%s: kind %d: a Velodyne cloud goes to flb_lidar_upload_velodyne_features; the XT32 "
+                    "has no feature branch (src/preprocess.cpp:432-464), so flb_lidar_upload serves it", who, fmt->kind);
+    if (fmt->kind != kLidarLivox && fmt->kind != kLidarOuster) return fail(h, FLB_ERR_INVALID, "%s: unknown kind %d", who, fmt->kind);
+    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || fmt->n_scans > 128 || !std::isfinite(fmt->blind))
+        return fail(h, FLB_ERR_INVALID, "%s: point_filter_num %d, n_scans %d (1..128: pl_buff[128]), blind %g", who,
+                    fmt->point_filter_num, fmt->n_scans, fmt->blind);
+    const int step = fmt->point_step;
+    const bool livox = fmt->kind == kLidarLivox;
+    if (step < 1 || !lidar_field_ok(fmt->off_x, 4, step) || !lidar_field_ok(fmt->off_y, 4, step) || !lidar_field_ok(fmt->off_z, 4, step) ||
+        !lidar_field_ok(fmt->off_time, 4, step) || !lidar_field_ok(fmt->off_line, 1, step) ||
+        (livox && !lidar_field_ok(fmt->off_tag, 1, step)))
+        return fail(h, FLB_ERR_INVALID, "%s: a field does not fit in point_step %d or is not aligned to its type", who, step);
+    LidarFmt f{};
+    f.kind = fmt->kind, f.step = step, f.off_x = fmt->off_x, f.off_y = fmt->off_y, f.off_z = fmt->off_z, f.off_time = fmt->off_time;
+    f.off_tag = livox ? fmt->off_tag : 0, f.off_line = fmt->off_line;
+    f.n_scans = fmt->n_scans, f.filter_num = fmt->point_filter_num, f.blind = fmt->blind;
+    return lidar_features_core(h, who, f, dis_b, records, n_records, false, n_points, last_offset_ms);
+}
+
+int flb_lidar_upload_velodyne_features(flb_handle* h, const flb_velodyne_format* fmt, double dis_b, const void* records,
+                                       int n_records, int* n_points, float* last_offset_ms, int* yaw_times) {
+    FLB_CHECK_H(h);
+    const char* who = "flb_lidar_upload_velodyne_features";
+    if (n_records < 0 || !fmt || (n_records > 0 && !records) || !std::isfinite(dis_b))
+        return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
+    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || fmt->n_scans > 128 || !std::isfinite(fmt->blind))
+        return fail(h, FLB_ERR_INVALID, "%s: point_filter_num %d, n_scans %d (1..128: pl_buff[128]), blind %g", who,
+                    fmt->point_filter_num, fmt->n_scans, fmt->blind);
+    const int step = fmt->point_step;
+    if (step < 1 || !velo_field_ok(fmt->off_x, 4, step) || !velo_field_ok(fmt->off_y, 4, step) || !velo_field_ok(fmt->off_z, 4, step) ||
+        !velo_field_ok(fmt->off_ring, 2, step) || (fmt->off_time != -1 && !velo_field_ok(fmt->off_time, 4, step)))
+        return fail(h, FLB_ERR_INVALID, "%s: a field does not fit in point_step %d", who, step);
+    LidarFmt f{};
+    f.kind = kLidarVelodyne, f.step = step, f.off_x = fmt->off_x, f.off_y = fmt->off_y, f.off_z = fmt->off_z;
+    f.off_time = fmt->off_time >= 0 ? fmt->off_time : 0, f.off_line = fmt->off_ring;
+    f.n_scans = fmt->n_scans, f.filter_num = fmt->point_filter_num, f.blind = fmt->blind;
+    bool given = n_records == 0;                                                  // given_offset_time (:279)
+    if (n_records > 0 && fmt->off_time >= 0) {
+        float t_last;
+        std::memcpy(&t_last, static_cast<const unsigned char*>(records) + (size_t)(n_records - 1) * step + fmt->off_time, sizeof(t_last));
+        given = t_last > 0;
+    }
+    const int rc = lidar_features_core(h, who, f, dis_b, records, n_records, !given, n_points, last_offset_ms);
     if (rc) return rc;
     if (yaw_times) *yaw_times = given ? 0 : 1;
     return FLB_OK;

@@ -1739,4 +1739,355 @@ FLB_HD VeloMap velo_step(double yaw, double yaw_fp) {
     return m;
 }
 
+// ------------------------------------------------------------------ LiDAR surface features (give_feature)
+// The feature branches of avia_handler (:94-135), oust64_handler (:174-227) and velodyne_handler (:299-373), with
+// give_feature (:466-775), plane_judge (:786-898) and edge_jump_judge (:900-936), one point at a time
+// (flb_lidar_upload_features).  The points sit line-major in one array; a line is the segment [b, b + m) of it and the
+// functions below take `pl`, `rng` and `dista` already offset to the line's first point, with local indices.
+enum { kFtNor = 0, kFtPossPlane = 1, kFtRealPlane = 2, kFtEdgeJump = 3, kFtEdgePlane = 4, kFtWire = 5 };   // Feature
+enum { kNrNor = 0, kNrZero = 1, kNr180 = 2, kNrInf = 3, kNrBlind = 4 };                                  // E_jump
+enum { kStepNone = -1, kStepNonPlane = 0, kStepPlane = 1, kStepBlind = 2, kStepSkip = 3 };   // plane_judge's result; kStepSkip: a blind i (:495)
+constexpr int kFeatGroup = 8;          // group_size (:11)
+
+// Preprocess's constants (:9-30).  The four cosines are the constructor's std::cos values, computed on the host.
+struct FeatConst {
+    double blind, dis_b;
+    double jump_up, jump_down, cos160, smallp_intersect;
+    int avia;                          // lidar_type == AVIA: plane_judge's median test and range without sqrt
+};
+
+FLB_HD unsigned long long feat_d2u(double d) {
+#if defined(__CUDA_ARCH__)
+    return (unsigned long long)__double_as_longlong(d);
+#else
+    unsigned long long u;
+    memcpy(&u, &d, sizeof(u));
+    return u;
+#endif
+}
+FLB_HD double feat_u2d(unsigned long long u) {
+#if defined(__CUDA_ARCH__)
+    return __longlong_as_double((long long)u);
+#else
+    double d;
+    memcpy(&d, &u, sizeof(d));
+    return d;
+#endif
+}
+FLB_HD bool feat_isnan(double d) { return d != d; }
+
+// Livox, :94-111: the line of record i, or n_scans when the record is not kept.  abs is the float overload on the raw
+// previous record; x*x + y*y is compared with blind itself.  line == N_SCANS passes the filter but lands in a buffer
+// that is never processed (:114), so it is dropped too.
+FLB_HD int feat_livox_line(const unsigned char* r, int i, const LidarFmt& f) {
+    if (i < 1) return f.n_scans;
+    const LidarPoint q = lidar_decode(r, f), p = lidar_decode(r - f.step, f);
+    const int line = r[f.off_line];
+    if ((double)fabsf(q.x - p.x) < 1e-8 || (double)fabsf(q.y - p.y) < 1e-8 || (double)fabsf(q.z - p.z) < 1e-8 ||
+        (double)(q.x * q.x + q.y * q.y) < f.blind || line > f.n_scans || (r[f.off_tag] & 0x30u) != 0x10u)
+        return f.n_scans;
+    return line;
+}
+// Ouster, :182-205: the 3-D float sum widened to double against blind * blind; the u8 ring (off_line) below N_SCANS.
+FLB_HD int feat_ouster_line(const unsigned char* r, const LidarFmt& f) {
+    const LidarPoint q = lidar_decode(r, f);
+    if ((double)(q.x * q.x + q.y * q.y + q.z * q.z) < f.blind * f.blind) return f.n_scans;
+    const int ring = r[f.off_line];
+    return ring < f.n_scans ? ring : f.n_scans;
+}
+
+// types[i].range (:126, :218, :364): Livox the unsquared 2-D sum, the others its float sqrt.
+FLB_HD double feat_range(const LidarPoint& p, int avia) {
+    const float s = p.x * p.x + p.y * p.y;
+    return avia ? (double)s : (double)sqrtf(s);
+}
+// types[i].dista (:127-130): float differences into the double members vx, vy, vz.  The line's last point has none
+// (types.resize leaves it unwritten); the project defines it as 0.0.
+FLB_HD double feat_dista(const LidarPoint& a, const LidarPoint& b) {
+    const double vx = a.x - b.x, vy = a.y - b.y, vz = a.z - b.z;
+    return vx * vx + vy * vy + vz * vz;
+}
+
+// The value at position `pos` of disarr[0, n) after plane_judge's exchange sort (:855-867).  A NaN never moves there
+// (both comparisons with it are false), and the other values end up sorted descending in the remaining positions, as
+// the same exchange sort of them alone would leave them.  So a NaN position reads NaN, and any other reads the r-th
+// largest non-NaN value, r = the non-NaN positions before it.  Dista values are >= +0.0 or NaN, so their bit patterns
+// order as the values; the r-th largest is found bit by bit.
+// The largest, the smallest and the second smallest (the positions plane_judge reads in a group without NaN) take one
+// pass; any other rank is found bit by bit.
+FLB_HD double feat_sorted_at(const double* d, int n, int pos) {
+    if (feat_isnan(d[pos])) return d[pos];
+    int r = 0, cnt = 0;
+    for (int j = 0; j < n; ++j) {
+        const int ok = !feat_isnan(d[j]);
+        r += j < pos ? ok : 0;
+        cnt += ok;
+    }
+    if (r == 0 || r >= cnt - 2) {
+        unsigned long long hi = 0ull, lo1 = ~0ull, lo2 = ~0ull;     // the max; the two smallest, with multiplicity
+        for (int j = 0; j < n; ++j) {
+            if (feat_isnan(d[j])) continue;
+            const unsigned long long u = feat_d2u(d[j]);
+            hi = u > hi ? u : hi;
+            if (u < lo1) lo2 = lo1, lo1 = u;
+            else if (u < lo2) lo2 = u;
+        }
+        return feat_u2d(r == 0 ? hi : r == cnt - 1 ? lo1 : lo2);
+    }
+    unsigned long long pre = 0ull;
+    for (int bit = 62; bit >= 0; --bit) {
+        const unsigned long long cand = pre | (1ull << bit);
+        int cnt = 0;
+        for (int j = 0; j < n; ++j) cnt += (!feat_isnan(d[j]) && feat_d2u(d[j]) >= cand) ? 1 : 0;
+        if (cnt > r) pre = cand;
+    }
+    return feat_u2d(pre);
+}
+
+struct FeatStep {
+    int type;            // kStepNonPlane, kStepPlane, kStepBlind
+    int nex;             // i_nex on return; == m when a plane group reaches the line's last point
+    float vx, vy, vz;    // the last (vx, vy, vz) of :815-817: exact float differences
+};
+
+// plane_judge (:786-898) for a point i with i + group_size < m (the caller's loop bound, :483).  The first loop pushes
+// group_size values; the second runs at least once, so vx, vy, vz and two_dis are always this call's own.
+FLB_HD FeatStep feat_plane_judge(const LidarPoint* pl, const double* rng, const double* dista, int m, int i, const FeatConst& c) {
+    FeatStep s;
+    s.type = kStepNonPlane, s.vx = s.vy = s.vz = 0.f;
+    double group_dis = 0.1 * rng[i] + c.dis_b;                                    // disA = 0.1 (:13)
+    group_dis = group_dis * group_dis;
+    int nex;
+    for (nex = i; nex < i + kFeatGroup; nex++)
+        if (rng[nex] < c.blind) { s.type = kStepBlind, s.nex = nex; return s; }
+    double vx = 0.0, vy = 0.0, vz = 0.0, two_dis = 0.0;
+    for (;;) {
+        if (i >= m || nex >= m) break;
+        if (rng[nex] < c.blind) { s.type = kStepBlind, s.nex = nex; return s; }
+        vx = pl[nex].x - pl[i].x;
+        vy = pl[nex].y - pl[i].y;
+        vz = pl[nex].z - pl[i].z;
+        two_dis = vx * vx + vy * vy + vz * vz;
+        if (two_dis >= group_dis) break;
+        nex++;
+    }
+    s.nex = nex;
+    double leng_wid = 0.0;
+    for (int j = i + 1; j < nex; j++) {
+        const double v1x = pl[j].x - pl[i].x, v1y = pl[j].y - pl[i].y, v1z = pl[j].z - pl[i].z;
+        const double v2x = v1y * vz - vy * v1z, v2y = v1z * vx - v1x * vz, v2z = v1x * vy - vx * v1y;
+        const double lw = v2x * v2x + v2y * v2y + v2z * v2z;
+        if (lw > leng_wid) leng_wid = lw;
+    }
+    const int n = nex - i;                                                        // disarr = dista[i, nex)
+    if ((two_dis * two_dis / leng_wid) < 225.0) return s;                         // p2l_ratio (:14)
+    const double dlow = feat_sorted_at(dista + i, n, n - 2);
+    if (dlow < 1e-16) return s;
+    const double d0 = feat_sorted_at(dista + i, n, 0);
+    if (c.avia) {
+        const double dmid = feat_sorted_at(dista + i, n, n / 2);
+        const double dismax_mid = d0 / dmid, dismid_min = dmid / dlow;
+        if (dismax_mid >= 6.25 || dismid_min >= 6.25) return s;                    // limit_maxmid, limit_midmin
+    } else {
+        if (d0 / dlow >= 3.24) return s;                                           // limit_maxmin
+    }
+    s.type = kStepPlane;
+    s.vx = (float)vx, s.vy = (float)vy, s.vz = (float)vz;
+    return s;
+}
+
+// Eigen's Vector3d dot, norm and normalize as DESIGN §2 defines them: left to right, no FMA.
+FLB_HD double feat_dot(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+FLB_HD void feat_normalize(float vx, float vy, float vz, double* v) {
+    v[0] = vx, v[1] = vy, v[2] = vz;
+    const double z = feat_dot(v, v);
+    if (z > 0.0) {
+        const double s = sqrt(z);
+        v[0] /= s, v[1] /= s, v[2] /= s;
+    }
+}
+
+// The ftype of point j after the plane loop (:493-590), given the visited steps: j's own step when j is visited, and
+// p, the last visited point before j (-1: none).  A visited plane step writes [i, i_nex] (:506-516); consecutive plane
+// steps share one endpoint, and the later step's write wins there.  last_state == 1 exactly when p is a plane step: a
+// plane's i_nex is never within blind, so a blind step never follows one.
+FLB_HD int feat_plane_ftype(int j, bool vis_j, const FeatStep& sj, int p, const FeatStep& sp) {
+    const bool p_plane = p >= 0 && sp.type == kStepPlane;
+    if (vis_j && sj.type == kStepPlane) {
+        if (p_plane) {
+            double last_direct[3], curr_direct[3];
+            feat_normalize(sp.vx, sp.vy, sp.vz, last_direct);
+            feat_normalize(sj.vx, sj.vy, sj.vz, curr_direct);
+            if (sqrt(feat_dot(last_direct, last_direct)) > 0.1) {                 // :519
+                const double mod = feat_dot(last_direct, curr_direct);
+                return (mod > -0.707 && mod < 0.707) ? kFtEdgePlane : kFtRealPlane;
+            }
+        }
+        return kFtPossPlane;
+    }
+    if (p_plane && sp.nex >= j) return j == sp.nex ? kFtPossPlane : kFtRealPlane;
+    return kFtNor;
+}
+
+// edge_jump_judge (:900-936)
+FLB_HD bool feat_edge_jump_judge(const double* rng, const double* dista, int i, int nor_dir, const FeatConst& c) {
+    if (nor_dir == 0) {
+        if (rng[i - 1] < c.blind || rng[i - 2] < c.blind) return false;
+    } else {
+        if (rng[i + 1] < c.blind || rng[i + 2] < c.blind) return false;
+    }
+    double d1 = dista[i + nor_dir - 1];
+    double d2 = dista[i + 3 * nor_dir - 2];
+    if (d1 < d2) {
+        const double d = d1;
+        d1 = d2, d2 = d;
+    }
+    d1 = sqrt(d1), d2 = sqrt(d2);
+    if (d1 > 2.0 * d2 || (d1 - d2) > 0.1) return false;                        // edgea, edgeb
+    return true;
+}
+
+struct FeatEdge {
+    int ftype;
+    double intersect;    // types[i].intersect: 2 (the constructor's) unless both neighbours were measured
+};
+
+// The edge pass for point i (:592-686); ftype is i's type after the plane loop.  Each point reads only its own type.
+// When a neighbour is within blind its vecs[] entry is not computed and the reference's intersect reads stale stack
+// memory; intersect is then used by neither this pass nor the small-plane pass (which skips a blind neighbour), so it
+// is recorded as 2.
+FLB_HD FeatEdge feat_edge(const LidarPoint* pl, const double* rng, const double* dista, int m, int head, int i, int ftype,
+                          const FeatConst& c) {
+    FeatEdge e;
+    e.ftype = ftype, e.intersect = 2.0;
+    const int plsize2 = m > 3 ? m - 3 : 0;
+    if (i < head + 3 || i >= plsize2) return e;
+    if (rng[i] < c.blind || ftype >= kFtRealPlane) return e;
+    if (dista[i - 1] < 1e-16 || dista[i] < 1e-16) return e;
+    const double vec_a[3] = {(double)pl[i].x, (double)pl[i].y, (double)pl[i].z};
+    double vecs[2][3];
+    int edj[2] = {kNrNor, kNrNor};
+    bool both = true;
+    for (int j = 0; j < 2; j++) {
+        const int k = j == 1 ? i + 1 : i - 1;
+        if (rng[k] < c.blind) {
+            edj[j] = rng[i] > 10.0 ? kNrInf : kNrBlind;                             // inf_bound (:9)
+            both = false;
+            continue;
+        }
+        vecs[j][0] = (double)pl[k].x - vec_a[0];
+        vecs[j][1] = (double)pl[k].y - vec_a[1];
+        vecs[j][2] = (double)pl[k].z - vec_a[2];
+        const double angle = feat_dot(vec_a, vecs[j]) / sqrt(feat_dot(vec_a, vec_a)) / sqrt(feat_dot(vecs[j], vecs[j]));
+        if (angle < c.jump_up) edj[j] = kNr180;
+        else if (angle > c.jump_down) edj[j] = kNrZero;
+    }
+    if (both) e.intersect = feat_dot(vecs[0], vecs[1]) / sqrt(feat_dot(vecs[0], vecs[0])) / sqrt(feat_dot(vecs[1], vecs[1]));
+    const double di = dista[i], dp = dista[i - 1];
+    if (edj[0] == kNrNor && edj[1] == kNrZero && di > 0.0225 && di > 4 * dp) {
+        if (e.intersect > c.cos160 && feat_edge_jump_judge(rng, dista, i, 0, c)) e.ftype = kFtEdgeJump;
+    } else if (edj[0] == kNrZero && edj[1] == kNrNor && dp > 0.0225 && dp > 4 * di) {
+        if (e.intersect > c.cos160 && feat_edge_jump_judge(rng, dista, i, 1, c)) e.ftype = kFtEdgeJump;
+    } else if (edj[0] == kNrNor && edj[1] == kNrInf) {
+        if (feat_edge_jump_judge(rng, dista, i, 0, c)) e.ftype = kFtEdgeJump;
+    } else if (edj[0] == kNrInf && edj[1] == kNrNor) {
+        if (feat_edge_jump_judge(rng, dista, i, 1, c)) e.ftype = kFtEdgeJump;
+    } else if (edj[0] > kNrNor && edj[1] > kNrNor) {
+        if (e.ftype == kFtNor) e.ftype = kFtWire;
+    }
+    return e;
+}
+
+// The small-plane pass (:688-726): iteration i would fire on the types the edge pass left (ftype, intersect).
+// Iteration i-1 changes ftype[i] only when it fires, so fire(i) = small_cond(i) && !fire(i-1): along a run of
+// consecutive conditions the firing alternates from the run's first point.
+FLB_HD bool feat_small_cond(const double* rng, const double* dista, int m, int head, int i, int ftype, double intersect,
+                            const FeatConst& c) {
+    if (i < head + 1 || i >= m - 1) return false;
+    if (rng[i] < c.blind || rng[i - 1] < c.blind || rng[i + 1] < c.blind) return false;
+    if (dista[i - 1] < 1e-8 || dista[i] < 1e-8) return false;
+    if (ftype != kFtNor) return false;
+    const double ratio = dista[i - 1] > dista[i] ? dista[i - 1] / dista[i] : dista[i] / dista[i - 1];
+    return intersect < c.smallp_intersect && ratio < 1.2;                          // smallp_ratio (:24)
+}
+FLB_HD bool feat_is_surf(int ftype) { return ftype == kFtPossPlane || ftype == kFtRealPlane; }
+
+// ---- the parallel formulation: one function per kernel, over the global line-major index q ----------------------
+// lbeg / lend: each line's segment (0 / 0 when empty); lhead: the first point not within blind (INT_MAX: none).
+struct FeatLine { int b, m, head; };   // head == m: the line yields nothing (skipped by its size, or all within blind)
+FLB_HD FeatLine feat_line(const int* lbeg, const int* lend, const int* lhead, int k, int min_size) {
+    FeatLine L;
+    L.b = lbeg[k], L.m = lend[k] - lbeg[k];
+    L.head = (L.m < min_size || lhead[k] >= lend[k]) ? L.m : lhead[k] - L.b;
+    return L;
+}
+FLB_HD int feat_plsize2(const FeatLine& L) { return L.m > kFeatGroup ? L.m - kFeatGroup : 0; }
+
+// The step of the plane loop (:493-590) that would start at q.  A step depends on its own i alone, never on the walk
+// that reaches it.
+FLB_HD FeatStep feat_step_at(const LidarPoint* P, const double* rng, const double* dista, const FeatLine& L, int q,
+                             const FeatConst& c) {
+    const int j = q - L.b;
+    FeatStep s;
+    s.type = kStepNone, s.nex = j, s.vx = s.vy = s.vz = 0.f;
+    if (j < L.head || j >= feat_plsize2(L)) return s;
+    if (rng[q] < c.blind) {
+        s.type = kStepSkip;
+        return s;
+    }
+    return feat_plane_judge(P + L.b, rng + L.b, dista + L.b, L.m, j, c);
+}
+// The next point the loop visits after the step s at q: i_nex for a plane, i_nex + 1 otherwise, i + 1 for a blind i;
+// -1 for no step, or once that leaves the loop's range.
+FLB_HD int feat_succ(const FeatStep& s, const FeatLine& L, int q) {
+    if (s.type == kStepNone) return -1;
+    const int nx = s.type == kStepSkip ? q - L.b + 1 : s.type == kStepPlane ? s.nex : s.nex + 1;
+    return nx < feat_plsize2(L) ? L.b + nx : -1;
+}
+
+// ftype after the plane loop and the edge pass for point q.  vis: q is visited; p: the last visited point before q
+// (global, -1 or outside the line: none).
+FLB_HD FeatEdge feat_types_at(const LidarPoint* P, const double* rng, const double* dista, const FeatLine& L, int q, bool vis,
+                              const FeatStep& sq, int p, const FeatStep& sp, const FeatConst& c) {
+    const int j = q - L.b;
+    const int pj = p >= L.b ? p - L.b : -1;
+    const int ft = feat_plane_ftype(j, vis, sq, pj, sp);
+    return feat_edge(P + L.b, rng + L.b, dista + L.b, L.m, L.head, j, ft, c);
+}
+
+// The type after the small-plane pass: fire(x) = small(x) && x is an even distance from its run's start (rs[x]).
+FLB_HD bool feat_fire(const unsigned char* small, const int* rs, int M, int x) {
+    return x >= 0 && x < M && small[x] && ((x - rs[x]) & 1) == 0;
+}
+FLB_HD int feat_final_at(const int* ft_edge, const unsigned char* small, const int* rs, int M, int q) {
+    const int ft = ft_edge[q];
+    if (ft == kFtNor && (feat_fire(small, rs, M, q - 1) || feat_fire(small, rs, M, q) || feat_fire(small, rs, M, q + 1)))
+        return kFtRealPlane;
+    return ft;
+}
+
+// The surface output (:728-774) at q: runs of Poss_Plane / Real_Plane from head on, cut into chunks of filter_num from
+// the run's start (rs2 = that start).  A full chunk emits its last point; a partial one the float mean of its points,
+// in index order, at the non-surface point that closes it; a partial one at the line's end is dropped.
+FLB_HD bool feat_emit_at(const LidarPoint* P, const int* ft_final, const int* rs2, const FeatLine& L, int q, int filter_num,
+                         LidarPoint* out) {
+    const int j = q - L.b;
+    if (j < L.head || j >= L.m) return false;
+    if (feat_is_surf(ft_final[q])) {
+        if ((q - rs2[q]) % filter_num != filter_num - 1) return false;
+        *out = P[q];
+        return true;
+    }
+    if (j == L.head || !feat_is_surf(ft_final[q - 1])) return false;
+    const int len = q - rs2[q - 1], r = len % filter_num;
+    if (r == 0) return false;
+    LidarPoint ap;
+    ap.x = ap.y = ap.z = ap.t = 0.f;
+    for (int k = q - r; k < q; k++) ap.x += P[k].x, ap.y += P[k].y, ap.z += P[k].z, ap.t += P[k].t;
+    const float d = (float)(unsigned)r;
+    ap.x /= d, ap.y /= d, ap.z /= d, ap.t /= d;
+    *out = ap;
+    return true;
+}
+
 }  // namespace flb

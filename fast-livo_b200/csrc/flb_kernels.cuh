@@ -3685,4 +3685,177 @@ __global__ void __launch_bounds__(256) k_velo_flags(const unsigned char* __restr
     kept[i] = (k < (unsigned)n_rings && !head && lidar_pc2_keep(q, i, f)) ? 1 : 0;
 }
 
+// ---- LiDAR surface features (flb_lidar_upload_features / flb_lidar_upload_velodyne_features) -----------------------
+// give_feature (src/preprocess.cpp:466-775) over every line at once.  The kept records go line-major into one array
+// (a stable radix sort by line); lines are segments of it.  Every step of give_feature is then a per-point kernel: one
+// plane_judge per candidate, the plane loop's visited chain by pointer doubling over the successor links, the plane and
+// edge types, the small-plane firing from a max-scan of run starts, and the chunked surface output from a max-scan of
+// surface-run starts.  The per-point math is flb_device.cuh's feat_*; a thread owns one record or one point.
+
+struct FeatMaxOp {
+    __device__ __forceinline__ int operator()(int a, int b) const { return a > b ? a : b; }
+};
+
+// The kind's per-record filter: key[i] = the record's line, or n_scans when it is dropped; idx[i] = i.
+__global__ void __launch_bounds__(256) k_feat_keys(const unsigned char* __restrict__ raw, int n, LidarFmt f,
+                                                   unsigned* __restrict__ key, int* __restrict__ idx) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned char* r = raw + (size_t)i * f.step;
+    int k;
+    if (f.kind == kLidarLivox) k = feat_livox_line(r, i, f);
+    else if (f.kind == kLidarOuster) k = feat_ouster_line(r, f);
+    else k = min((int)lidar_ld16(r + f.off_line), f.n_scans);                   // Velodyne: the ring (:313-314)
+    key[i] = (unsigned)k;
+    idx[i] = i;
+}
+
+// take[p] = the record at line-order position p enters its line: a kept line, and on the yaw route not the ring's
+// first record (:324-333).
+__global__ void __launch_bounds__(256) k_feat_take(const unsigned* __restrict__ key, int n, int n_scans, int yaw,
+                                                   int* __restrict__ take) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    const bool head = p == 0 || key[p - 1] != key[p];
+    take[p] = ((int)key[p] < n_scans && !(yaw && head)) ? 1 : 0;
+}
+
+// The line array: P[pos] = x, y, z and the time (the handler's, or the scanned yaw map's), lkey[pos] = the line;
+// *count = its size.
+__global__ void __launch_bounds__(256) k_feat_gather(const unsigned char* __restrict__ raw, int n, LidarFmt f, int yaw,
+                                                     const unsigned* __restrict__ key, const int* __restrict__ idx,
+                                                     const VeloMap* __restrict__ scanned, const int* __restrict__ take,
+                                                     const int* __restrict__ pos, float4* __restrict__ P, int* __restrict__ lkey,
+                                                     int* __restrict__ count) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    if (p == n - 1) *count = pos[p] + take[p];
+    if (!take[p]) return;
+    LidarPoint q = lidar_decode(raw + (size_t)idx[p] * f.step, f);
+    if (yaw) q.t = velo_apply(scanned[p], 0.f);
+    P[pos[p]] = make_float4(q.x, q.y, q.z, q.t);
+    lkey[pos[p]] = (int)key[p];
+}
+
+// range and dista per point (the line's last dista is 0.0), each line's segment, and its head: the first point not
+// within blind (lbeg / lend zeroed, lhead preset to 0x7f7f7f7f before the launch).
+__global__ void __launch_bounds__(256) k_feat_range(const float4* __restrict__ P, const int* __restrict__ lkey, int M, int avia,
+                                                    double blind, double* __restrict__ rng, double* __restrict__ dista,
+                                                    int* __restrict__ lbeg, int* __restrict__ lend, int* __restrict__ lhead) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= M) return;
+    const LidarPoint* pl = reinterpret_cast<const LidarPoint*>(P);
+    const int k = lkey[q];
+    const bool last = q + 1 == M || lkey[q + 1] != k;
+    const double r = feat_range(pl[q], avia);
+    rng[q] = r;
+    dista[q] = last ? 0.0 : feat_dista(pl[q], pl[q + 1]);
+    if (q == 0 || lkey[q - 1] != k) lbeg[k] = q;
+    if (last) lend[k] = q + 1;
+    if (!(r < blind)) atomicMin(&lhead[k], q);
+}
+
+// One plane_judge per candidate: st[q], the successor link J0[q] (-1: the loop ends), and the chain's start marked.
+__global__ void __launch_bounds__(256) k_feat_steps(const float4* __restrict__ P, const double* __restrict__ rng,
+                                                    const double* __restrict__ dista, const int* __restrict__ lkey,
+                                                    const int* __restrict__ lbeg, const int* __restrict__ lend,
+                                                    const int* __restrict__ lhead, int M, int min_size, FeatConst c,
+                                                    FeatStep* __restrict__ st, int* __restrict__ J0, unsigned char* __restrict__ vis) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= M) return;
+    const FeatLine L = feat_line(lbeg, lend, lhead, lkey[q], min_size);
+    const FeatStep s = feat_step_at(reinterpret_cast<const LidarPoint*>(P), rng, dista, L, q, c);
+    st[q] = s;
+    J0[q] = feat_succ(s, L, q);
+    vis[q] = (q - L.b == L.head && L.head < feat_plsize2(L)) ? 1 : 0;
+}
+
+// Pointer doubling: Jn = J o J.
+__global__ void __launch_bounds__(256) k_feat_jump(const int* __restrict__ J, int M, int* __restrict__ Jn) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= M) return;
+    const int a = J[q];
+    Jn[q] = a < 0 ? -1 : J[a];
+}
+
+// From the top level down, every marked point marks its 2^l-th successor.  A mark set during the same launch is a
+// point of the chain too, so a thread that sees it early adds only chain points: the final set is exact.
+__global__ void __launch_bounds__(256) k_feat_mark(const int* __restrict__ J, int M, unsigned char* vis) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= M) return;
+    if (vis[q] && J[q] >= 0) vis[J[q]] = 1;
+}
+
+__global__ void __launch_bounds__(256) k_feat_vis_index(const unsigned char* __restrict__ vis, int M, int* __restrict__ s) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < M) s[q] = vis[q] ? q : -1;
+}
+
+// The type after the plane loop and the edge pass, and intersect.  pv[q]: the last visited point before q.
+__global__ void __launch_bounds__(256) k_feat_types(const float4* __restrict__ P, const double* __restrict__ rng,
+                                                    const double* __restrict__ dista, const int* __restrict__ lkey,
+                                                    const int* __restrict__ lbeg, const int* __restrict__ lend,
+                                                    const int* __restrict__ lhead, int M, int min_size, FeatConst c,
+                                                    const FeatStep* __restrict__ st, const unsigned char* __restrict__ vis,
+                                                    const int* __restrict__ pv, int* __restrict__ ft, double* __restrict__ isect) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= M) return;
+    const FeatLine L = feat_line(lbeg, lend, lhead, lkey[q], min_size);
+    const int p = pv[q];
+    const FeatStep sq = st[q];
+    const FeatStep sp = p >= 0 ? st[p] : sq;
+    const FeatEdge e = feat_types_at(reinterpret_cast<const LidarPoint*>(P), rng, dista, L, q, vis[q] != 0, sq, p, sp, c);
+    ft[q] = e.ftype;
+    isect[q] = e.intersect;
+}
+
+__global__ void __launch_bounds__(256) k_feat_small(const double* __restrict__ rng, const double* __restrict__ dista,
+                                                    const int* __restrict__ lkey, const int* __restrict__ lbeg,
+                                                    const int* __restrict__ lend, const int* __restrict__ lhead, int M, int min_size,
+                                                    FeatConst c, const int* __restrict__ ft, const double* __restrict__ isect,
+                                                    unsigned char* __restrict__ small) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= M) return;
+    const FeatLine L = feat_line(lbeg, lend, lhead, lkey[q], min_size);
+    small[q] = feat_small_cond(rng + L.b, dista + L.b, L.m, L.head, q - L.b, ft[q], isect[q], c) ? 1 : 0;
+}
+
+// s[q] = q where a run of small-plane conditions starts (a run never crosses a line: the condition is false at both
+// ends of every line), else -1; the inclusive max-scan gives each point its run's start.
+__global__ void __launch_bounds__(256) k_feat_small_seed(const unsigned char* __restrict__ small, int M, int* __restrict__ s) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q < M) s[q] = (small[q] && !(q > 0 && small[q - 1])) ? q : -1;
+}
+
+// The final type, and s[q] = q where a surface run starts (at the head, or after a non-surface point), else -1.
+__global__ void __launch_bounds__(256) k_feat_final(const int* __restrict__ ft, const unsigned char* __restrict__ small,
+                                                    const int* __restrict__ rs, const int* __restrict__ lkey,
+                                                    const int* __restrict__ lbeg, const int* __restrict__ lend,
+                                                    const int* __restrict__ lhead, int M, int min_size, int* __restrict__ fin,
+                                                    int* __restrict__ s) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= M) return;
+    const FeatLine L = feat_line(lbeg, lend, lhead, lkey[q], min_size);
+    const int j = q - L.b;
+    const int f = feat_final_at(ft, small, rs, M, q);
+    fin[q] = f;
+    const bool surf = j >= L.head && feat_is_surf(f);
+    s[q] = (surf && (j == L.head || !feat_is_surf(feat_final_at(ft, small, rs, M, q - 1)))) ? q : -1;
+}
+
+// The surface output at q into dec / kept, which flb_lidar_upload's compaction and time sort then take.
+__global__ void __launch_bounds__(256) k_feat_emit(const float4* __restrict__ P, const int* __restrict__ fin,
+                                                   const int* __restrict__ rs2, const int* __restrict__ lkey,
+                                                   const int* __restrict__ lbeg, const int* __restrict__ lend,
+                                                   const int* __restrict__ lhead, int M, int min_size, int filter_num,
+                                                   float4* __restrict__ dec, int* __restrict__ kept) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= M) return;
+    const FeatLine L = feat_line(lbeg, lend, lhead, lkey[q], min_size);
+    LidarPoint o;
+    const bool e = feat_emit_at(reinterpret_cast<const LidarPoint*>(P), fin, rs2, L, q, filter_num, &o);
+    if (e) dec[q] = make_float4(o.x, o.y, o.z, o.t);
+    kept[q] = e ? 1 : 0;
+}
+
 }  // namespace flb

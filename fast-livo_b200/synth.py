@@ -535,6 +535,132 @@ def make_velodyne_spin(layout="xyzirt", seed=1, n_scans=16, n_cols=1800, point_f
     return a.tobytes(), fmt
 
 
+def _feature_scene_range(az, el):
+    """Ray-cast distance from the origin along (az, el) into a structured scene: the ground, two walls meeting at a
+    right angle, a wall at a shallow angle, a pole, a thin wire and a plate that occludes the walls (range jumps).
+    inf where nothing is hit within 60 m."""
+    dx, dy, dz = np.cos(el) * np.cos(az), np.cos(el) * np.sin(az), np.sin(el)
+    best = np.full(az.shape, np.inf)
+
+    def take(t, ok):
+        ok = ok & (t > 0) & (t < best)
+        best[ok] = t[ok]
+
+    with np.errstate(divide="ignore", invalid="ignore"):
+        t = -1.6 / dz                                                       # ground z = -1.6
+        take(t, dz < 0)
+        t = 6.0 / dx                                                        # wall x = 6, y in [-8, 5]
+        take(t, (dx > 0) & (np.abs(dy * t + 1.5) <= 6.5) & (dz * t < 3))
+        t = 5.0 / dy                                                        # wall y = 5, x in [-3, 6]: the right-angle corner
+        take(t, (dy > 0) & (dx * t >= -3) & (dx * t <= 6) & (dz * t < 3))
+        nx, ny = -np.cos(np.deg2rad(8.0)), np.sin(np.deg2rad(8.0))          # shallow wall behind: n . p = 7
+        t = 7.0 / (nx * dx + ny * dy)
+        take(t, (nx * dx + ny * dy > 0) & (dz * t < 3))
+        t = 2.5 / dx                                                        # occluding plate x = 2.5, y in [1.0, 1.6]
+        take(t, (dx > 0) & (dy * t >= 1.0) & (dy * t <= 1.6) & (dz * t < 0.8))
+        cx, cy, r = 3.0, -2.0, 0.08                                          # a pole
+        b = dx * cx + dy * cy
+        h2 = dx * dx + dy * dy
+        disc = b * b - h2 * (cx * cx + cy * cy - r * r)
+        t = (b - np.sqrt(np.maximum(disc, 0))) / h2
+        take(t, disc >= 0)
+        take(1.2 / dz,                                                      # a wire along x at y = -1, z = 1.2
+             (dz > 0) & (np.abs(dy * 1.2 / dz + 1.0) < 0.02))
+    best[best > 60.0] = np.inf
+    return best
+
+
+def make_feature_scan(kind, seed=1, n_scans=None, n_cols=None, point_filter_num=1, timed=True, blind=None, nan_returns=True):
+    """One structured message for the feature branches (flb_lidar_upload_features, flb_lidar_upload_velodyne_features)
+    as (records, fmt).  The sensor scans a scene of ground, walls at right and shallow angles, a pole, a wire and an
+    occluding plate line by line, so planes, edges and range jumps all occur; also runs of points inside blind, empty,
+    one-point and five-point lines, lines that end on a wall, and records the input filters drop.
+    kind: "livox" (6 lines fired in turn, repeated coordinates, tags, lines >= n_scans), "ouster" (u8 ring at 26,
+    zeros for no return, records with ring >= n_scans), "velodyne" (NaN for no return; `timed` False: no times, so they
+    come from the yaw; `nan_returns` False: a ray that hits nothing returns from 59 m instead of NaN, as NaN points
+    in pl_surf make the upload refuse the cloud).  fmt: flb_lidar_format's fields, with off_line the ring (Velodyne: flb_velodyne_format's)."""
+    rng = np.random.default_rng(4099 * seed + LIDAR_KINDS[kind])
+    if kind == "livox":
+        n_scans = n_scans or 6
+        n_cols = n_cols or 400
+        blind = 0.5 if blind is None else blind
+        col = np.repeat(np.arange(n_cols), n_scans)
+        line = np.tile(np.arange(n_scans), n_cols)
+        az = np.deg2rad(-35.0 + 70.0 * col / n_cols + 3.0 * np.sin(col / 37.0 + line)) + rng.normal(0, 2e-4, col.size)
+        el = np.deg2rad(-12.0 + 4.0 * line + 6.0 * np.sin(col / 53.0 + 0.7 * line))
+    else:
+        n_scans = n_scans or (64 if kind == "ouster" else 16)
+        n_cols = n_cols or (256 if kind == "ouster" else 450)
+        blind = (0.8 if kind == "ouster" else 1.0) if blind is None else blind
+        col = np.repeat(np.arange(n_cols), n_scans)
+        line = np.tile(np.arange(n_scans), n_cols)
+        az = np.pi - 2 * np.pi * (col + 0.5) / n_cols + rng.normal(0, 2e-4, col.size)
+        el = np.deg2rad(-22.0 + 40.0 * line / max(n_scans - 1, 1))
+    d = _feature_scene_range(az, el)
+    d += rng.normal(0, 0.004, d.size) * np.isfinite(d)
+    n = d.size
+    near = (col % 97 < 6) & (line % 3 == 0)                                 # runs of points inside blind
+    d[near] = 0.3 * blind + 0.02 * (col[near] % 97)
+    miss = ~np.isfinite(d)
+    if kind == "velodyne" and not nan_returns:
+        d[miss] = 59.0
+        miss[:] = False
+    xyz = np.stack([d * np.cos(el) * np.cos(az), d * np.cos(el) * np.sin(az), d * np.sin(el)], 1).astype(np.float32)
+    xyz[miss] = np.nan if kind == "velodyne" else 0.0
+    ring = line.copy()
+    sparse = [n_scans - 1, n_scans - 2, n_scans - 3] if n_scans >= 6 else []
+    keep = np.ones(n, bool)
+    for r, cnt in zip(sparse, (0, 1, 5)):                                   # empty, one-point and five-point lines
+        idx = np.flatnonzero(ring == r)
+        keep[idx[cnt:]] = False
+    if kind != "livox" and n_scans >= 8:
+        idx = np.flatnonzero(ring == n_scans - 4)                           # 14 points 2 cm apart on a wall: the plane
+        keep[idx[14:]] = False                                              # group from the head reaches the line's end
+        dense = np.stack([np.full(14, 6.0), 0.3 + 0.02 * np.arange(14), np.full(14, 0.4)], 1)
+        xyz[idx[:14]] = dense + rng.normal(0, 1e-4, (14, 3))
+    if kind == "velodyne" and n_scans >= 8:
+        idx = np.flatnonzero(ring == n_scans - 5)                           # a line entirely within blind
+        xyz[idx] *= np.float32(0.3 * blind) / np.maximum(np.linalg.norm(xyz[idx], axis=1, keepdims=True), 1e-6)
+    if kind == "livox":
+        keep[:] = True
+        keep[np.flatnonzero(ring == n_scans - 1)[5:]] = False               # a five-point line
+    xyz, ring, col = xyz[keep], ring[keep], col[keep]
+    n = len(ring)
+    if kind == "livox":
+        a = np.zeros(n, LIVOX_POINT)
+        a["offset_time"] = (np.arange(n, dtype=np.int64) * 4167 + 3).astype(np.uint32)
+        rep = np.flatnonzero(rng.random(n) < 0.02)
+        for i in rep[rep > 0]:                                              # repeated coordinates: all three, or one
+            if rng.random() < 0.5:
+                xyz[i] = xyz[i - 1]
+            else:
+                xyz[i, 2] = xyz[i - 1, 2]
+        a["line"] = ring
+        over = rng.random(n) < 0.01
+        a["line"][over] = rng.integers(n_scans, n_scans + 3, over.sum())
+        tag = rng.choice(np.array([0x10, 0x00, 0x20, 0x30], np.uint8), n, p=[0.93, 0.03, 0.02, 0.02])
+        a["tag"] = tag | (rng.integers(0, 256, n).astype(np.uint8) & 0xC0)
+        fmt = dict(kind=1, off_time=0, off_x=4, off_y=8, off_z=12, off_tag=17, off_line=18)
+    elif kind == "ouster":
+        a = np.zeros(n, OUSTER_POINT)
+        a["t"] = col * 97656 + ring * 50
+        a["ring"] = ring
+        over = rng.random(n) < 0.005
+        a["ring"][over] = n_scans
+        fmt = dict(kind=3, off_x=0, off_y=4, off_z=8, off_time=20, off_tag=0, off_line=26)
+    else:
+        a = np.zeros(n, VELODYNE_POINT)
+        a["ring"] = ring
+        over = rng.random(n) < 0.005
+        a["ring"][over] = n_scans + 1
+        if timed:
+            a["time"] = col * 55.296e-6 + ring * 2.304e-6 + 1e-6
+        fmt = dict(kind=2, off_x=0, off_y=4, off_z=8, off_time=20, off_tag=0, off_line=16)
+    a["x"], a["y"], a["z"] = xyz[:, 0], xyz[:, 1], xyz[:, 2]
+    fmt.update(point_step=a.dtype.itemsize, n_scans=n_scans, point_filter_num=point_filter_num, blind=blind)
+    return a.tobytes(), fmt
+
+
 # ---------------------------------------------------------------------------------------------------------
 # Visual-map sequences (SURVEY.md section 8 rows f2 / f4): several frames of ONE scene along a short trajectory
 # ---------------------------------------------------------------------------------------------------------

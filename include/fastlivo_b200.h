@@ -284,6 +284,35 @@ typedef struct flb_velodyne_format {
 int flb_lidar_upload_velodyne(flb_handle* h, const flb_velodyne_format* fmt, const void* records, int n_records, int* n_points,
                               float* last_offset_ms, int* yaw_times);
 
+/* ---- surface features (feature_extract_enable: 1) ------------------------------------------------------------------
+ * The feature branches of Preprocess: avia_handler :94-135, oust64_handler :174-227 and velodyne_handler :299-373,
+ * each bucketing its points by line and running give_feature (:466-775) per line.  The result is pl_surf (the only
+ * cloud FAST-LIVO reads, :43-70), sorted by time stably on pl_surf's line-major order, and it goes exactly where
+ * flb_lidar_upload's goes: the idle set on the copy stream, a page-locked source read in place, the swap on success
+ * only, the cursor reset to 0; on any error the previous cloud and cursor stay current and unchanged.  So
+ * flb_lidar_download, flb_imu_undistort_lidar, flb_scan_from_undistorted and flb_world_cloud work on it unchanged.
+ *   dis_b: Preprocess::disB.  The reference's constructor assigns disA twice (:12-13) and never disB, so its value there
+ *     is whatever the heap held; the caller states it.  The other constants are the constructor's (group_size 8,
+ *     disA 0.1, p2l_ratio 225, ...), and its four cos() thresholds are computed with the host's std::cos.
+ *   point_filter_num: the chunk length of the surface output (:728-774), not an input decimation.
+ *   Per handler: Livox (FLB_LIDAR_LIVOX): from record 1, a record is dropped when |dx|, |dy| or |dz| against the raw
+ *     previous record is below 1e-8, x*x + y*y < blind, line > n_scans or (tag & 0x30) != 0x10; line == n_scans is
+ *     dropped too (its buffer is never processed); lines of <= 5 points are skipped; range = x*x + y*y.  Ouster
+ *     (FLB_LIDAR_OUSTER): off_line names the u8 ring (26 in ouster_ros::Point); the float x*x + y*y + z*z < blind *
+ *     blind drops a point, and ring < n_scans is required; an empty ring is skipped (the reference indexes types[-1]).
+ *     Velodyne: no blind filter at input; a ring >= n_scans is dropped; on the yaw route (no per-point times, as
+ *     flb_lidar_upload_velodyne) each ring's first record is not kept; lines of < 2 points are skipped.
+ *   Defined where the reference is not (DESIGN §2): a line's last dista is 0.0; a plane step's write past the line's
+ *   end is dropped; a line entirely within blind yields nothing; Eigen's reductions are left to right.
+ *   FLB_ERR_INVALID: fmt NULL, records NULL with n_records > 0, n_records < 0, dis_b not finite, point_filter_num < 1,
+ *   n_scans outside 1..128 (pl_buff[128]), blind not finite, a field that does not fit or is misaligned, a point of
+ *   pl_surf or its time that is not finite; flb_lidar_upload_features with FLB_LIDAR_VELODYNE or FLB_LIDAR_XT32 (the
+ *   XT32 has no feature branch, :432-464: flb_lidar_upload serves it with either setting). */
+int flb_lidar_upload_features(flb_handle* h, const flb_lidar_format* fmt, double dis_b, const void* records, int n_records,
+                              int* n_points, float* last_offset_ms);
+int flb_lidar_upload_velodyne_features(flb_handle* h, const flb_velodyne_format* fmt, double dis_b, const void* records,
+                                       int n_records, int* n_points, float* last_offset_ms, int* yaw_times);
+
 /* ---- scan ------------------------------------------------------------------------
  * feats_down_body (src/laserMapping.cpp:1398-1399): N already-downsampled points in
  * the LiDAR body frame. */
