@@ -23,6 +23,8 @@
 //        replace lasermap_fov_segment()  src/laserMapping.cpp:363-421  (local-map cube + box delete on the device)
 //   flb::upload_camera_frame(h, bgr, gray_rule)   replaces the resize / img_rgb / cvtColor lines of
 //        LidarSelector::detect  src/lidar_selection.cpp:1029-1037  (one BGR upload; the gray image is made on the device)
+//   flb::upload_camera_msg(h, msg, gray_rule)   the same from the sensor_msgs::Image itself, replacing getImageFromMsg
+//        (src/laserMapping.cpp:490-493): mono8, rgb8, bgra8, rgba8 and Bayer frames are converted on the device
 //   flb::preprocess(h, livox_msg, n_scans, blind, point_filter_num)  /  flb::preprocess(h, pc2_msg, kind, n_scans, blind,
 //        point_filter_num)   replace p_pre->process (src/preprocess.cpp:43-70) and the sort of sync_packages
 //        (src/laserMapping.cpp:551): the driver's records go up as they are; the cloud is decoded and sorted on the device
@@ -242,6 +244,26 @@ inline flb_vio_params make_vio_params(const Mat3& Rcl, const Vec3& Pcl, const Ma
 template <class Image>
 inline void upload_camera_frame(flb_handle* h, const Image& bgr, int gray_rule) {
     check(h, flb_image_upload_bgr(h, bgr.data, bgr.cols, bgr.rows, (int)bgr.step, gray_rule));
+}
+
+// The FLB_ENC_* of a sensor_msgs::Image encoding string (sensor_msgs/image_encodings.h); any other string throws
+// flb::Error (FLB_ERR_INVALID) before anything is uploaded, so the caller can fall back to cv_bridge.
+inline int camera_encoding(const std::string& encoding) {
+    static const struct { const char* name; int enc; } table[] = {
+        {"bgr8", FLB_ENC_BGR8},   {"rgb8", FLB_ENC_RGB8},   {"mono8", FLB_ENC_MONO8},
+        {"bgra8", FLB_ENC_BGRA8}, {"rgba8", FLB_ENC_RGBA8}, {"bayer_rggb8", FLB_ENC_BAYER_RGGB8},
+        {"bayer_bggr8", FLB_ENC_BAYER_BGGR8}, {"bayer_gbrg8", FLB_ENC_BAYER_GBRG8}, {"bayer_grbg8", FLB_ENC_BAYER_GRBG8}};
+    for (const auto& e : table)
+        if (encoding == e.name) return e.enc;
+    throw Error(FLB_ERR_INVALID, "flb::camera_encoding: encoding '" + encoding + "' is not taken on the device");
+}
+// ImageMsg: sensor_msgs::Image-like (.encoding, .width, .height, .step, .data with .data()), the message img_cbk
+// receives (src/laserMapping.cpp:490-493).  Replaces getImageFromMsg + upload_camera_frame: the message's own bytes go
+// up and the device converts, demosaics and resizes them as cv_bridge::toCvCopy(msg, "bgr8") and detect() would.
+template <class ImageMsg>
+inline void upload_camera_msg(flb_handle* h, const ImageMsg& msg, int gray_rule) {
+    const int enc = camera_encoding(msg.encoding);
+    check(h, flb_image_upload_msg(h, msg.data.data(), (int)msg.width, (int)msg.height, (int)msg.step, enc, gray_rule));
 }
 
 template <class Image, class SubMap, class StatesGroup>

@@ -183,6 +183,10 @@ class FovParams(C.Structure):
 CLOUD_SCAN, CLOUD_UNDISTORTED = 0, 1       # flb_world_cloud sources (FLB_CLOUD_*)
 LIDAR_LIVOX, LIDAR_VELODYNE, LIDAR_OUSTER, LIDAR_XT32 = 1, 2, 3, 4    # flb_lidar_format.kind (FLB_LIDAR_*)
 GRAY_CV4, GRAY_CV3 = 0, 1                  # flb_image_upload_bgr's cvtColor rules (FLB_GRAY_*)
+# flb_image_upload_msg's encodings (FLB_ENC_*), keyed by sensor_msgs::Image's encoding string
+ENCODINGS = {"bgr8": 0, "rgb8": 1, "mono8": 2, "bgra8": 3, "rgba8": 4,
+             "bayer_rggb8": 5, "bayer_bggr8": 6, "bayer_gbrg8": 7, "bayer_grbg8": 8}
+ENC_BYTES = {0: 3, 1: 3, 2: 1, 3: 4, 4: 4, 5: 1, 6: 1, 7: 1, 8: 1}       # bytes per pixel
 
 # every symbol include/fastlivo_b200.h declares (checked by the CPU-only test tier)
 SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "flb_set_stream", "flb_synchronize", "flb_host_alloc", "flb_host_free",
@@ -201,7 +205,7 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset",
            "flb_image_upload_bgr", "flb_image_download",
            "flb_lidar_upload", "flb_lidar_download", "flb_imu_undistort_lidar", "flb_lidar_upload_velodyne",
-           "flb_lidar_upload_features", "flb_lidar_upload_velodyne_features"]
+           "flb_lidar_upload_features", "flb_lidar_upload_velodyne_features", "flb_image_upload_msg"]
 
 
 def lib_path() -> str:
@@ -269,6 +273,7 @@ def lib():
         L.flb_visual_candidates.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
         L.flb_image_upload.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int]
         L.flb_image_upload_bgr.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
+        L.flb_image_upload_msg.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
         L.flb_image_download.argtypes = [vp, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.flb_patches_upload.argtypes = [vp, vp, vp, vp, C.c_int]
         L.flb_camera_set.argtypes = [vp, C.POINTER(Camera)]
@@ -496,6 +501,21 @@ class Handle:
         if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.strides[1:] != (3, 1) or a.strides[0] < 0:
             a = np.ascontiguousarray(a, np.uint8)
         self._ck(self.L.flb_image_upload_bgr(self.h, _p(a), a.shape[1], a.shape[0], a.strides[0], int(gray_rule)))
+
+    def image_upload_msg(self, img, encoding, gray_rule=GRAY_CV4):
+        """flb_image_upload_msg: a camera message's pixels as a uint8 array, (height, width) for mono8 and Bayer or
+        (height, width, bytes per pixel) for the others; encoding: a sensor_msgs::Image encoding string or FLB_ENC_*.
+        A strided view (e.g. a column slice) is passed with its own row step; its pixels must be contiguous in a row."""
+        enc = ENCODINGS[encoding] if isinstance(encoding, str) else int(encoding)
+        bpp = ENC_BYTES.get(enc, 1)
+        a = np.asarray(img)
+        if a.ndim == 2:
+            a = a[:, :, None]
+        if a.dtype != np.uint8 or a.ndim != 3 or a.strides[1:] != (a.shape[2], 1) or a.strides[0] < 0:
+            a = np.ascontiguousarray(a, np.uint8)
+        if a.shape[2] != bpp:
+            raise ValueError(f"image_upload_msg: encoding {encoding} has {bpp} bytes per pixel, the array {a.shape[2]}")
+        self._ck(self.L.flb_image_upload_msg(self.h, _p(a), a.shape[1], a.shape[0], a.strides[0], enc, int(gray_rule)))
 
     def image_download(self, gray=True, bgr=True):
         """flb_image_download: (gray (H, W) uint8 or None, bgr (H, W, 3) uint8 or None) of the current image set."""

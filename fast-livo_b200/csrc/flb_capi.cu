@@ -616,6 +616,78 @@ int vio_inputs_acquire(flb_handle* h) {
     }
     return FLB_OK;
 }
+
+// The camera-size outputs of image_upload_frame from the dense frame `src` (packed encoding ENC) on copy_stream.
+template <int ENC>
+void launch_image_out(flb_handle* h, const unsigned char* src, int width, int height, int gray_rule) {
+    const int W = h->cam.width, H = h->cam.height;
+    const unsigned rows = (unsigned)std::min(H, 65535);
+    const dim3 grid4((unsigned)((W + 4 * 128 - 1) / (4 * 128)), rows);
+    const bool vec = (W % 4) == 0;
+    if (width == W && height == H) {
+        if (vec) k_image_prep<false, true, ENC><<<grid4, 128, 0, h->copy_stream>>>(src, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
+        else k_image_prep<false, false, ENC><<<grid4, 128, 0, h->copy_stream>>>(src, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
+    } else if (width == 2 * W && height == 2 * H) {
+        if (vec) k_image_prep<true, true, ENC><<<grid4, 128, 0, h->copy_stream>>>(src, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
+        else k_image_prep<true, false, ENC><<<grid4, 128, 0, h->copy_stream>>>(src, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
+    } else {
+        const dim3 grid((unsigned)((W + 127) / 128), rows);
+        k_image_resize_linear<ENC><<<grid, 128, 0, h->copy_stream>>>(src, width, height, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
+    }
+}
+
+// flb_image_upload_bgr / flb_image_upload_msg once their arguments are checked: the frame (width x height pixels of
+// `encoding`, step_bytes a row) into the idle image set as the camera-size colour frame and gray image.  The frame's
+// rows go up dense into img_raw, a Bayer mosaic behind the room for its demosaiced BGR8 frame, which k_bayer_bgr fills
+// before the outputs are made from it.  The copy and every kernel run on copy_stream, so stream order fences img_raw's
+// reuse by the next frame.
+int image_upload_frame(flb_handle* h, const uint8_t* src, int width, int height, int step_bytes, int encoding, int gray_rule) {
+    const int W = h->cam.width, H = h->cam.height;
+    const bool bayer = encoding >= kEncBayerRggb8;
+    const size_t row = (size_t)width * enc_bpp(encoding), raw_bytes = row * height, px = (size_t)W * H;
+    const size_t decoded = bayer ? (size_t)width * height * 3 : 0;
+    FLB_CUDA(h, h->img_raw.reserve(decoded + raw_bytes));
+    FLB_CUDA(h, h->img_alt.reserve(px));
+    FLB_CUDA(h, h->img_bgr_alt.reserve(px * 3));
+    unsigned char* raw = h->img_raw.p + decoded;
+    // the raw frame goes up before the wait for the idle set's readers: only the kernel that writes the set waits for them
+    if (is_pinned(src)) {
+        FLB_CUDA(h, cudaMemcpy2DAsync(raw, row, src, step_bytes, row, height, cudaMemcpyHostToDevice, h->copy_stream));
+    } else {
+        void* stv = nullptr;
+        FLB_CUDA(h, h->st_img.acquire(raw_bytes, &stv));
+        unsigned char* st = static_cast<unsigned char*>(stv);
+        if ((size_t)step_bytes == row) std::memcpy(st, src, raw_bytes);
+        else for (int r = 0; r < height; ++r) std::memcpy(st + (size_t)r * row, src + (size_t)r * step_bytes, row);
+        FLB_CUDA(h, cudaMemcpyAsync(raw, st, raw_bytes, cudaMemcpyHostToDevice, h->copy_stream));
+        FLB_CUDA(h, h->st_img.mark(h->copy_stream));
+    }
+    if (bayer) {
+        const dim3 grid((unsigned)((width + 127) / 128), (unsigned)std::min(height, 65535));
+        k_bayer_bgr<<<grid, 128, 0, h->copy_stream>>>(raw, width, height, encoding, h->img_raw.p);
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches++;
+    }
+    { int rcq = vio_copy_begin(h, h->img_slot); if (rcq) return rcq; }
+    switch (bayer ? (int)kEncBgr8 : encoding) {
+        case kEncRgb8: launch_image_out<kEncRgb8>(h, raw, width, height, gray_rule); break;
+        case kEncMono8: launch_image_out<kEncMono8>(h, raw, width, height, gray_rule); break;
+        case kEncBgra8: launch_image_out<kEncBgra8>(h, raw, width, height, gray_rule); break;
+        case kEncRgba8: launch_image_out<kEncRgba8>(h, raw, width, height, gray_rule); break;
+        default: launch_image_out<kEncBgr8>(h, h->img_raw.p, width, height, gray_rule); break;
+    }
+    FLB_CUDA(h, cudaGetLastError());
+    h->launches++;
+    { int rcq = vio_copy_end(h); if (rcq) return rcq; }
+    std::swap(h->img, h->img_alt);
+    std::swap(h->img_bgr, h->img_bgr_alt);
+    h->img_bgr_valid = true;
+    h->img_slot.slot ^= 1;
+    h->img_w = W;
+    h->img_h = H;
+    h->last_vio_valid = false;
+    return FLB_OK;
+}
 int vio_inputs_release(flb_handle*) { return FLB_OK; }   // (readers are fenced per slot at the next upload: vio_copy_begin)
 
 // Perform the deferred device-side state moves with plain copies (every consumer other than the persistent kernels).
@@ -3147,45 +3219,23 @@ int flb_image_upload_bgr(flb_handle* h, const uint8_t* bgr, int width, int heigh
     if (!bgr || !(halve || (width == W && height == H)) || stride_bytes < 3 * width || (gray_rule != kGrayCv4 && gray_rule != kGrayCv3))
         return fail(h, FLB_ERR_INVALID, "flb_image_upload_bgr: bad arguments (%dx%d, stride %d, rule %d; camera %dx%d)", width, height,
                     stride_bytes, gray_rule, W, H);
-    const size_t row = (size_t)width * 3, raw_bytes = row * height, px = (size_t)W * H;
-    FLB_CUDA(h, h->img_raw.reserve(raw_bytes));
-    FLB_CUDA(h, h->img_alt.reserve(px));
-    FLB_CUDA(h, h->img_bgr_alt.reserve(px * 3));
-    // the raw frame goes up before the wait for the idle set's readers: only k_image_prep has to wait for them
-    if (is_pinned(bgr)) {
-        FLB_CUDA(h, cudaMemcpy2DAsync(h->img_raw.p, row, bgr, stride_bytes, row, height, cudaMemcpyHostToDevice, h->copy_stream));
-    } else {
-        void* stv = nullptr;
-        FLB_CUDA(h, h->st_img.acquire(raw_bytes, &stv));
-        unsigned char* st = static_cast<unsigned char*>(stv);
-        if ((size_t)stride_bytes == row) std::memcpy(st, bgr, raw_bytes);
-        else for (int r = 0; r < height; ++r) std::memcpy(st + (size_t)r * row, bgr + (size_t)r * stride_bytes, row);
-        FLB_CUDA(h, cudaMemcpyAsync(h->img_raw.p, st, raw_bytes, cudaMemcpyHostToDevice, h->copy_stream));
-        FLB_CUDA(h, h->st_img.mark(h->copy_stream));
-    }
-    { int rcq = vio_copy_begin(h, h->img_slot); if (rcq) return rcq; }
-    {
-        const dim3 grid((unsigned)((W + 4 * 128 - 1) / (4 * 128)), (unsigned)std::min(H, 65535));
-        const bool vec = (W % 4) == 0;
-        if (halve) {
-            if (vec) k_image_prep<true, true><<<grid, 128, 0, h->copy_stream>>>(h->img_raw.p, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
-            else k_image_prep<true, false><<<grid, 128, 0, h->copy_stream>>>(h->img_raw.p, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
-        } else {
-            if (vec) k_image_prep<false, true><<<grid, 128, 0, h->copy_stream>>>(h->img_raw.p, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
-            else k_image_prep<false, false><<<grid, 128, 0, h->copy_stream>>>(h->img_raw.p, W, H, gray_rule, h->img_bgr_alt.p, h->img_alt.p);
-        }
-        FLB_CUDA(h, cudaGetLastError());
-        h->launches++;
-    }
-    { int rcq = vio_copy_end(h); if (rcq) return rcq; }
-    std::swap(h->img, h->img_alt);
-    std::swap(h->img_bgr, h->img_bgr_alt);
-    h->img_bgr_valid = true;
-    h->img_slot.slot ^= 1;
-    h->img_w = W;
-    h->img_h = H;
-    h->last_vio_valid = false;
-    return FLB_OK;
+    return image_upload_frame(h, bgr, width, height, stride_bytes, kEncBgr8, gray_rule);
+}
+
+int flb_image_upload_msg(flb_handle* h, const uint8_t* data, int width, int height, int step_bytes, int encoding, int gray_rule) {
+    FLB_CHECK_H(h);
+    if (!h->cam_set) return fail(h, FLB_ERR_STATE, "flb_image_upload_msg: flb_camera_set first");
+    const int W = h->cam.width, H = h->cam.height;
+    const bool known = encoding >= kEncBgr8 && encoding <= kEncBayerGrbg8;
+    const bool same = (width == W && height == H);
+    // detect() resizes to (int)(cols * 0.5) x (int)(rows * 0.5): any other size leaves the camera's size behind
+    const bool resized = !same && (width == 2 * W || width == 2 * W + 1) && (height == 2 * H || height == 2 * H + 1);
+    const bool linear = resized && !(width == 2 * W && height == 2 * H);
+    if (!data || !known || !(same || resized) || (gray_rule != kGrayCv4 && gray_rule != kGrayCv3) ||
+        (linear && gray_rule == kGrayCv3) || (known && (int64_t)step_bytes < (int64_t)enc_bpp(encoding) * width))
+        return fail(h, FLB_ERR_INVALID, "flb_image_upload_msg: bad arguments (%dx%d, step %d, encoding %d, rule %d; camera %dx%d)", width,
+                    height, step_bytes, encoding, gray_rule, W, H);
+    return image_upload_frame(h, data, width, height, step_bytes, encoding, gray_rule);
 }
 
 int flb_image_download(flb_handle* h, uint8_t* gray, uint8_t* bgr, int capacity_pixels, int* width, int* height) {

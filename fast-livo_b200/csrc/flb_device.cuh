@@ -1627,6 +1627,65 @@ FLB_HD unsigned bgr_to_gray(unsigned b, unsigned g, unsigned r, int rule) {
 // 2x2 area path there, one rounded mean per channel of each 2x2 source block.
 FLB_HD unsigned mean2x2(unsigned a, unsigned b, unsigned c, unsigned d) { return (a + b + c + d + 2u) >> 2; }
 
+// The camera message's encodings (FLB_ENC_* in the C ABI), each as cv_bridge::toCvCopy(msg, "bgr8") converts it.
+enum { kEncBgr8 = 0, kEncRgb8 = 1, kEncMono8 = 2, kEncBgra8 = 3, kEncRgba8 = 4,
+       kEncBayerRggb8 = 5, kEncBayerBggr8 = 6, kEncBayerGbrg8 = 7, kEncBayerGrbg8 = 8 };
+FLB_HD constexpr int enc_bpp(int enc) { return (enc == kEncMono8 || enc >= kEncBayerRggb8) ? 1 : (enc == kEncBgra8 || enc == kEncRgba8) ? 4 : 3; }
+// The byte of a packed pixel (BGR8, RGB8, MONO8, BGRA8, RGBA8) that holds BGR channel ch (0 b, 1 g, 2 r): the
+// cvtColor of each to BGR is this byte permutation (GRAY2BGR repeats the one byte, the alpha byte is dropped).
+FLB_HD constexpr int enc_byte(int enc, int ch) { return enc == kEncMono8 ? 0 : (enc == kEncRgb8 || enc == kEncRgba8) ? 2 - ch : ch; }
+
+// The colour (0 b, 1 g, 2 r) of site (x, y) of a Bayer mosaic; the ROS encoding names the 2x2 tile from its top-left.
+FLB_HD int bayer_site(int enc, int x, int y) {
+    const unsigned tile = enc == kEncBayerRggb8 ? 0x0112u : enc == kEncBayerBggr8 ? 0x2110u : enc == kEncBayerGbrg8 ? 0x1201u : 0x1021u;
+    return (int)((tile >> (4 * (2 * (y & 1) + (x & 1)))) & 0xfu);
+}
+// cv_bridge's Bayer -> bgr8 (cvtColor COLOR_Bayer{BG,RG,GR,GB}2BGR for rggb8, bggr8, gbrg8, grbg8): OpenCV's bilinear
+// demosaic of pixel (x, y) of a dense w x h mosaic m, w >= 3 and h >= 3.  Interior: the site's own colour as it is; G
+// at an R / B site the rounded mean of its 4 edge neighbours, the other of R / B the rounded mean of its 4 diagonals;
+// R and B at a G site the rounded mean of the horizontal or the vertical pair of that colour.  The outer rows and
+// columns copy the nearest interior pixel.
+FLB_HD void bayer_bgr(const unsigned char* m, int w, int h, int enc, int x, int y, unsigned& b, unsigned& g, unsigned& r) {
+    x = x < 1 ? 1 : (x > w - 2 ? w - 2 : x);
+    y = y < 1 ? 1 : (y > h - 2 ? h - 2 : y);
+    const unsigned char* p = m + (size_t)y * w + x;
+    const unsigned v = p[0];
+    const int site = bayer_site(enc, x, y);
+    if (site == 1) {
+        const unsigned hp = (p[-1] + p[1] + 1u) >> 1, vp = (p[-w] + p[w] + 1u) >> 1;
+        const bool b_horizontal = bayer_site(enc, x - 1, y) == 0;
+        g = v;
+        b = b_horizontal ? hp : vp;
+        r = b_horizontal ? vp : hp;
+    } else {
+        const unsigned diag = (p[-w - 1] + p[-w + 1] + p[w - 1] + p[w + 1] + 2u) >> 2;
+        g = (p[-w] + p[w] + p[-1] + p[1] + 2u) >> 2;
+        b = site == 0 ? v : diag;
+        r = site == 2 ? v : diag;
+    }
+}
+
+// cv::resize(img, Size(w * 0.5, h * 0.5), INTER_LINEAR) of an 8-bit frame that is not exactly twice the output size
+// (an odd side): OpenCV's fixed-point linear rule, 11-bit weights (INTER_RESIZE_COEF_BITS).  Output index d of n from
+// a source axis of s: the first tap o (the second is min(o + 1, s - 1)) and the weights a0, a1, each rounded on its own
+// from the float position as OpenCV rounds them; positions outside the source take the edge pixel with weights
+// (2048, 0).  Needs double division, products and sums that round once each (no FMA contraction).
+struct LinearTap {
+    int o, a0, a1;
+};
+FLB_HD LinearTap linear_tap(int d, int n, int s) {
+    const double scale = 1.0 / ((double)n / s);
+    float f = (float)((d + 0.5) * scale - 0.5);
+    int o = (int)floorf(f);
+    f -= (float)o;
+    if (o < 0) { f = 0.f; o = 0; }
+    if (o >= s - 1) { f = 0.f; o = s - 1; }
+    return LinearTap{o, (int)rintf((1.f - f) * 2048.f), (int)rintf(f * 2048.f)};
+}
+// The vertical step of that rule on two horizontal sums (src * 2048 scale): OpenCV's 8-bit rounding, which drops 4
+// bits of each sum and 16 of each product before the final rounded shift.
+FLB_HD unsigned linear_v(int s0, int s1, int b0, int b1) { return (unsigned)((((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2); }
+
 // ------------------------------------------------------------------ LiDAR message decode (Preprocess::process)
 // The non-feature (`else`) branches of the four handlers of src/preprocess.cpp, one driver record at a time
 // (flb_lidar_upload).  A record is `step` bytes; its fields sit at the byte offsets of LidarFmt.

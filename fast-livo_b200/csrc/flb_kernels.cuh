@@ -3453,52 +3453,55 @@ __global__ void __launch_bounds__(BLOCK) k_lio_update_ikfom_persistent(LioArgs a
     }
 }
 
-// ---- camera frame preparation (flb_image_upload_bgr) ----------------------------------------------------------------
-// LidarSelector::detect's resize + cvtColor (src/lidar_selection.cpp:1029-1037) of one BGR8 frame held dense in `raw`
+// ---- camera frame preparation (flb_image_upload_bgr, flb_image_upload_msg) ------------------------------------------
+// LidarSelector::detect's resize + cvtColor (src/lidar_selection.cpp:1029-1037) of one frame held dense in `raw`
 // (W x H pixels, or 2W x 2H when HALVE) into the camera-size colour frame (img_rgb) and its gray image, both dense.
+// ENC: the packed encoding of `raw` (kEncBgr8, kEncRgb8, kEncMono8, kEncBgra8, kEncRgba8; P = enc_bpp bytes a pixel),
+// read through enc_byte, so a frame's conversion to BGR happens in the loads.
 // A thread makes 4 consecutive output pixels of a row; rows stride by gridDim.y.  VEC (W % 4 == 0, so every address
-// below is a multiple of 4): all loads and stores are 32-bit words, 3 per thread at 1x and 12 at 2x in, 4 out.
-template <bool HALVE, bool VEC>
+// below is a multiple of 4): all loads and stores are 32-bit words, P per thread at 1x and 4P at 2x in, 4 out.
+template <bool HALVE, bool VEC, int ENC = kEncBgr8>
 __global__ void __launch_bounds__(128) k_image_prep(const unsigned char* __restrict__ raw, int W, int H, int rule,
                                                     unsigned char* __restrict__ bgr, unsigned char* __restrict__ gray) {
     const int x0 = 4 * (blockIdx.x * blockDim.x + threadIdx.x);
     if (x0 >= W) return;
     const int n = min(4, W - x0);
+    constexpr int P = enc_bpp(ENC);
     auto byte = [](const unsigned* w, int j) { return (w[j >> 2] >> (8 * (j & 3))) & 0xffu; };
     for (int y = blockIdx.y; y < H; y += gridDim.y) {
         unsigned c[12] = {};                  // b, g, r of the 4 output pixels
         if (HALVE) {
-            const size_t pitch = (size_t)6 * W;
-            const unsigned char* s0 = raw + (size_t)(2 * y) * pitch + (size_t)6 * x0;
+            const size_t pitch = (size_t)2 * P * W;
+            const unsigned char* s0 = raw + (size_t)(2 * y) * pitch + (size_t)2 * P * x0;
             const unsigned char* s1 = s0 + pitch;
             if (VEC) {
-                unsigned a[6], b[6];
+                unsigned a[2 * P], b[2 * P];
 #pragma unroll
-                for (int k = 0; k < 6; ++k) { a[k] = reinterpret_cast<const unsigned*>(s0)[k]; b[k] = reinterpret_cast<const unsigned*>(s1)[k]; }
+                for (int k = 0; k < 2 * P; ++k) { a[k] = reinterpret_cast<const unsigned*>(s0)[k]; b[k] = reinterpret_cast<const unsigned*>(s1)[k]; }
 #pragma unroll
                 for (int j = 0; j < 12; ++j) {
-                    const int s = 6 * (j / 3) + j % 3;   // left source pixel of output pixel j / 3, channel j % 3
-                    c[j] = mean2x2(byte(a, s), byte(a, s + 3), byte(b, s), byte(b, s + 3));
+                    const int s = 2 * P * (j / 3) + enc_byte(ENC, j % 3);   // left source pixel of output pixel j / 3, channel j % 3
+                    c[j] = mean2x2(byte(a, s), byte(a, s + P), byte(b, s), byte(b, s + P));
                 }
             } else {
 #pragma unroll
                 for (int j = 0; j < 12; ++j) {
-                    const int s = 6 * (j / 3) + j % 3;
-                    if (j < 3 * n) c[j] = mean2x2(s0[s], s0[s + 3], s1[s], s1[s + 3]);
+                    const int s = 2 * P * (j / 3) + enc_byte(ENC, j % 3);
+                    if (j < 3 * n) c[j] = mean2x2(s0[s], s0[s + P], s1[s], s1[s + P]);
                 }
             }
         } else {
-            const unsigned char* s = raw + ((size_t)y * W + x0) * 3;
+            const unsigned char* s = raw + ((size_t)y * W + x0) * P;
             if (VEC) {
-                unsigned a[3];
+                unsigned a[P];
 #pragma unroll
-                for (int k = 0; k < 3; ++k) a[k] = reinterpret_cast<const unsigned*>(s)[k];
+                for (int k = 0; k < P; ++k) a[k] = reinterpret_cast<const unsigned*>(s)[k];
 #pragma unroll
-                for (int j = 0; j < 12; ++j) c[j] = byte(a, j);
+                for (int j = 0; j < 12; ++j) c[j] = byte(a, P * (j / 3) + enc_byte(ENC, j % 3));
             } else {
 #pragma unroll
                 for (int j = 0; j < 12; ++j)
-                    if (j < 3 * n) c[j] = s[j];
+                    if (j < 3 * n) c[j] = s[P * (j / 3) + enc_byte(ENC, j % 3)];
             }
         }
         unsigned char* ob = bgr + ((size_t)y * W + x0) * 3;
@@ -3519,6 +3522,51 @@ __global__ void __launch_bounds__(128) k_image_prep(const unsigned char* __restr
                     og[i] = (unsigned char)bgr_to_gray(c[3 * i], c[3 * i + 1], c[3 * i + 2], rule);
                 }
         }
+    }
+}
+
+// flb_image_upload_msg's Bayer frames: cv_bridge's demosaic (bayer_bgr) of the dense w x h mosaic `m` into the dense
+// w x h BGR8 frame `bgr` that k_image_prep or k_image_resize_linear then reads.  A thread per pixel; rows stride by
+// gridDim.y.
+__global__ void __launch_bounds__(128) k_bayer_bgr(const unsigned char* __restrict__ m, int w, int h, int enc,
+                                                   unsigned char* __restrict__ bgr) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= w) return;
+    for (int y = blockIdx.y; y < h; y += gridDim.y) {
+        unsigned b, g, r;
+        bayer_bgr(m, w, h, enc, x, y, b, g, r);
+        unsigned char* o = bgr + ((size_t)y * w + x) * 3;
+        o[0] = (unsigned char)b; o[1] = (unsigned char)g; o[2] = (unsigned char)r;
+    }
+}
+
+// flb_image_upload_msg's frames with an odd side (w in {2W, 2W + 1}, h in {2H, 2H + 1}): cv::resize(0.5,
+// INTER_LINEAR)'s fixed-point linear rule (linear_tap, linear_v) of the dense w x h frame `raw` in packed encoding ENC,
+// then cvtColor, into the camera-size colour frame and gray image as k_image_prep writes them.  A thread per output
+// pixel; rows stride by gridDim.y.
+template <int ENC>
+__global__ void __launch_bounds__(128) k_image_resize_linear(const unsigned char* __restrict__ raw, int w, int h, int W, int H, int rule,
+                                                             unsigned char* __restrict__ bgr, unsigned char* __restrict__ gray) {
+    constexpr int P = enc_bpp(ENC);
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= W) return;
+    const LinearTap tx = linear_tap(x, W, w);
+    const int x1 = min(tx.o + 1, w - 1);
+    for (int y = blockIdx.y; y < H; y += gridDim.y) {
+        const LinearTap ty = linear_tap(y, H, h);
+        const unsigned char* r0 = raw + (size_t)ty.o * w * P;
+        const unsigned char* r1 = raw + (size_t)min(ty.o + 1, h - 1) * w * P;
+        unsigned c[3];
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) {
+            const int k = enc_byte(ENC, ch);
+            const int s0 = r0[tx.o * P + k] * tx.a0 + r0[x1 * P + k] * tx.a1;
+            const int s1 = r1[tx.o * P + k] * tx.a0 + r1[x1 * P + k] * tx.a1;
+            c[ch] = linear_v(s0, s1, ty.a0, ty.a1);
+        }
+        unsigned char* o = bgr + ((size_t)y * W + x) * 3;
+        o[0] = (unsigned char)c[0]; o[1] = (unsigned char)c[1]; o[2] = (unsigned char)c[2];
+        gray[(size_t)y * W + x] = (unsigned char)bgr_to_gray(c[0], c[1], c[2], rule);
     }
 }
 

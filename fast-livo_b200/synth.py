@@ -662,6 +662,35 @@ def make_feature_scan(kind, seed=1, n_scans=None, n_cols=None, point_filter_num=
 
 
 # ---------------------------------------------------------------------------------------------------------
+# Camera messages (flb_image_upload_msg): the synthetic texture as a driver in another encoding would send it
+# ---------------------------------------------------------------------------------------------------------
+BAYER_TILES = {"bayer_rggb8": "RGGB", "bayer_bggr8": "BGGR", "bayer_gbrg8": "GBRG", "bayer_grbg8": "GRBG"}
+
+
+def texture_bgr(image: np.ndarray, width: int, height: int) -> np.ndarray:
+    """A width x height BGR8 frame of a gray texture: three distinct channels, the texture repeated to cover the size
+    (twice the camera's, give or take one pixel, is what a full-resolution camera sends)."""
+    bgr = np.stack([image, np.roll(image, 3, 1), 255 - image], -1)
+    reps = (-(-height // bgr.shape[0]), -(-width // bgr.shape[1]), 1)
+    return np.ascontiguousarray(np.tile(bgr, reps)[:height, :width])
+
+
+def mono_message(bgr: np.ndarray) -> np.ndarray:
+    """A mono8 camera's frame of the same scene: the green channel, (h, w) uint8."""
+    return np.ascontiguousarray(bgr[..., 1])
+
+
+def bayer_message(bgr: np.ndarray, encoding: str = "bayer_rggb8") -> np.ndarray:
+    """The (h, w) uint8 mosaic a camera with that colour-filter tile records of a BGR frame: each site keeps the
+    channel of its filter colour; the tile is named from its top-left site (ROS image_encodings)."""
+    tile = BAYER_TILES[encoding]
+    m = np.empty(bgr.shape[:2], np.uint8)
+    for k, c in enumerate(tile):
+        m[k // 2::2, k % 2::2] = bgr[k // 2::2, k % 2::2, "BGR".index(c)]
+    return m
+
+
+# ---------------------------------------------------------------------------------------------------------
 # Visual-map sequences (SURVEY.md section 8 rows f2 / f4): several frames of ONE scene along a short trajectory
 # ---------------------------------------------------------------------------------------------------------
 def voxel_centroids(xyz: np.ndarray, leaf: float) -> np.ndarray:

@@ -486,6 +486,34 @@ int flb_image_upload(flb_handle* h, const uint8_t* gray, int width, int height, 
 #define FLB_GRAY_CV4 0   /* (3735 B + 19235 G + 9798 R + 2^14) >> 15: OpenCV 4.x */
 #define FLB_GRAY_CV3 1   /* (1868 B + 9617 G + 4899 R + 2^13) >> 14: OpenCV 3.x  */
 int flb_image_upload_bgr(flb_handle* h, const uint8_t* bgr, int width, int height, int stride_bytes, int gray_rule);
+/* The camera message as the driver delivers it (sensor_msgs::Image: data, width, height, step, encoding): what
+ * flb_image_upload_bgr does with cv_bridge::toCvCopy(msg, "bgr8")->image (getImageFromMsg, src/laserMapping.cpp:
+ * 490-493), with the colour conversion on the device, so the host neither converts nor demosaics the frame and the
+ * upload carries the message's own bytes per pixel.  The current image set then holds the camera-size colour frame
+ * (img_rgb) and its gray image exactly as after flb_image_upload_bgr, and every reader works unchanged.
+ *   encoding: FLB_ENC_*.  Packed encodings are byte permutations to BGR (mono8 repeats its byte, the alpha byte is
+ *   dropped).  Bayer encodings are cv_bridge's bilinear demosaic (the OpenCV code beside each).
+ *   (width, height): the size rule of detect()'s cv::resize(Size(cols * 0.5, rows * 0.5), INTER_LINEAR):
+ *     the camera's size: no resize;  exactly twice it: the 2x2 area mean of flb_image_upload_bgr;
+ *     2W or 2W + 1 by 2H or 2H + 1 with an odd side: OpenCV 4's fixed-point linear resize, 11-bit weights.  That rule
+ *     is defined for FLB_GRAY_CV4 only: OpenCV 3's rounding there depends on its SIMD path, so FLB_GRAY_CV3 refuses it.
+ *   step_bytes >= width * the encoding's bytes per pixel.
+ * FLB_ENC_BGR8 at the camera's size or twice it is flb_image_upload_bgr, byte for byte.  Copy semantics, streams and
+ * FLB_ERR_STATE as flb_image_upload_bgr.  FLB_ERR_INVALID: data NULL, an unknown encoding or gray_rule, any other size,
+ * step_bytes too small, FLB_GRAY_CV3 with an odd side.  On any error the previous image set stays current and
+ * unchanged.
+ * Not handled: 16-bit encodings, YUV 4:2:2, sensor_msgs::CompressedImage (JPEG / PNG), and display_keypatch's drawing
+ * on img_cp (src/lidar_selection.cpp), which stays on the host. */
+#define FLB_ENC_BGR8        0
+#define FLB_ENC_RGB8        1
+#define FLB_ENC_MONO8       2
+#define FLB_ENC_BGRA8       3
+#define FLB_ENC_RGBA8       4
+#define FLB_ENC_BAYER_RGGB8 5   /* cv_bridge: COLOR_BayerBG2BGR */
+#define FLB_ENC_BAYER_BGGR8 6   /* COLOR_BayerRG2BGR */
+#define FLB_ENC_BAYER_GBRG8 7   /* COLOR_BayerGR2BGR */
+#define FLB_ENC_BAYER_GRBG8 8   /* COLOR_BayerGB2BGR */
+int flb_image_upload_msg(flb_handle* h, const uint8_t* data, int width, int height, int step_bytes, int encoding, int gray_rule);
 /* test / debugging aid (blocking): the current image set's gray (W*H) and colour (W*H*3) frames; either pointer may be
  * NULL.  capacity_pixels >= W*H when either is given.  *width / *height (may be NULL) = W, H.  FLB_ERR_STATE: no image
  * yet, or bgr != NULL for an image from flb_image_upload. */
