@@ -25,6 +25,8 @@
 //        LidarSelector::detect  src/lidar_selection.cpp:1029-1037  (one BGR upload; the gray image is made on the device)
 //   flb::upload_camera_msg(h, msg, gray_rule)   the same from the sensor_msgs::Image itself, replacing getImageFromMsg
 //        (src/laserMapping.cpp:490-493): mono8, rgb8, bgra8, rgba8 and Bayer frames are converted on the device
+//   flb::display_keypatch(h, img_cp, time)   replaces LidarSelector::display_keypatch (src/lidar_selection.cpp:985-1005):
+//        the circles are drawn on the device into img_cp, only the "N HZ" text on the host
 //   flb::preprocess(h, livox_msg, n_scans, blind, point_filter_num)  /  flb::preprocess(h, pc2_msg, kind, n_scans, blind,
 //        point_filter_num)   replace p_pre->process (src/preprocess.cpp:43-70) and the sort of sync_packages
 //        (src/laserMapping.cpp:551): the driver's records go up as they are; the cloud is decoded and sorted on the device
@@ -265,6 +267,30 @@ inline void upload_camera_msg(flb_handle* h, const ImageMsg& msg, int gray_rule)
     const int enc = camera_encoding(msg.encoding);
     check(h, flb_image_upload_msg(h, msg.data.data(), (int)msg.width, (int)msg.height, (int)msg.step, enc, gray_rule));
 }
+
+// ---- display_keypatch (src/lidar_selection.cpp:985-1005) on the device ---------------------------------------------
+// Mat: cv::Mat-like camera-size CV_8UC3 (.data, .cols, .rows, .step), img_cp.  The device draws the circles of the current
+// patch list into it (flb_keypatch_image, the pose the VIO update left on the device); a page-locked img_cp (its data
+// from flb_host_alloc) is filled by the copy engine in place.  When there are patches, put_text(img_cp, text, x, y)
+// draws the rate as :1000-1004 do (text = to_string(int(1 / time)) + " HZ" at (20, 20)); with none, display_keypatch
+// returns before its text and so does this.  Returns the patch count.
+template <class Mat, class PutText>
+inline int display_keypatch(flb_handle* h, Mat& img_cp, double time, PutText put_text) {
+    int n = 0;
+    check(h, flb_keypatch_image(h, nullptr, nullptr, img_cp.data, (int)img_cp.step, &n));
+    check(h, flb_synchronize(h));                     // the bytes of a page-locked img_cp land with the stream
+    if (n == 0) return 0;                             // :987-988
+    put_text(img_cp, std::to_string(int(1 / time)) + " HZ", 20.0f, 20.0f);
+    return n;
+}
+#if defined(CV_VERSION_MAJOR)
+// With OpenCV included first: the reference's own putText (:1003).
+inline int display_keypatch(flb_handle* h, cv::Mat& img_cp, double time) {
+    return display_keypatch(h, img_cp, time, [](cv::Mat& img, const std::string& text, float x, float y) {
+        cv::putText(img, text, cv::Point2f(x, y), cv::FONT_HERSHEY_COMPLEX, 0.6, cv::Scalar(255, 255, 255), 1, 8, 0);
+    });
+}
+#endif
 
 template <class Image, class SubMap, class StatesGroup>
 inline flb_vio_report compute_j(flb_handle* h, const flb_vio_params& prm, const Image& img, SubMap& sub_sparse_map,

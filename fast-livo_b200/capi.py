@@ -205,7 +205,8 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset",
            "flb_image_upload_bgr", "flb_image_download",
            "flb_lidar_upload", "flb_lidar_download", "flb_imu_undistort_lidar", "flb_lidar_upload_velodyne",
-           "flb_lidar_upload_features", "flb_lidar_upload_velodyne_features", "flb_image_upload_msg"]
+           "flb_lidar_upload_features", "flb_lidar_upload_velodyne_features", "flb_image_upload_msg",
+           "flb_keypatch_image"]
 
 
 def lib_path() -> str:
@@ -274,6 +275,7 @@ def lib():
         L.flb_image_upload.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int]
         L.flb_image_upload_bgr.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int]
         L.flb_image_upload_msg.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+        L.flb_keypatch_image.argtypes = [vp, vp, vp, vp, C.c_int, C.POINTER(C.c_int)]
         L.flb_image_download.argtypes = [vp, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
         L.flb_patches_upload.argtypes = [vp, vp, vp, vp, C.c_int]
         L.flb_camera_set.argtypes = [vp, C.POINTER(Camera)]
@@ -767,6 +769,20 @@ class Handle:
         val = np.zeros(self._wc_n, np.uint8)
         self._ck(self.L.flb_colorize_cloud(self.h, pr, pp, _p(img), 0 if img is None else img.shape[1] * 3, _p(rgb), _p(val)))
         return rgb, val.astype(bool)
+
+    def keypatch_image(self, Rcw=None, Pcw=None, out=None):
+        """flb_keypatch_image: (frame (H, W, 3) uint8, patch count) -- the current colour frame with display_keypatch's
+        circles.  Rcw / Pcw None: the pose from the device state.  out: a (H, W, 3) uint8 array to write into (rows may
+        be strided); a page-locked one (pinned_like) makes the call enqueue-only, its bytes valid after synchronize()."""
+        R, P, pr, pp = self._pose(Rcw, Pcw)
+        if out is None:
+            W, H = getattr(self, "_cam_wh", (0, 0))
+            out = np.zeros((H, W, 3), np.uint8)
+        if out.dtype != np.uint8 or out.ndim != 3 or out.strides[1:] != (3, 1):
+            raise ValueError("keypatch_image: out must be (H, W, 3) uint8 with packed pixels")
+        n = C.c_int(-1)
+        self._ck(self.L.flb_keypatch_image(self.h, pr, pp, _p(out), out.strides[0], C.byref(n)))
+        return out, n.value
 
     def vmap_counts(self):
         v = [C.c_int() for _ in range(5)]

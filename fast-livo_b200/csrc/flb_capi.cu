@@ -358,6 +358,12 @@ struct flb_handle {
         Staging st_pg;
     } vm;
     bool pn_on_device = false;   // the patch list was built on the device (flb_vmap_select without a count readback)
+    bool patches_set = false;    // a patch list exists (flb_patches_upload or a visual-map selection)
+    // sub_sparse_map->errors still holds the selection's errors (vm.sel_error, :576): no VIO pass has run on the list
+    bool err_from_sel = false;
+    // flb_keypatch_image: the owner of each pixel (W x H) and the annotated frame (W x H x 3)
+    DevBuf<int> kp_owner;
+    DevBuf<unsigned char> kp_out;
 
     // batched frames (SURVEY.md section 7 H2(iv)): B independent frames per launch, all against the handle's map
     struct Batch {
@@ -896,6 +902,7 @@ int enqueue_vio_update(flb_handle* h, const flb_vio_params* prm) {
         k_vio_begin<<<1, 32, 0, h->stream>>>(h->vio_ctrl.p, h->Pn);
         FLB_CUDA(h, cudaGetLastError());
     }
+    if (prm->max_iteration > 0) h->err_from_sel = false;        // the passes below write sub_sparse_map->errors (:851)
     VioArgs a{};
     a.img = h->img.p;
     a.cam = h->cam;
@@ -1133,7 +1140,7 @@ int flb_destroy(flb_handle* h) {
     h->x_nn_idx.release(); h->x_rowmask.release(); h->x_rows.release(); h->x_meas.release(); h->partials.release();
     h->packed.release(); h->pose12.release(); h->prior.release(); h->scan_raw.release(); h->skeys.release(); h->skeys_sorted.release(); h->svals.release(); h->svals_sorted.release(); h->x_pabcd.release(); h->G_last.release(); h->states.release();
     h->lio_ctrl.release(); h->vio_ctrl.release(); h->ik_states.release(); h->ik_ctrl.release(); h->barrier.release(); h->pkt.release(); h->arrive_lines.release(); h->trace.release(); h->dbg.release(); h->dbg_vio.release(); h->imu_buf.release(); h->imu_pts.release(); h->imu_heads.release(); h->vm_key.release(); h->vm_val.release(); h->vm_pts.release(); h->vm_win.release(); h->vm_pose.release(); h->img.release(); h->img_bgr.release(); h->img_bgr_alt.release(); h->img_raw.release(); h->patch_pos.release(); h->patch_ref.release();
-    h->patch_level.release(); h->errors.release(); h->err_units.release(); h->errors_all.release(); h->x_z.release(); h->x_H.release();
+    h->patch_level.release(); h->kp_owner.release(); h->kp_out.release(); h->errors.release(); h->err_units.release(); h->errors_all.release(); h->x_z.release(); h->x_H.release();
     h->st_map.release(); h->st_scan.release(); h->st_img.release(); h->st_patch.release(); h->st_state.release();
     h->st_misc.release(); h->pin_out.release();
     for (int k = 0; k < 2; ++k) { h->pin_res[k].release(); if (h->ev_res[k]) cudaEventDestroy(h->ev_res[k]); }
@@ -3320,6 +3327,8 @@ int flb_patches_upload(flb_handle* h, const double* pos, const float* patch, con
     FLB_CUDA(h, cudaMemsetAsync(h->errors.p, 0, h->errors.cap * sizeof(float), h->stream));
     h->Pn = Pn;
     h->pn_on_device = false;
+    h->patches_set = true;
+    h->err_from_sel = false;
     h->last_vio_valid = false;
     return FLB_OK;
 }
@@ -3412,6 +3421,7 @@ int flb_vio_pass(flb_handle* h, const flb_vio_params* prm, const double R[9], co
     for (size_t i = 0; i < Pn; ++i) e = e + pe[i];
     out->error = e / (float)(size_t)out->n_meas;
     h->last_vio_valid = true;
+    h->err_from_sel = false;
     return FLB_OK;
 }
 
@@ -3492,6 +3502,7 @@ int flb_vio_update_level(flb_handle* h, const flb_vio_params* prm, int level, fl
         k_vio_begin_level<<<1, 32, 0, h->stream>>>(h->vio_ctrl.p, h->Pn, level, total_residual);
         FLB_CUDA(h, cudaGetLastError());
     }
+    if (prm->max_iteration > 0) h->err_from_sel = false;
     const int nb = vio_nblocks(h);
     for (int it = 0; it < std::max(prm->max_iteration, 0); ++it) {      // later launches return at once when the level has ended
         {
@@ -4182,6 +4193,8 @@ int vm_select_dev(flb_handle* h, const float* pg_down, int n, const int* n_dev, 
     }
     { int rcq = vio_inputs_release(h); if (rcq) return rcq; }
     h->pn_on_device = true;
+    h->patches_set = true;
+    h->err_from_sel = true;
     h->Pn = L;
     h->last_vio_valid = false;
     if (n_selected) {
@@ -4433,6 +4446,46 @@ int flb_colorize_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], 
     if (n == 0) return FLB_OK;
     { int rc = colorize_pose(h, "flb_colorize_cloud", Rcw, Pcw); if (rc) return rc; }
     return colorize_dev(h, bgr, stride_bytes, h->wc_xyz.p, n, rgb, valid);
+}
+
+// LidarSelector::display_keypatch (src/lidar_selection.cpp:985-1005) without its text, into a copy of the current colour
+// frame: k_kp_stamp marks each pixel with the highest patch index whose disk covers it, k_kp_compose colours it.
+int flb_keypatch_image(flb_handle* h, const double Rcw[9], const double Pcw[3], uint8_t* bgr_out, int stride_bytes, int* n_patches) {
+    FLB_CHECK_H(h);
+    if (!bgr_out || (!Rcw != !Pcw)) return fail(h, FLB_ERR_INVALID, "flb_keypatch_image: bad arguments");
+    if (!h->cam_set) return fail(h, FLB_ERR_STATE, "flb_keypatch_image: flb_camera_set first");
+    const int W = h->cam.width, H = h->cam.height;
+    if (stride_bytes < 3 * W) return fail(h, FLB_ERR_INVALID, "flb_keypatch_image: stride_bytes %d < 3 * %d", stride_bytes, W);
+    { int rc = colorize_frame_check(h, "flb_keypatch_image", nullptr); if (rc) return rc; }
+    if (h->comm || h->p2p.world > 1) return fail(h, FLB_ERR_STATE, "flb_keypatch_image: each rank holds only its shard of the patch list");
+    if (!h->patches_set) return fail(h, FLB_ERR_STATE, "flb_keypatch_image: no patch list (flb_vmap_select* or flb_patches_upload)");
+    { int rc = colorize_pose(h, "flb_keypatch_image", Rcw, Pcw); if (rc) return rc; }
+    const size_t npix = (size_t)W * H;
+    FLB_CUDA(h, h->kp_owner.reserve(npix));
+    FLB_CUDA(h, h->kp_out.reserve(npix * 3));
+    { int rcq = vio_inputs_acquire(h); if (rcq) return rcq; }                      // the colour frame and the patches have landed
+    const int n = h->pn_on_device ? h->vm.prm.length : h->Pn;
+    const int* n_dev = h->pn_on_device ? h->vm.counters.p + VM_N_SEL : nullptr;
+    const float* errors = h->err_from_sel ? h->vm.sel_error.p : h->errors.p;
+    const int* err_half = h->err_from_sel ? nullptr : &h->vio_ctrl.p->err_buf;
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        FLB_CUDA(h, cudaMemsetAsync(h->kp_owner.p, 0xff, npix * sizeof(int), h->stream));
+        if (n > 0)
+            k_kp_stamp<<<(unsigned)(((size_t)n * 32 + 255) / 256), 256, 0, h->stream>>>(h->cam, h->vm.pose.p, h->patch_pos.p, n, n_dev, W, H,
+                                                                                   h->kp_owner.p);
+        k_kp_compose<<<(unsigned)((npix + 255) / 256), 256, 0, h->stream>>>(h->img_bgr.p, h->kp_owner.p, errors, err_half, h->err_stride,
+                                                                            (int)npix, h->kp_out.p);
+        FLB_CUDA(h, cudaGetLastError());
+        if (n > 0) h->launches++;
+    }
+    FLB_CUDA(h, cudaMemcpy2DAsync(bgr_out, stride_bytes, h->kp_out.p, (size_t)W * 3, (size_t)W * 3, H, cudaMemcpyDeviceToHost, h->stream));
+    if (n_patches) {
+        if (n_dev) FLB_CUDA(h, cudaMemcpyAsync(n_patches, n_dev, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        else *n_patches = h->Pn;
+    }
+    if (!is_pinned(bgr_out)) FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    return vio_inputs_release(h);
 }
 
 int flb_vmap_counts(flb_handle* h, int* points, int* features, int* images, int* selected, int* last_added) {

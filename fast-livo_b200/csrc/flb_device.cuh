@@ -2149,4 +2149,38 @@ FLB_HD bool feat_emit_at(const LidarPoint* P, const int* ft_final, const int* rs
     return true;
 }
 
+// ------------------------------------------------------------------ display_keypatch (src/lidar_selection.cpp:985-1005)
+// One pixel coordinate of a circle's centre: cv::Point2f rounds the double to float, cv::circle's cv::Point takes
+// cvRound of that float (half to even, as x86-64's cvtss2si does).  false, and nothing is drawn, for a non-finite
+// coordinate or one that rounds beyond +-2^30: cvRound gives INT_MIN there and OpenCV's clipping overflows, so this
+// is a definition, not the reference's behaviour.  Floats are integers from 2^23 on, so the bound holds for the float.
+FLB_HD bool keypatch_round(double v, int* out) {
+    const float f = (float)v;
+    if (!(fabsf(f) <= 1073741824.f)) return false;
+    *out = (int)rintf(f);
+    return true;
+}
+// The centre of patch position pos: new_frame_->w2c(pos) = world2cam(Rcw * pos + Pcw), then keypatch_round.
+FLB_HD bool keypatch_center(const CamModel& cam, const double* Rcw, const double* Pcw, const double* pos, int* cx, int* cy) {
+    double pf[3], pc[2];
+    se3_apply(Rcw, Pcw, pos, pf);
+    world2cam(cam, pf, pc);
+    return keypatch_round(pc[0], cx) && keypatch_round(pc[1], cy);
+}
+// cv::circle(img, c, 6, colour, FILLED, LINE_8) with no shift: 113 pixels, rows 1 7 9 11 11 11 13 11 11 11 9 7 1 wide
+// (half-widths 6 5 5 5 4 3 0 by |dy|), clipped to the image and nothing else.
+constexpr int kKeypatchRadius = 6;
+FLB_HD bool keypatch_in_disk(int dx, int dy) {
+    const int ax = dx < 0 ? -dx : dx, ay = dy < 0 ? -dy : dy;
+    const int hw = ay == 0 ? 6 : ay <= 3 ? 5 : ay == 4 ? 4 : ay == 5 ? 3 : ay == 6 ? 0 : -1;
+    return ax <= hw;
+}
+// errors[i] < 8000 (float compare): green; otherwise, NaN included, cv::Scalar(255, 0, 0), i.e. blue.  BGR bytes.
+FLB_HD void keypatch_colour(float err, unsigned char* bgr) {
+    const bool green = err < 8000.f;
+    bgr[0] = green ? 0 : 255;
+    bgr[1] = green ? 255 : 0;
+    bgr[2] = 0;
+}
+
 }  // namespace flb

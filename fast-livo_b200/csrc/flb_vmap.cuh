@@ -448,4 +448,39 @@ __global__ void k_vm_colorize(CamModel cam, const double* __restrict__ pose12, c
     valid[i] = ok ? 1 : 0;
 }
 
+// display_keypatch (src/lidar_selection.cpp:985-1005), step 1: one warp per patch (n patches, or *n_dev of at most n)
+// stamps its index into owner (W x H, all -1 before) over its clipped disk.  atomicMax leaves the highest index where
+// disks overlap, which is what drawing in list order leaves, without ordering the warps.
+__global__ void k_kp_stamp(CamModel cam, const double* __restrict__ pose12, const double* __restrict__ pos, int n,
+                           const int* __restrict__ n_dev, int W, int H, int* __restrict__ owner) {
+    const int i = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    const int m = n_dev ? min(*n_dev, n) : n;
+    if (i >= m) return;
+    int cx, cy;
+    if (!keypatch_center(cam, pose12, pose12 + 9, pos + 3 * (size_t)i, &cx, &cy)) return;
+    constexpr int side = 2 * kKeypatchRadius + 1;
+    for (int k = lane; k < side * side; k += 32) {
+        const int dx = k % side - kKeypatchRadius, dy = k / side - kKeypatchRadius;
+        const int x = cx + dx, y = cy + dy;                     // |cx|, |cy| <= 2^30: no overflow
+        if (keypatch_in_disk(dx, dy) && x >= 0 && x < W && y >= 0 && y < H) atomicMax(owner + (size_t)y * W + x, i);
+    }
+}
+
+// Step 2, per pixel: the colour frame where no disk lies, the colour of its owner's error elsewhere.  errors: the
+// selection's errors (err_half == NULL) or the VIO errors, whose half the last executed pass wrote is *err_half.
+__global__ void k_kp_compose(const unsigned char* __restrict__ bgr, const int* __restrict__ owner, const float* __restrict__ errors,
+                             const int* __restrict__ err_half, int err_stride, int npix, unsigned char* __restrict__ out) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= npix) return;
+    const int o = owner[p];
+    unsigned char c[3];
+    if (o < 0) {
+        c[0] = bgr[3 * (size_t)p]; c[1] = bgr[3 * (size_t)p + 1]; c[2] = bgr[3 * (size_t)p + 2];
+    } else {
+        const float* e = errors + (err_half && *err_half == 1 ? (size_t)err_stride : 0);
+        keypatch_colour(e[o], c);
+    }
+    out[3 * (size_t)p] = c[0]; out[3 * (size_t)p + 1] = c[1]; out[3 * (size_t)p + 2] = c[2];
+}
+
 }  // namespace flb

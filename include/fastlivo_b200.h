@@ -502,8 +502,8 @@ int flb_image_upload_bgr(flb_handle* h, const uint8_t* bgr, int width, int heigh
  * FLB_ERR_STATE as flb_image_upload_bgr.  FLB_ERR_INVALID: data NULL, an unknown encoding or gray_rule, any other size,
  * step_bytes too small, FLB_GRAY_CV3 with an odd side.  On any error the previous image set stays current and
  * unchanged.
- * Not handled: 16-bit encodings, YUV 4:2:2, sensor_msgs::CompressedImage (JPEG / PNG), and display_keypatch's drawing
- * on img_cp (src/lidar_selection.cpp), which stays on the host. */
+ * Not handled: 16-bit encodings, YUV 4:2:2 and sensor_msgs::CompressedImage (JPEG / PNG).  display_keypatch's circles
+ * on img_cp are drawn on the device too (flb_keypatch_image); only its "N HZ" text stays on the host. */
 #define FLB_ENC_BGR8        0
 #define FLB_ENC_RGB8        1
 #define FLB_ENC_MONO8       2
@@ -622,6 +622,32 @@ int flb_vmap_select_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3
 int flb_vmap_grow_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], int frame_id);
 int flb_colorize_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, uint8_t* rgb,
                        uint8_t* valid);
+/* LidarSelector::display_keypatch (src/lidar_selection.cpp:985-1005) without its putText: the current image set's
+ * camera-size colour frame (img_cp = img_rgb, :1035-1036) with one filled circle per patch of the current patch list,
+ * written to bgr_out (W x H x 3 BGR8, stride_bytes a row).  The image set's colour frame itself is not modified, so
+ * flb_colorize(_cloud) still read the undrawn img_rgb.  For patch i, in list order:
+ *   centre: cvRound of cv::Point2f(world2cam(Rcw * pos_i + Pcw)) -- the double projection rounded to float, then to
+ *     int half to even; a non-finite coordinate, or one that rounds beyond +-2^30, draws nothing (a definition: OpenCV's
+ *     clipping overflows there);
+ *   shape: cv::circle(img, c, 6, colour, FILLED, LINE_8), the fixed 113-pixel disk, clipped to the image;
+ *   colour: errors[i] < 8000 (float) green (0, 255, 0), otherwise (NaN included) blue (255, 0, 0);
+ *   overlaps: the highest patch index wins, as drawing in list order leaves it.
+ * errors[i] = sub_sparse_map->errors[i] at :995: the errors of the last VIO pass executed on this patch list
+ * (flb_vio_errors' values), or, when no pass has run since a visual-map selection, that selection's errors
+ * (flb_vmap_selected's, :576); zero after flb_patches_upload until a pass runs.
+ * Rcw / Pcw: new_frame_->T_f_w_; NULL for both = from the device state in stream order (after flb_vmap_reset), which
+ * after flb_vio_update_enqueue is the pose ComputeJ leaves (:982).  *n_patches (may be NULL) = the list's length; 0
+ * leaves the frame unchanged (display_keypatch returns before its text).
+ * Completion: bgr_out page-locked (flb_host_alloc): enqueue-only, the bytes are valid after the next synchronising call
+ * (flb_synchronize, flb_state_download); *n_patches too when it is page-locked or the count is on the host (a count an
+ * enqueue-only flb_vmap_select* left on the device is copied into pageable memory before the call returns).  Pageable
+ * bgr_out: blocking.
+ *   FLB_ERR_INVALID: bgr_out NULL, stride_bytes < 3 W, exactly one of Rcw / Pcw NULL.
+ *   FLB_ERR_STATE: no camera; no colour frame of the camera's size (no image, or one from flb_image_upload); after
+ *   flb_comm_init / flb_p2p_attach (each rank holds only its shard of the patch list); no patch list; no pose given and
+ *   no flb_vmap_reset or no device state.
+ * On any error nothing is written. */
+int flb_keypatch_image(flb_handle* h, const double Rcw[9], const double Pcw[3], uint8_t* bgr_out, int stride_bytes, int* n_patches);
 /* Gives back what the reference frees (opt-in; enqueue-only, no host synchronisation).  A Feature is owned by
  * Point::obs_ alone, so it dies when addObservation evicts it (deleteFeatureRef(getFurthestViewObs),
  * src/lidar_selection.cpp:946-950); its keyframe image (Feature::img, :183, :957) dies with the last Feature that refers
