@@ -19,6 +19,8 @@
 //        1398-1399) + upload_scan: feats_undistort stays on the device and becomes the scan there
 //   flb::map_incremental(h, lio_prm, filter_size_map_min)  /  flb::map_incremental(h, lio_prm, R, p, filter_size_map_min)   replace
 //        map_incremental()  src/laserMapping.cpp:692-706  (the uploaded scan into the map, no host transform)
+//   flb::publish_effect_world(h, lio_prm, cloud)  /  flb::publish_effect_world(h, lio_prm, R, p, cloud)   fill the cloud of
+//        publish_effect_world()  src/laserMapping.cpp:871-885  (the last LIO pass's laserCloudOri, transformed on the device)
 //   flb::lasermap_fov_segment(h, cube_len, &kdtree_delete_counter)  /  (h, cube_len, pos_lid, &kdtree_delete_counter)
 //        replace lasermap_fov_segment()  src/laserMapping.cpp:363-421  (local-map cube + box delete on the device)
 //   flb::upload_camera_frame(h, bgr, gray_rule)   replaces the resize / img_rgb / cvtColor lines of
@@ -154,6 +156,43 @@ inline void map_incremental(flb_handle* h, const flb_lio_params& lio_prm, const 
         pv[i] = p(i);
     }
     check(h, flb_map_add_scan(h, &lio_prm, Rm, pv, filter_size_map_min));
+}
+
+// ---- publish_effect_world (src/laserMapping.cpp:871-885) from the last LIO pass on the device -----------------
+// Fills `laserCloudWorld` (a PCL cloud: resize(n) and .points with x, y, z) with laserCloudOri of the last LIO pass
+// (:1588-1600) transformed by RGBpointBodyToWorld; the caller converts and publishes it as before.  Only x, y, z are
+// written: the device holds no intensity.  18-DoF path: at the device state the LIO update left.
+template <class PointCloud>
+inline int effect_cloud_fill(flb_handle* h, int n, PointCloud& cloud) {
+    std::vector<float> xyz((size_t)n * 3);
+    int m = 0;
+    check(h, flb_effect_cloud_download(h, xyz.data(), n, &m));
+    cloud.resize((size_t)n);
+    for (int i = 0; i < n; ++i) {
+        cloud.points[i].x = xyz[3 * (size_t)i];
+        cloud.points[i].y = xyz[3 * (size_t)i + 1];
+        cloud.points[i].z = xyz[3 * (size_t)i + 2];
+    }
+    return n;
+}
+template <class PointCloud>
+inline int publish_effect_world(flb_handle* h, const flb_lio_params& lio_prm, PointCloud& laserCloudWorld) {
+    int n = 0;
+    check(h, flb_effect_cloud(h, &lio_prm, nullptr, nullptr, &n));
+    return effect_cloud_fill(h, n, laserCloudWorld);
+}
+// IKFoM callers: R = state_point.rot.toRotationMatrix(), p = state_point.pos, and lio_prm.R_LI / t_LI from
+// state_point.offset_R_L_I.toRotationMatrix() / offset_T_L_I (make_lio_params), as for map_incremental.
+template <class Mat3, class Vec3, class PointCloud>
+inline int publish_effect_world(flb_handle* h, const flb_lio_params& lio_prm, const Mat3& R, const Vec3& p, PointCloud& laserCloudWorld) {
+    double Rm[9], pv[3];
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) Rm[3 * i + j] = R(i, j);
+        pv[i] = p(i);
+    }
+    int n = 0;
+    check(h, flb_effect_cloud(h, &lio_prm, Rm, pv, &n));
+    return effect_cloud_fill(h, n, laserCloudWorld);
 }
 
 // ---- lasermap_fov_segment (src/laserMapping.cpp:363-421) with the cube on the device ---------------

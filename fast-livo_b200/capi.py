@@ -199,7 +199,7 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_vio_update_level", "flb_state_download_enqueue", "flb_state_download_wait", "flb_frame_enqueue",
            "flb_vmap_reset", "flb_vmap_select", "flb_vmap_selected", "flb_vmap_grow", "flb_vmap_add_observations", "flb_vmap_counts",
            "flb_vmap_map_value", "flb_vmap_dump", "flb_vmap_reclaim", "flb_vmap_usage", "flb_vmap_keyframe", "flb_colorize", "flb_voxel_grid",
-           "flb_world_cloud", "flb_world_cloud_download", "flb_vmap_select_cloud", "flb_vmap_grow_cloud", "flb_colorize_cloud",
+           "flb_world_cloud", "flb_world_cloud_download", "flb_effect_cloud", "flb_effect_cloud_download", "flb_vmap_select_cloud", "flb_vmap_grow_cloud", "flb_colorize_cloud",
            "flb_batch_begin", "flb_batch_set_frame", "flb_batch_state_reset_enqueue", "flb_batch_update_enqueue", "flb_batch_state_download",
            "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
            "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset",
@@ -297,6 +297,8 @@ def lib():
         L.flb_colorize.argtypes = [vp, vp, vp, vp, C.c_int, vp, C.c_int, C.c_int, vp, vp]
         L.flb_world_cloud.argtypes = [vp, C.POINTER(LioParams), vp, vp, C.c_int, C.POINTER(C.c_int)]
         L.flb_world_cloud_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_effect_cloud.argtypes = [vp, C.POINTER(LioParams), vp, vp, C.POINTER(C.c_int)]
+        L.flb_effect_cloud_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
         L.flb_vmap_select_cloud.argtypes = [vp, vp, vp, C.c_float, vp]
         L.flb_vmap_grow_cloud.argtypes = [vp, vp, vp, C.c_int]
         L.flb_colorize_cloud.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp]
@@ -380,6 +382,7 @@ class Handle:
             raise FlbError(rc, self.L.flb_last_error(None).decode())
         self.N = self.M = self.Pn = 0
         self._wc_n = 0                  # points of the world cloud flb_world_cloud last built
+        self._ef_n = 0                  # points of the effect cloud flb_effect_cloud last built
 
     def close(self):
         if getattr(self, "h", None):
@@ -744,6 +747,25 @@ class Handle:
         out = np.zeros((self._wc_n, 3), np.float32)
         n = C.c_int()
         self._ck(self.L.flb_world_cloud_download(self.h, _p(out), len(out), C.byref(n)))
+        return out[:n.value]
+
+    # ---- the last LIO pass's effective points (publish_effect_world) on the device
+    def effect_cloud(self, prm, R=None, p=None):
+        """flb_effect_cloud: laserCloudOri of the last LIO pass at pose (R, p), or at the device state x when both are
+        None; returns its number of points."""
+        R = None if R is None else np.ascontiguousarray(R, np.float64)
+        p = None if p is None else np.ascontiguousarray(p, np.float64)
+        n = C.c_int()
+        self._ef_n = 0
+        self._ck(self.L.flb_effect_cloud(self.h, C.byref(prm) if prm is not None else None, _p(R), _p(p), C.byref(n)))
+        self._ef_n = n.value
+        return n.value
+
+    def effect_cloud_download(self):
+        """flb_effect_cloud_download: the effect cloud (n, 3) float32."""
+        out = np.zeros((self._ef_n, 3), np.float32)
+        n = C.c_int()
+        self._ck(self.L.flb_effect_cloud_download(self.h, _p(out), len(out), C.byref(n)))
         return out[:n.value]
 
     def vmap_select_cloud(self, Rcw, Pcw, leaf=0.2, blocking=True):

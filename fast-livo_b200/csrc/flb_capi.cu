@@ -279,6 +279,18 @@ struct flb_handle {
     DevBuf<unsigned> wc_rec;           // bounds + non-finite record of the transform (kScanRec*)
     int wc_n = -1;
     float wc_lo[3] = {0, 0, 0}, wc_hi[3] = {0, 0, 0};
+    // flb_effect_cloud: laserCloudOri of the last LIO pass.  scan_gen counts scan installs; a pass records the generation
+    // and point count of the set it ran on (ef_gen, ef_N) and is pending until captured.  The set survives one more
+    // install (it becomes scan_alt), not two, nor flb_voxel_grid: then the pass is lost.  The capture keeps the rows'
+    // body points (ef_body, ef_n of them, scan-index order); ef_xyz holds their world transform (ef_wn < 0: none).
+    enum { kEfNone = 0, kEfPending = 1, kEfLost = 2 };
+    long long scan_gen = 0, ef_gen = 0;
+    int ef_state = kEfNone, ef_N = 0, ef_n = 0, ef_wn = -1;
+    DevBuf<float4> ef_scatter, ef_body;
+    DevBuf<unsigned char> ef_flag;
+    DevBuf<int> ef_count;
+    DevBuf<float> ef_xyz;
+    DevBuf<unsigned> ef_rec;
     // flb_vmap_select_cloud: downSizeFilter of the world cloud and its scratch (the scan slot's stays untouched)
     DevBuf<float> wc_down;
     DevBuf<unsigned> wc_keys, wc_keys_sorted;
@@ -709,6 +721,13 @@ int flush_state_ops(flb_handle* h) {
     return FLB_OK;
 }
 
+// A LIO pass was enqueued on the current scan set: its sel bytes (lio_sel_byte) are laserCloudOri until captured.
+void note_lio_pass(flb_handle* h) {
+    h->ef_state = flb_handle::kEfPending;
+    h->ef_gen = h->scan_gen;
+    h->ef_N = h->N;
+}
+
 // Flag base for one persistent launch: flags epoch+1 .. epoch+4095 belong to it alone.  On wrap-around the
 // packet and the arrival lines are cleared (stream-ordered) so that no stale unit can ever match.
 int next_epoch(flb_handle* h, unsigned* epoch) {
@@ -822,6 +841,7 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
         FLB_CUDA(h, cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(kLioPersBlock), args, 0,
                                                 h->stream));
         h->last_pass_valid = false;
+        note_lio_pass(h);
         return FLB_OK;
     }
     {
@@ -846,6 +866,7 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
         FLB_CUDA(h, cudaGetLastError());
     }
     h->last_pass_valid = false;
+    note_lio_pass(h);                    // the passes after the stop pass return at once: its sel bytes stay
     return FLB_OK;
 }
 
@@ -1130,6 +1151,7 @@ int flb_destroy(flb_handle* h) {
     h->add_xyz.release(); h->add_rec.release(); h->fov_rec.release();
     h->wc_xyz.release(); h->wc_rec.release(); h->wc_down.release(); h->wc_keys.release(); h->wc_keys_sorted.release();
     h->wc_vals.release(); h->wc_vals_sorted.release(); h->wc_heads.release(); h->wc_box.release();
+    h->ef_scatter.release(); h->ef_body.release(); h->ef_flag.release(); h->ef_count.release(); h->ef_xyz.release(); h->ef_rec.release();
     h->sf_keys.release(); h->sf_keys_sorted.release(); h->sf_rec.release(); h->sf_vals.release(); h->sf_vals_sorted.release();
     h->sf_heads.release(); h->sf_xyz.release();
     h->cell_table.release(); h->cell_keys.release(); h->cell_keys_alt.release();
@@ -1779,6 +1801,81 @@ int flb_world_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out
     const int m = std::min(capacity, h->wc_n);
     if (m > 0) {
         FLB_CUDA(h, cudaMemcpyAsync(xyz, h->wc_xyz.p, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    }
+    return FLB_OK;
+}
+
+// laserCloudOri of the pending pass into ef_body: the rows of the scan set it ran on (the current one, or scan_alt after
+// one more install), scattered to their caller's index by k_effect_scatter and compacted in that order by cub's select.
+// Runs on `stream` after the pass; the count read ends with a stream synchronise, so a later install cannot overwrite
+// the set under it.
+static int effect_capture(flb_handle* h) {
+    const bool cur = h->scan_gen == h->ef_gen;
+    const float4* scan = cur ? h->scan.p : h->scan_alt.p;
+    const unsigned char* sel = cur ? h->sel.p : h->sel_alt.p;
+    const int N = h->ef_N;
+    int n = 0;
+    if (N > 0) {
+        FLB_CUDA(h, h->ef_scatter.reserve(N));
+        FLB_CUDA(h, h->ef_flag.reserve(N));
+        FLB_CUDA(h, h->ef_body.reserve(N));
+        FLB_CUDA(h, h->ef_count.reserve(1));
+        {
+            LaunchScope ls(h, FAM_OTHER);
+            k_effect_scatter<<<(N + 255) / 256, 256, 0, h->stream>>>(scan, sel, N, h->ef_flag.p, h->ef_scatter.p);
+            FLB_CUDA(h, cudaGetLastError());
+        }
+        size_t tmp_bytes = 0;
+        FLB_CUDA(h, cub::DeviceSelect::Flagged(nullptr, tmp_bytes, h->ef_scatter.p, h->ef_flag.p, h->ef_body.p, h->ef_count.p, N, h->stream));
+        FLB_CUDA(h, h->cub_tmp.reserve(tmp_bytes));
+        FLB_CUDA(h, cub::DeviceSelect::Flagged(h->cub_tmp.p, tmp_bytes, h->ef_scatter.p, h->ef_flag.p, h->ef_body.p, h->ef_count.p, N, h->stream));
+        h->launches++;
+        int* cnt = static_cast<int*>(h->pin_out.p);
+        FLB_CUDA(h, cudaMemcpyAsync(cnt, h->ef_count.p, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+        n = *cnt;
+    }
+    h->ef_n = n;
+    h->ef_state = flb_handle::kEfNone;
+    return FLB_OK;
+}
+
+// publish_effect_world (src/laserMapping.cpp:871-885): laserCloudOri (:1588-1600) of the last LIO pass, transformed
+// by RGBpointBodyToWorld at (R, p) or at the device state x -- scan_to_world, the kernel of flb_world_cloud.
+int flb_effect_cloud(flb_handle* h, const flb_lio_params* prm, const double R[9], const double p[3], int* n_out) {
+    FLB_CHECK_H(h);
+    h->ef_wn = -1;                                    // on any error below, no world cloud is held
+    if (n_out) *n_out = 0;
+    if (!prm || (R == nullptr) != (p == nullptr))
+        return fail(h, FLB_ERR_INVALID, "flb_effect_cloud: bad arguments (prm, R and p both or neither)");
+    if (h->comm || h->p2p.world > 0)
+        return fail(h, FLB_ERR_STATE, "flb_effect_cloud: single GPU only (each rank holds only its shard of the scan)");
+    if (!R && !h->state_valid) return fail(h, FLB_ERR_STATE, "flb_effect_cloud: no pose given and no device state");
+    if (h->ef_state == flb_handle::kEfPending && h->scan_gen - h->ef_gen >= 2) h->ef_state = flb_handle::kEfLost;
+    if (h->ef_state == flb_handle::kEfLost)
+        return fail(h, FLB_ERR_STATE, "flb_effect_cloud: the last LIO pass's scan was replaced (two scan uploads or flb_voxel_grid) before capture");
+    if (h->ef_state == flb_handle::kEfPending) { int rcc = effect_capture(h); if (rcc) return rcc; }
+    const int n = h->ef_n;
+    if (n > 0) {
+        bool bad = false;
+        float lo[3], hi[3];
+        { int rcw = scan_to_world(h, prm, R, p, h->ef_body.p, n, false, h->ef_xyz, h->ef_rec, &bad, lo, hi); if (rcw) return rcw; }
+        if (bad) return fail(h, FLB_ERR_INVALID, "flb_effect_cloud: non-finite coordinate");
+    }
+    h->ef_wn = n;
+    if (n_out) *n_out = n;
+    return FLB_OK;
+}
+
+int flb_effect_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out) {
+    FLB_CHECK_H(h);
+    if (capacity < 0 || (capacity > 0 && !xyz)) return fail(h, FLB_ERR_INVALID, "flb_effect_cloud_download: bad arguments");
+    if (h->ef_wn < 0) return fail(h, FLB_ERR_STATE, "flb_effect_cloud_download: no effect cloud (flb_effect_cloud first, or it failed)");
+    if (n_out) *n_out = h->ef_wn;
+    const int m = std::min(capacity, h->ef_wn);
+    if (m > 0) {
+        FLB_CUDA(h, cudaMemcpyAsync(xyz, h->ef_xyz.p, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
         FLB_CUDA(h, cudaStreamSynchronize(h->stream));
     }
     return FLB_OK;
@@ -2604,6 +2701,7 @@ int flb_voxel_grid(flb_handle* h, const float* xyz, int n, int stride, float lea
     h->N = 0;                                    // the scan slot was used as scratch
     h->scan_valid = false;
     h->last_pass_valid = false;
+    if (h->ef_state == flb_handle::kEfPending) h->ef_state = flb_handle::kEfLost;
     return FLB_OK;
 }
 
@@ -2690,6 +2788,7 @@ static int scan_install_dev(flb_handle* h, const float* xyz, int N, const float 
     h->scan_slot = alt;
     h->N = N;     // enqueue-only: everything later on this handle's stream is ordered after the upload
     h->scan_valid = true;
+    h->scan_gen++;
     h->last_pass_valid = false;
     return FLB_OK;
 }
@@ -2895,6 +2994,7 @@ int flb_lio_pass(flb_handle* h, const flb_lio_params* prm, const double R[9], co
     a.pose_override = h->pose12.p;
     int rc = launch_lio_pass(h, a, width, rematch != 0);
     if (rc) return rc;
+    note_lio_pass(h);
     const int K = lio_packed(width);
     if (h->comm) {
         rc = allreduce_packed(h, h->partials.p, lio_nblocks(h), K);
@@ -3164,6 +3264,7 @@ int flb_lio_update_ikfom(flb_handle* h, const flb_ikfom_params* prm, flb_state_i
                                                 h->stream));
     }
     h->last_pass_valid = false;
+    note_lio_pass(h);                    // the last h_share_model evaluation's sel bytes
     FLB_CUDA(h, h->pin_out.reserve(sizeof(StateIkfom) + sizeof(IkfomCtrl) + sizeof(GridBarrier)));
     char* po = static_cast<char*>(h->pin_out.p);
     FLB_CUDA(h, cudaMemcpyAsync(po, &h->ik_states.p[0], sizeof(StateIkfom), cudaMemcpyDeviceToHost, h->stream));

@@ -294,6 +294,16 @@ FLB_HD bool lio_residual(const float* pabcd, const float* pw, const float* pb, f
     return (double)s > 0.9;
 }
 
+// The per-point byte a LIO pass leaves: bit 0 = point_selected_surf after the pass (:1570-1584), bit 1 = the point is a
+// row of the pass (point_selected_surf[i] && res_last[i] <= 2.0, :1593), i.e. a member of laserCloudOri.  Bit 1 implies
+// bit 0, so `byte != 0` still reads point_selected_surf.  The row test is not implied by s > 0.9: that gate admits
+// |pd2| > 2 for points beyond 324 m (|pd2| < sqrt(|p_body|) / 9).
+constexpr unsigned char kLioSel = 1, kLioRow = 3;
+FLB_HD unsigned char lio_sel_byte(bool sel, float pd2) {
+    return sel ? (((double)fabsf(pd2) <= 2.0) ? kLioRow : kLioSel) : (unsigned char)0;
+}
+FLB_HD bool lio_sel_is_row(unsigned char b) { return b == kLioRow; }
+
 // Live-layout row [A, n], A = [p_I]x * R^T * n   (src/laserMapping.cpp:1611-1625)
 FLB_HD void lio_row6(const LioPose& c, const double* pI, const float* pabcd, double* row) {
     double cross[9], M1[9], A[3];
@@ -428,6 +438,15 @@ FLB_HD int map_scan_point(const LioPose& c, const map_pt& b, float* pw) {
     double pI[3];
     lio_body_to_world(c, pb, pI, pw);
     return (int)float_as_u32(b.w);
+}
+
+// publish_effect_world's capture (flb_effect_cloud), one point of the ordered scan: its row flag (lio_sel_byte) and its
+// body point go to its caller's index (w), so that an order-preserving select over the flags yields laserCloudOri in
+// scan-index order (src/laserMapping.cpp:1588-1600).
+FLB_HD void effect_scatter_point(const map_pt& b, unsigned char sel_byte, unsigned char* flag, map_pt* body) {
+    const int oi = (int)float_as_u32(b.w);
+    flag[oi] = lio_sel_is_row(sel_byte) ? 1 : 0;
+    body[oi] = b;
 }
 
 // Whether all three floats are finite (exponent field not all ones), as flb_map_add_points tests its input.

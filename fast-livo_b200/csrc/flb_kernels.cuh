@@ -461,6 +461,14 @@ __global__ void k_gather_xyz(const float* __restrict__ src, const int* __restric
     dst[3 * (size_t)i + 2] = src[3 * (size_t)s + 2];
 }
 
+// flb_effect_cloud's capture: one thread per point of the ordered scan set the last LIO pass ran on scatters its row
+// flag and body point to its caller's index (effect_scatter_point); cub's order-preserving select compacts them.
+__global__ void __launch_bounds__(256) k_effect_scatter(const float4* __restrict__ scan, const unsigned char* __restrict__ sel, int n,
+                                                        unsigned char* __restrict__ flag, float4* __restrict__ body) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) effect_scatter_point(scan[i], sel[i], flag, body);
+}
+
 // ---------------------------------------------------------------------------------------
 // Incremental Add_Points: only the voxels the NEW points fall into are looked at.  The new points are sorted by
 // downsample voxel; one thread per touched voxel finds the live points of its box through the kNN grid (a box overlaps
@@ -947,7 +955,7 @@ __device__ __forceinline__ void lio_point(const LioArgs& a, const LioPose& pose,
             }
         }
     } else {
-        sel = a.sel[i] != 0;
+        sel = a.sel[i] != 0;                                   // bit 0 (lio_sel_byte)
         pok = a.plane_ok[i] != 0;
         const float4 pl = a.plane[i];
         pabcd[0] = pl.x; pabcd[1] = pl.y; pabcd[2] = pl.z; pabcd[3] = pl.w;
@@ -959,8 +967,9 @@ __device__ __forceinline__ void lio_point(const LioArgs& a, const LioPose& pose,
             if (lio_residual(pabcd, pw, pb, &pd2)) sel = true; // :1573-1584
         }
     }
-    a.sel[i] = sel ? 1 : 0;
-    active = sel && ((double)fabsf(pd2) <= 2.0);               // :1593
+    const unsigned char sb = lio_sel_byte(sel, pd2);           // the pass's row mask survives it (flb_effect_cloud)
+    a.sel[i] = sb;
+    active = lio_sel_is_row(sb);                               // :1593
     if (active) {
         if (W == 6) lio_row6(pose, pI, pabcd, row);
         else lio_row12(pose, pI, pb, pabcd, row);

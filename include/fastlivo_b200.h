@@ -612,6 +612,31 @@ int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const 
 int flb_world_cloud(flb_handle* h, const struct flb_lio_params* prm, const double R[9], const double p[3], int source, int* n_out);
 /* publish_frame_world / the PCD save: up to `capacity` points of the world cloud, xyz floats (blocking). */
 int flb_world_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out);
+
+/* ---- the effective points of the last LIO pass on the device (publish_effect_world) ------------------------------
+ * publish_effect_world (src/laserMapping.cpp:871-885, called at :1776) publishes laserCloudOri -- the body points of the
+ * effective rows point_selected_surf[i] && res_last[i] <= 2.0 of the last iteration the LIO loop ran (:1588-1600) --
+ * transformed by RGBpointBodyToWorld at the state after the update.  Every LIO pass keeps its row mask on the device,
+ * so the cloud costs no extra pass and no read-back of the scan.
+ *   The effect cloud is the rows of the last LIO pass executed on the handle (stream order), in scan-index order
+ * (laserCloudOri's), body x, y, z, transformed at (R, p) with prm->R_LI / prm->t_LI, or at the device state x when
+ * R == p == NULL.  The passes that count: the stop pass of flb_lio_update, flb_lio_update_enqueue and flb_frame_enqueue;
+ * the last h_share_model evaluation of flb_lio_update_ikfom; the pass of flb_lio_pass.  Batched frames (flb_batch_*) do
+ * not touch it.  IKFoM callers pass R = rot, p = pos and the offset_R_L_I / offset_T_L_I extrinsic, as for
+ * flb_world_cloud.
+ *   The first call after a pass captures that pass's rows; with no pass since, the rows captured last are transformed
+ * at the new pose (the reference republishes its stale laserCloudOri when the loop does not run: before flg_EKF_inited,
+ * :1506, or with lidar_en off).  No pass ever: 0 points.  The scan, its row mask and its plane cache are double-buffered
+ * together, so a pass's rows can be captured until the second scan upload after it (or an flb_voxel_grid, which uses
+ * the scan slot as scratch); after that the call returns FLB_ERR_STATE until the next pass.  Intensity is not carried.
+ * Blocking.  *n_out (may be NULL) = points.  On any error no effect cloud is held.
+ *   FLB_ERR_STATE: the pass's rows were replaced before capture, no pose given and no device state, after flb_comm_init
+ *   / flb_p2p_attach (each rank holds only its shard of the scan).
+ *   FLB_ERR_INVALID: prm == NULL, exactly one of R / p NULL, a transformed point that is not finite. */
+int flb_effect_cloud(flb_handle* h, const struct flb_lio_params* prm, const double R[9], const double p[3], int* n_out);
+/* pubLaserCloudEffect's points: up to `capacity` points of the effect cloud, xyz floats (blocking, as
+ * flb_world_cloud_download).  FLB_ERR_INVALID for a bad capacity or buffer, FLB_ERR_STATE when no effect cloud is held. */
+int flb_effect_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out);
 /* flb_vmap_select / flb_vmap_grow / flb_colorize with pg = the world cloud: the same pose, enqueue and blocking rules and
  * byte-identical results to those calls on the host-transformed cloud.  flb_vmap_select_cloud applies downSizeFilter
  * (pcl::VoxelGrid with `leaf`, 0.2 in the reference: src/lidar_selection.cpp:7, :351-353; flb_voxel_grid's result) on
