@@ -863,52 +863,38 @@ class Handle:
         return out, poses[:npo.value]
 
     # ---- the driver's LiDAR message (Preprocess::process, the time sort, UndistortPcl's window)
-    def lidar_upload(self, fmt: LidarFormat, records, n_records=None):
-        """flb_lidar_upload: records = a uint8 array (or bytes) of n_records records of fmt.point_step bytes.  Returns
-        (pl_surf.size(), points.back().curvature after the sort)."""
+    def _lidar_upload(self, fn, fmt, records, n_records, *dis_b, yaw=False):
+        """The four LiDAR uploads' shared binding: records = a uint8 array (or bytes) of n_records records of
+        fmt.point_step bytes (default: all of them).  Returns (n_points, last_offset_ms), and yaw_times as a bool when
+        `yaw`."""
         a = np.frombuffer(records, np.uint8) if isinstance(records, (bytes, bytearray)) else records
         if n_records is None:
             n_records = a.size // max(fmt.point_step, 1)
-        n, last = C.c_int(), C.c_float()
-        self._ck(self.L.flb_lidar_upload(self.h, C.byref(fmt), _p(a) if a.size else None, int(n_records), C.byref(n), C.byref(last)))
+        n, last, yaw_times = C.c_int(), C.c_float(), C.c_int()
+        outs = (C.byref(n), C.byref(last)) + ((C.byref(yaw_times),) if yaw else ())
+        self._ck(fn(self.h, C.byref(fmt), *dis_b, _p(a) if a.size else None, int(n_records), *outs))
         self._lid_n = n.value
-        return n.value, np.float32(last.value)
+        return (n.value, np.float32(last.value)) + ((bool(yaw_times.value),) if yaw else ())
+
+    def lidar_upload(self, fmt: LidarFormat, records, n_records=None):
+        """flb_lidar_upload: records = a uint8 array (or bytes) of n_records records of fmt.point_step bytes.  Returns
+        (pl_surf.size(), points.back().curvature after the sort)."""
+        return self._lidar_upload(self.L.flb_lidar_upload, fmt, records, n_records)
 
     def lidar_upload_velodyne(self, fmt: VelodyneFormat, records, n_records=None):
         """flb_lidar_upload_velodyne: records = a uint8 array (or bytes) of n_records Velodyne records of fmt.point_step
         bytes.  Returns (pl_surf.size(), points.back().curvature after the sort, whether the times came from the yaw)."""
-        a = np.frombuffer(records, np.uint8) if isinstance(records, (bytes, bytearray)) else records
-        if n_records is None:
-            n_records = a.size // max(fmt.point_step, 1)
-        n, last, yaw = C.c_int(), C.c_float(), C.c_int()
-        self._ck(self.L.flb_lidar_upload_velodyne(self.h, C.byref(fmt), _p(a) if a.size else None, int(n_records), C.byref(n),
-                                                  C.byref(last), C.byref(yaw)))
-        self._lid_n = n.value
-        return n.value, np.float32(last.value), bool(yaw.value)
+        return self._lidar_upload(self.L.flb_lidar_upload_velodyne, fmt, records, n_records, yaw=True)
 
     def lidar_upload_features(self, fmt: LidarFormat, records, dis_b=0.0, n_records=None):
         """flb_lidar_upload_features (feature_extract_enable: 1) for a Livox or Ouster message; fmt.off_line is the Livox
         line or the Ouster's u8 ring.  Returns (pl_surf.size(), points.back().curvature after the sort)."""
-        a = np.frombuffer(records, np.uint8) if isinstance(records, (bytes, bytearray)) else records
-        if n_records is None:
-            n_records = a.size // max(fmt.point_step, 1)
-        n, last = C.c_int(), C.c_float()
-        self._ck(self.L.flb_lidar_upload_features(self.h, C.byref(fmt), float(dis_b), _p(a) if a.size else None, int(n_records),
-                                                  C.byref(n), C.byref(last)))
-        self._lid_n = n.value
-        return n.value, np.float32(last.value)
+        return self._lidar_upload(self.L.flb_lidar_upload_features, fmt, records, n_records, float(dis_b))
 
     def lidar_upload_velodyne_features(self, fmt: VelodyneFormat, records, dis_b=0.0, n_records=None):
         """flb_lidar_upload_velodyne_features (feature_extract_enable: 1).  Returns (pl_surf.size(),
         points.back().curvature after the sort, whether the times came from the yaw)."""
-        a = np.frombuffer(records, np.uint8) if isinstance(records, (bytes, bytearray)) else records
-        if n_records is None:
-            n_records = a.size // max(fmt.point_step, 1)
-        n, last, yaw = C.c_int(), C.c_float(), C.c_int()
-        self._ck(self.L.flb_lidar_upload_velodyne_features(self.h, C.byref(fmt), float(dis_b), _p(a) if a.size else None,
-                                                           int(n_records), C.byref(n), C.byref(last), C.byref(yaw)))
-        self._lid_n = n.value
-        return n.value, np.float32(last.value), bool(yaw.value)
+        return self._lidar_upload(self.L.flb_lidar_upload_velodyne_features, fmt, records, n_records, float(dis_b), yaw=True)
 
     def lidar_download(self):
         """flb_lidar_download: the decoded, time-sorted cloud, (n, 4) float32 x, y, z, curvature."""

@@ -2100,54 +2100,80 @@ namespace {
 int lidar_time_bytes(int kind) { return kind == kLidarXt32 ? 8 : 4; }
 
 bool lidar_field_ok(int off, int bytes, int step) { return off >= 0 && off % bytes == 0 && off + bytes <= step; }
+// Velodyne drivers place their fields anywhere, so no alignment is asked of them
+bool velo_field_ok(int off, int bytes, int step) { return off >= 0 && off <= step - bytes; }
+
+// flb_lidar_format -> LidarFmt, the checks in the order flb_lidar_upload and (features) flb_lidar_upload_features
+// report them.  The features call also checks dis_b, refuses the Velodyne and the XT32 (so its time field is 4 bytes),
+// caps n_scans at pl_buff's 128, and always reads off_line: the Livox line or the Ouster's ring.
+int lidar_format(flb_handle* h, const char* who, const flb_lidar_format* fmt, const void* records, int n_records, bool features,
+                 double dis_b, LidarFmt* f) {
+    if (n_records < 0 || !fmt || (n_records > 0 && !records) || (features && !std::isfinite(dis_b)))
+        return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
+    if (features && (fmt->kind == kLidarVelodyne || fmt->kind == kLidarXt32))
+        return fail(h, FLB_ERR_INVALID, "%s: kind %d: a Velodyne cloud goes to flb_lidar_upload_velodyne_features; the XT32 "
+                    "has no feature branch (src/preprocess.cpp:432-464), so flb_lidar_upload serves it", who, fmt->kind);
+    if (fmt->kind < kLidarLivox || fmt->kind > kLidarXt32) return fail(h, FLB_ERR_INVALID, "%s: unknown kind %d", who, fmt->kind);
+    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || (features && fmt->n_scans > 128) || !std::isfinite(fmt->blind))
+        return fail(h, FLB_ERR_INVALID, "%s: point_filter_num %d, n_scans %d%s, blind %g", who, fmt->point_filter_num,
+                    fmt->n_scans, features ? " (1..128: pl_buff[128])" : "", fmt->blind);
+    const int step = fmt->point_step;
+    const bool livox = fmt->kind == kLidarLivox, line = livox || features;
+    if (step < 1 || !lidar_field_ok(fmt->off_x, 4, step) || !lidar_field_ok(fmt->off_y, 4, step) || !lidar_field_ok(fmt->off_z, 4, step) ||
+        !lidar_field_ok(fmt->off_time, lidar_time_bytes(fmt->kind), step) || (line && !lidar_field_ok(fmt->off_line, 1, step)) ||
+        (livox && !lidar_field_ok(fmt->off_tag, 1, step)))
+        return fail(h, FLB_ERR_INVALID, "%s: a field does not fit in point_step %d or is not aligned to its type", who, step);
+    *f = LidarFmt{};
+    f->kind = fmt->kind, f->step = step, f->off_x = fmt->off_x, f->off_y = fmt->off_y, f->off_z = fmt->off_z, f->off_time = fmt->off_time;
+    f->off_tag = livox ? fmt->off_tag : 0, f->off_line = line ? fmt->off_line : 0;
+    f->n_scans = fmt->n_scans, f->filter_num = fmt->point_filter_num, f->blind = fmt->blind;
+    return FLB_OK;
+}
+
+// flb_velodyne_format -> LidarFmt for flb_lidar_upload_velodyne and (features) flb_lidar_upload_velodyne_features, which
+// also checks dis_b, caps n_scans at pl_buff's 128 and reads the ring as the line.  *given: given_offset_time (:279), the
+// last record's time > 0; without a time field the reference reads 0.
+int velo_format(flb_handle* h, const char* who, const flb_velodyne_format* fmt, const void* records, int n_records, bool features,
+                double dis_b, LidarFmt* f, bool* given) {
+    if (n_records < 0 || !fmt || (n_records > 0 && !records) || (features && !std::isfinite(dis_b)))
+        return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
+    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || (features && fmt->n_scans > 128) || !std::isfinite(fmt->blind))
+        return fail(h, FLB_ERR_INVALID, "%s: point_filter_num %d, n_scans %d%s, blind %g", who, fmt->point_filter_num,
+                    fmt->n_scans, features ? " (1..128: pl_buff[128])" : "", fmt->blind);
+    const int step = fmt->point_step;
+    if (step < 1 || !velo_field_ok(fmt->off_x, 4, step) || !velo_field_ok(fmt->off_y, 4, step) || !velo_field_ok(fmt->off_z, 4, step) ||
+        !velo_field_ok(fmt->off_ring, 2, step) || (fmt->off_time != -1 && !velo_field_ok(fmt->off_time, 4, step)))
+        return fail(h, FLB_ERR_INVALID, "%s: a field does not fit in point_step %d", who, step);
+    *f = LidarFmt{};
+    f->kind = kLidarVelodyne, f->step = step, f->off_x = fmt->off_x, f->off_y = fmt->off_y, f->off_z = fmt->off_z;
+    f->off_time = fmt->off_time >= 0 ? fmt->off_time : 0, f->off_line = features ? fmt->off_ring : 0;
+    f->n_scans = fmt->n_scans, f->filter_num = fmt->point_filter_num, f->blind = fmt->blind;
+    *given = n_records == 0;
+    if (n_records > 0 && fmt->off_time >= 0) {
+        float t_last;
+        std::memcpy(&t_last, static_cast<const unsigned char*>(records) + (size_t)(n_records - 1) * step + fmt->off_time, sizeof(t_last));
+        *given = t_last > 0;
+    }
+    return FLB_OK;
+}
 
 struct VeloYaw { int off_ring, n_scans; };      // flb_lidar_upload_velodyne's route without per-point times
 
-int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const void* records, int n_records, const VeloYaw* yaw,
-                      int* n_points, float* last_offset_ms);
+// lid_flags as every route lays it out (3 * n1 + 8 ints): n1 ints of the route's own, kept[n1], pos[n1], the
+// LidarRecord, and one int of the route's own right after it (the yaw route's bad ring, the features' point count)
+struct LidarFlags {
+    int *own, *kept, *pos;
+    LidarRecord* rec;
+    int* after;
+    LidarFlags(int* p, size_t n1)
+        : own(p), kept(p + n1), pos(p + 2 * n1), rec(reinterpret_cast<LidarRecord*>(p + 3 * n1)), after(reinterpret_cast<int*>(rec + 1)) {}
+};
+static_assert(sizeof(LidarRecord) == 4 * sizeof(int), "LidarRecord sits in lid_flags");
 
-}  // namespace
-
-int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* records, int n_records, int* n_points,
-                     float* last_offset_ms) {
-    FLB_CHECK_H(h);
-    if (n_records < 0 || !fmt || (n_records > 0 && !records)) return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: bad arguments");
-    if (fmt->kind < kLidarLivox || fmt->kind > kLidarXt32) return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: unknown kind %d", fmt->kind);
-    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || !std::isfinite(fmt->blind))
-        return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: point_filter_num %d, n_scans %d, blind %g", fmt->point_filter_num,
-                    fmt->n_scans, fmt->blind);
-    const int step = fmt->point_step;
-    const bool livox = fmt->kind == kLidarLivox;
-    if (step < 1 || !lidar_field_ok(fmt->off_x, 4, step) || !lidar_field_ok(fmt->off_y, 4, step) || !lidar_field_ok(fmt->off_z, 4, step) ||
-        !lidar_field_ok(fmt->off_time, lidar_time_bytes(fmt->kind), step) ||
-        (livox && (!lidar_field_ok(fmt->off_tag, 1, step) || !lidar_field_ok(fmt->off_line, 1, step))))
-        return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: a field does not fit in point_step %d or is not aligned to its type", step);
-    LidarFmt f{};
-    f.kind = fmt->kind, f.step = step, f.off_x = fmt->off_x, f.off_y = fmt->off_y, f.off_z = fmt->off_z, f.off_time = fmt->off_time;
-    f.off_tag = livox ? fmt->off_tag : 0, f.off_line = livox ? fmt->off_line : 0;
-    f.n_scans = fmt->n_scans, f.filter_num = fmt->point_filter_num, f.blind = fmt->blind;
-    const unsigned char* rec_h = static_cast<const unsigned char*>(records);
-    if (n_records > 0 && fmt->kind == kLidarVelodyne) {
-        float t_last;                                                              // given_offset_time, :279
-        std::memcpy(&t_last, rec_h + (size_t)(n_records - 1) * step + f.off_time, sizeof(t_last));
-        if (!(t_last > 0))
-            return fail(h, FLB_ERR_INVALID, "flb_lidar_upload: a Velodyne cloud without per-point times (last time %g): its times "
-                        "come from the yaw angle (src/preprocess.cpp:389-419), which flb_lidar_upload_velodyne derives", (double)t_last);
-    }
-    if (n_records > 0 && fmt->kind == kLidarXt32) std::memcpy(&f.time_head, rec_h + f.off_time, sizeof(double));   // :441
-    return lidar_upload_core(h, "flb_lidar_upload", f, records, n_records, nullptr, n_points, last_offset_ms);
-}
-
-namespace {
-
-// flb_lidar_upload and flb_lidar_upload_velodyne from the argument checks on: decode, filter, compact and time-sort the
-// records into the idle cloud set, and swap it in.  yaw: the Velodyne route without per-point times; nullptr: the
-// handler's own per-record times.
-int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const void* records, int n_records, const VeloYaw* yaw,
-                      int* n_points, float* last_offset_ms) {
-    const int step = f.step;
-    const bool livox = f.kind == kLidarLivox;
-    const size_t n = (size_t)n_records, n1 = std::max<size_t>(n, 1), raw_bytes = n * step;
+// Every route's start: reserve what all routes write, send the raw records to lid_raw on copy_stream (a page-locked
+// source read in place), then wait for the idle cloud set's readers: only the kernels that write that set wait.
+int lidar_begin(flb_handle* h, const void* records, int n_records, int step) {
+    const size_t n1 = std::max(n_records, 1), raw_bytes = (size_t)n_records * step;
     FLB_CUDA(h, h->lid_raw.reserve(std::max<size_t>(raw_bytes, 4)));
     FLB_CUDA(h, h->lid_cloud_alt.reserve(n1));
     FLB_CUDA(h, h->lid_dec.reserve(n1));
@@ -2157,13 +2183,6 @@ int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const v
     FLB_CUDA(h, h->lid_flags.reserve(3 * n1 + 8));
     FLB_CUDA(h, h->pin_lidar.reserve(64));
     cudaStream_t cs = h->copy_stream;
-    int* d_vnum = h->lid_flags.p;
-    int* d_kept = d_vnum + n1;
-    int* d_pos = d_kept + n1;
-    LidarRecord* d_rec = reinterpret_cast<LidarRecord*>(d_pos + n1);
-    static_assert(sizeof(LidarRecord) == 4 * sizeof(int), "LidarRecord sits in lid_flags");
-    LidarRecord rec{};
-    // the raw records go up before the wait for the idle set's readers: only the kernels that write that set wait
     if (n_records > 0) {
         if (is_pinned(records)) {
             FLB_CUDA(h, cudaMemcpyAsync(h->lid_raw.p, records, raw_bytes, cudaMemcpyHostToDevice, cs));
@@ -2174,84 +2193,12 @@ int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const v
             FLB_CUDA(h, cudaMemcpyAsync(h->lid_raw.p, stv, raw_bytes, cudaMemcpyHostToDevice, cs));
             FLB_CUDA(h, h->st_lidar.mark(cs));
         }
-        { int rcq = vio_copy_begin(h, h->lid_slot); if (rcq) return rcq; }
-        size_t t1 = 0, t2 = 0, t3 = 0;
-        FLB_CUDA(h, cub::DeviceScan::InclusiveSum(nullptr, t1, d_vnum, d_vnum, n_records, cs));
-        FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t2, d_kept, d_pos, n_records, cs));
-        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p, h->lid_sorted.p,
-                                                    n_records, 0, 32, cs));
-        // the yaw route: ring keys in [0, n_rings], record indices, and the ring-order maps
-        const int n_rings = yaw ? std::min(yaw->n_scans, 65536) : 0;
-        int key_bits = 1;
-        while (key_bits < 17 && (1 << key_bits) <= n_rings) ++key_bits;
-        int* d_idx = nullptr;
-        int* d_idx_sorted = nullptr;
-        int* d_bad_ring = reinterpret_cast<int*>(d_rec + 1);
-        size_t t4 = 0, t5 = 0;
-        if (yaw) {
-            FLB_CUDA(h, h->lid_idx.reserve(2 * n1));
-            FLB_CUDA(h, h->lid_map.reserve(n1));
-            d_idx = h->lid_idx.p, d_idx_sorted = h->lid_idx.p + n1;
-            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t4, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted, n_records,
-                                                        0, key_bits, cs));
-            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(nullptr, t5, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
-        }
-        FLB_CUDA(h, h->lid_cub.reserve(std::max(std::max(t1, std::max(t2, t3)), std::max(t4, t5))));
-        const int g = (n_records + 255) / 256;
-        FLB_CUDA(h, cudaMemsetAsync(d_rec, 0, sizeof(LidarRecord), cs));
-        if (yaw) {
-            FLB_CUDA(h, cudaMemsetAsync(d_bad_ring, 0x7f, sizeof(int), cs));      // 0x7f7f7f7f: no bad ring
-            k_velo_rings<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, step, yaw->off_ring, yaw->n_scans, n_rings, h->lid_keys.p, d_idx,
-                                           d_bad_ring);
-            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t4, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted,
-                                                        n_records, 0, key_bits, cs));
-            k_velo_maps<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, n_rings, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p);
-            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t5, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
-            k_velo_flags<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, n_rings, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p,
-                                           h->lid_dec.p, d_kept);
-            h->launches += 5;
-        } else {
-            if (livox) {
-                k_lidar_valid<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum);
-                FLB_CUDA(h, cub::DeviceScan::InclusiveSum(h->lid_cub.p, t1, d_vnum, d_vnum, n_records, cs));
-                h->launches += 2;
-            }
-            k_lidar_flags<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum, h->lid_dec.p, d_kept);
-            h->launches += 1;
-        }
-        FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t2, d_kept, d_pos, n_records, cs));
-        k_lidar_scatter<<<g, 256, 0, cs>>>(h->lid_dec.p, d_kept, d_pos, n_records, h->lid_cloud_alt.p, h->lid_keys.p, d_rec);
-        k_lidar_order<<<g, 256, 0, cs>>>(h->lid_cloud_alt.p, h->lid_keys.p, n_records, d_rec);
-        FLB_CUDA(h, cudaGetLastError());
-        h->launches += 3;
-        int bad_ring = INT_MAX;
-        FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec) + (yaw ? sizeof(int) : 0), cudaMemcpyDeviceToHost, cs));
-        FLB_CUDA(h, cudaStreamSynchronize(cs));
-        std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
-        if (yaw) std::memcpy(&bad_ring, static_cast<const char*>(h->pin_lidar.p) + sizeof(rec), sizeof(int));
-        if (bad_ring < n_records) {
-            uint16_t ring;
-            std::memcpy(&ring, static_cast<const unsigned char*>(records) + (size_t)bad_ring * step + yaw->off_ring, sizeof(ring));
-            return fail(h, FLB_ERR_INVALID, "%s: record %d has ring %u >= n_scans %d (the per-ring yaw state has no such ring)", who,
-                        bad_ring, (unsigned)ring, yaw->n_scans);
-        }
-        if (rec.bad) return fail(h, FLB_ERR_INVALID, "%s: a kept point or time is not finite", who);
-        if (rec.unsorted) {
-            // stable: equal times keep record order (std::sort leaves that order unspecified in the reference)
-            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p,
-                                                        h->lid_sorted.p, rec.n_kept, 0, 32, cs));
-            FLB_CUDA(h, cudaMemcpyAsync(h->lid_cloud_alt.p, h->lid_sorted.p, (size_t)rec.n_kept * sizeof(float4), cudaMemcpyDeviceToDevice, cs));
-            k_lidar_last<<<1, 1, 0, cs>>>(h->lid_cloud_alt.p, d_rec);
-            FLB_CUDA(h, cudaGetLastError());
-            h->launches += 3;
-            FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
-            FLB_CUDA(h, cudaStreamSynchronize(cs));
-            std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
-        }
-    } else {
-        int rcq = vio_copy_begin(h, h->lid_slot);
-        if (rcq) return rcq;
     }
+    return vio_copy_begin(h, h->lid_slot);
+}
+
+// the idle cloud set, holding rec.n_kept points, becomes the current cloud with its cursor at the start
+int lidar_publish(flb_handle* h, const LidarRecord& rec, int* n_points, float* last_offset_ms) {
     std::swap(h->lid_cloud, h->lid_cloud_alt);
     h->lid_slot.slot ^= 1;
     h->lid_n = rec.n_kept;
@@ -2261,33 +2208,134 @@ int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const v
     return FLB_OK;
 }
 
-bool velo_field_ok(int off, int bytes, int step) { return off >= 0 && off <= step - bytes; }
+// Every route's end, from n > 0 candidates (lid_dec, lf.kept): compact them into the idle cloud set, refuse (yaw: a ring
+// >= n_scans, named from the host records; then a kept value that is not finite, in the caller's words `what`), re-sort
+// the times when they are out of order, and publish.  t_sum, t_sort: lid_cub's sizes for the ExclusiveSum and the 32-bit
+// SortPairs over n items.  A refusal publishes nothing.
+int lidar_tail(flb_handle* h, const char* who, const char* what, const LidarFlags& lf, int n, size_t t_sum, size_t t_sort,
+               const VeloYaw* yaw, const void* records, int step, int* n_points, float* last_offset_ms) {
+    cudaStream_t cs = h->copy_stream;
+    const int g = (n + 255) / 256;
+    FLB_CUDA(h, cudaMemsetAsync(lf.rec, 0, sizeof(LidarRecord), cs));
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t_sum, lf.kept, lf.pos, n, cs));
+    k_lidar_scatter<<<g, 256, 0, cs>>>(h->lid_dec.p, lf.kept, lf.pos, n, h->lid_cloud_alt.p, h->lid_keys.p, lf.rec);
+    k_lidar_order<<<g, 256, 0, cs>>>(h->lid_cloud_alt.p, h->lid_keys.p, n, lf.rec);
+    FLB_CUDA(h, cudaGetLastError());
+    h->launches += 3;
+    LidarRecord rec{};
+    int bad_ring = INT_MAX;
+    FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, lf.rec, sizeof(rec) + (yaw ? sizeof(int) : 0), cudaMemcpyDeviceToHost, cs));
+    FLB_CUDA(h, cudaStreamSynchronize(cs));
+    std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
+    if (yaw) std::memcpy(&bad_ring, static_cast<const char*>(h->pin_lidar.p) + sizeof(rec), sizeof(int));
+    if (bad_ring < n) {
+        uint16_t ring;
+        std::memcpy(&ring, static_cast<const unsigned char*>(records) + (size_t)bad_ring * step + yaw->off_ring, sizeof(ring));
+        return fail(h, FLB_ERR_INVALID, "%s: record %d has ring %u >= n_scans %d (the per-ring yaw state has no such ring)", who,
+                    bad_ring, (unsigned)ring, yaw->n_scans);
+    }
+    if (rec.bad) return fail(h, FLB_ERR_INVALID, "%s: %s is not finite", who, what);
+    if (rec.unsorted) {
+        // stable: equal times keep the candidates' order, record order or pl_surf's line-major order (std::sort leaves it
+        // unspecified in the reference)
+        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t_sort, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p,
+                                                    h->lid_sorted.p, rec.n_kept, 0, 32, cs));
+        FLB_CUDA(h, cudaMemcpyAsync(h->lid_cloud_alt.p, h->lid_sorted.p, (size_t)rec.n_kept * sizeof(float4), cudaMemcpyDeviceToDevice, cs));
+        k_lidar_last<<<1, 1, 0, cs>>>(h->lid_cloud_alt.p, lf.rec);
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches += 3;
+        FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, lf.rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
+        FLB_CUDA(h, cudaStreamSynchronize(cs));
+        std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
+    }
+    return lidar_publish(h, rec, n_points, last_offset_ms);
+}
+
+// flb_lidar_upload and flb_lidar_upload_velodyne from the argument checks on: decode and filter the records into
+// candidates, then lidar_tail.  yaw: the Velodyne route without per-point times; nullptr: the handler's own per-record
+// times.
+int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const void* records, int n_records, const VeloYaw* yaw,
+                      int* n_points, float* last_offset_ms) {
+    const int step = f.step;
+    const bool livox = f.kind == kLidarLivox;
+    const size_t n1 = std::max(n_records, 1);
+    { int rcq = lidar_begin(h, records, n_records, step); if (rcq) return rcq; }
+    if (n_records == 0) return lidar_publish(h, LidarRecord{}, n_points, last_offset_ms);
+    cudaStream_t cs = h->copy_stream;
+    const LidarFlags lf(h->lid_flags.p, n1);
+    int* d_vnum = lf.own;
+    size_t t1 = 0, t2 = 0, t3 = 0;
+    FLB_CUDA(h, cub::DeviceScan::InclusiveSum(nullptr, t1, d_vnum, d_vnum, n_records, cs));
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t2, lf.kept, lf.pos, n_records, cs));
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p, h->lid_sorted.p,
+                                                n_records, 0, 32, cs));
+    // the yaw route: ring keys in [0, n_rings], record indices, and the ring-order maps
+    const int n_rings = yaw ? std::min(yaw->n_scans, 65536) : 0;
+    int key_bits = 1;
+    while (key_bits < 17 && (1 << key_bits) <= n_rings) ++key_bits;
+    int* d_idx = nullptr;
+    int* d_idx_sorted = nullptr;
+    size_t t4 = 0, t5 = 0;
+    if (yaw) {
+        FLB_CUDA(h, h->lid_idx.reserve(2 * n1));
+        FLB_CUDA(h, h->lid_map.reserve(n1));
+        d_idx = h->lid_idx.p, d_idx_sorted = h->lid_idx.p + n1;
+        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t4, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted, n_records,
+                                                    0, key_bits, cs));
+        FLB_CUDA(h, cub::DeviceScan::InclusiveScan(nullptr, t5, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
+    }
+    FLB_CUDA(h, h->lid_cub.reserve(std::max(std::max(t1, std::max(t2, t3)), std::max(t4, t5))));
+    const int g = (n_records + 255) / 256;
+    if (yaw) {
+        FLB_CUDA(h, cudaMemsetAsync(lf.after, 0x7f, sizeof(int), cs));         // 0x7f7f7f7f: no bad ring
+        k_velo_rings<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, step, yaw->off_ring, yaw->n_scans, n_rings, h->lid_keys.p, d_idx,
+                                       lf.after);
+        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t4, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted,
+                                                    n_records, 0, key_bits, cs));
+        k_velo_maps<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, n_rings, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p);
+        FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t5, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
+        k_velo_flags<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, n_rings, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p,
+                                       h->lid_dec.p, lf.kept);
+        h->launches += 5;
+    } else {
+        if (livox) {
+            k_lidar_valid<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum);
+            FLB_CUDA(h, cub::DeviceScan::InclusiveSum(h->lid_cub.p, t1, d_vnum, d_vnum, n_records, cs));
+            h->launches += 2;
+        }
+        k_lidar_flags<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum, h->lid_dec.p, lf.kept);
+        h->launches += 1;
+    }
+    return lidar_tail(h, who, "a kept point or time", lf, n_records, t2, t3, yaw, records, step, n_points, last_offset_ms);
+}
 
 }  // namespace
+
+int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* records, int n_records, int* n_points,
+                     float* last_offset_ms) {
+    FLB_CHECK_H(h);
+    const char* who = "flb_lidar_upload";
+    LidarFmt f;
+    { int rcq = lidar_format(h, who, fmt, records, n_records, false, 0.0, &f); if (rcq) return rcq; }
+    const unsigned char* rec_h = static_cast<const unsigned char*>(records);
+    if (n_records > 0 && f.kind == kLidarVelodyne) {
+        float t_last;                                                              // given_offset_time, :279
+        std::memcpy(&t_last, rec_h + (size_t)(n_records - 1) * f.step + f.off_time, sizeof(t_last));
+        if (!(t_last > 0))
+            return fail(h, FLB_ERR_INVALID, "%s: a Velodyne cloud without per-point times (last time %g): its times come from "
+                        "the yaw angle (src/preprocess.cpp:389-419), which flb_lidar_upload_velodyne derives", who, (double)t_last);
+    }
+    if (n_records > 0 && f.kind == kLidarXt32) std::memcpy(&f.time_head, rec_h + f.off_time, sizeof(double));   // :441
+    return lidar_upload_core(h, who, f, records, n_records, nullptr, n_points, last_offset_ms);
+}
 
 int flb_lidar_upload_velodyne(flb_handle* h, const flb_velodyne_format* fmt, const void* records, int n_records, int* n_points,
                               float* last_offset_ms, int* yaw_times) {
     FLB_CHECK_H(h);
     const char* who = "flb_lidar_upload_velodyne";
-    if (n_records < 0 || !fmt || (n_records > 0 && !records)) return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
-    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || !std::isfinite(fmt->blind))
-        return fail(h, FLB_ERR_INVALID, "%s: point_filter_num %d, n_scans %d, blind %g", who, fmt->point_filter_num, fmt->n_scans,
-                    fmt->blind);
-    const int step = fmt->point_step;
-    if (step < 1 || !velo_field_ok(fmt->off_x, 4, step) || !velo_field_ok(fmt->off_y, 4, step) || !velo_field_ok(fmt->off_z, 4, step) ||
-        !velo_field_ok(fmt->off_ring, 2, step) || (fmt->off_time != -1 && !velo_field_ok(fmt->off_time, 4, step)))
-        return fail(h, FLB_ERR_INVALID, "%s: a field does not fit in point_step %d", who, step);
-    LidarFmt f{};
-    f.kind = kLidarVelodyne, f.step = step, f.off_x = fmt->off_x, f.off_y = fmt->off_y, f.off_z = fmt->off_z;
-    f.off_time = fmt->off_time >= 0 ? fmt->off_time : 0;
-    f.n_scans = fmt->n_scans, f.filter_num = fmt->point_filter_num, f.blind = fmt->blind;
-    // given_offset_time (:279): the last record's time > 0.  Without a time field the reference reads 0.
-    bool given = n_records == 0;
-    if (n_records > 0 && fmt->off_time >= 0) {
-        float t_last;
-        std::memcpy(&t_last, static_cast<const unsigned char*>(records) + (size_t)(n_records - 1) * step + fmt->off_time, sizeof(t_last));
-        given = t_last > 0;
-    }
+    LidarFmt f;
+    bool given = false;
+    { int rcq = velo_format(h, who, fmt, records, n_records, false, 0.0, &f, &given); if (rcq) return rcq; }
     VeloYaw yaw{fmt->off_ring, fmt->n_scans};
     const int rc = lidar_upload_core(h, who, f, records, n_records, given ? nullptr : &yaw, n_points, last_offset_ms);
     if (rc) return rc;
@@ -2310,38 +2358,30 @@ FeatConst feat_const(const LidarFmt& f, double dis_b) {
     return c;
 }
 
-// flb_lidar_upload_features and flb_lidar_upload_velodyne_features from the argument checks on.  f.off_line: the
-// Livox line, the Ouster's u8 ring or the Velodyne's u16 ring.  yaw: Velodyne times from the yaw angle.
+// flb_lidar_upload_features and flb_lidar_upload_velodyne_features from the argument checks on: pl_surf's points as
+// candidates, then lidar_tail.  f.off_line: the Livox line, the Ouster's u8 ring or the Velodyne's u16 ring.  yaw:
+// Velodyne times from the yaw angle.
 int lidar_features_core(flb_handle* h, const char* who, const LidarFmt& f, double dis_b, const void* records, int n_records,
                         bool yaw, int* n_points, float* last_offset_ms) {
     const FeatConst c = feat_const(f, dis_b);
     const int min_size = f.kind == kLidarLivox ? 6 : f.kind == kLidarVelodyne ? 2 : 1;   // :117, :357; the Ouster: any
-    const int step = f.step;
-    const size_t n = (size_t)n_records, n1 = std::max<size_t>(n, 1), raw_bytes = n * step;
+    const size_t n1 = std::max(n_records, 1);
     const int ns = f.n_scans;
     int levels = 1;                                      // 2^levels > any chain length (<= the point count)
     while (levels < 31 && ((size_t)1 << levels) <= n1) ++levels;
-    FLB_CUDA(h, h->lid_raw.reserve(std::max<size_t>(raw_bytes, 4)));
-    FLB_CUDA(h, h->lid_cloud_alt.reserve(n1));
-    FLB_CUDA(h, h->lid_dec.reserve(n1));
-    FLB_CUDA(h, h->lid_sorted.reserve(n1));
-    FLB_CUDA(h, h->lid_keys.reserve(n1));
-    FLB_CUDA(h, h->lid_keys_sorted.reserve(n1));
     FLB_CUDA(h, h->lid_idx.reserve(2 * n1));
     FLB_CUDA(h, h->lid_map.reserve(n1));
-    FLB_CUDA(h, h->lid_flags.reserve(3 * n1 + 8));
     FLB_CUDA(h, h->feat_pts.reserve(n1));
     FLB_CUDA(h, h->feat_i.reserve((size_t)(levels + 8) * n1 + 3 * (size_t)ns + 1));
     FLB_CUDA(h, h->feat_d.reserve(3 * n1));
     FLB_CUDA(h, h->feat_st.reserve(n1));
     FLB_CUDA(h, h->feat_u8.reserve(2 * n1));
-    FLB_CUDA(h, h->pin_lidar.reserve(64));
+    { int rcq = lidar_begin(h, records, n_records, f.step); if (rcq) return rcq; }
+    if (n_records == 0) return lidar_publish(h, LidarRecord{}, n_points, last_offset_ms);
     cudaStream_t cs = h->copy_stream;
-    int* d_take = h->lid_flags.p;
-    int* d_kept = d_take + n1;
-    int* d_pos = d_kept + n1;
-    LidarRecord* d_rec = reinterpret_cast<LidarRecord*>(d_pos + n1);
-    int* d_count = reinterpret_cast<int*>(d_rec + 1);
+    const LidarFlags lf(h->lid_flags.p, n1);
+    int* d_take = lf.own;
+    int* d_count = lf.after;
     int* d_idx = h->lid_idx.p;
     int* d_idx_sorted = h->lid_idx.p + n1;
     // per-point ints: lkey | pv | rs | rs2 | seed | ft | fin | J[levels] | lbeg | lend | lhead
@@ -2361,106 +2401,61 @@ int lidar_features_core(flb_handle* h, const char* who, const LidarFmt& f, doubl
     double* d_isect = d_dista + n1;
     unsigned char* d_vis = h->feat_u8.p;
     unsigned char* d_small = d_vis + n1;
-    LidarRecord rec{};
-    if (n_records > 0) {
-        if (is_pinned(records)) {
-            FLB_CUDA(h, cudaMemcpyAsync(h->lid_raw.p, records, raw_bytes, cudaMemcpyHostToDevice, cs));
-        } else {
-            void* stv = nullptr;
-            FLB_CUDA(h, h->st_lidar.acquire(raw_bytes, &stv));
-            std::memcpy(stv, records, raw_bytes);
-            FLB_CUDA(h, cudaMemcpyAsync(h->lid_raw.p, stv, raw_bytes, cudaMemcpyHostToDevice, cs));
-            FLB_CUDA(h, h->st_lidar.mark(cs));
-        }
-        { int rcq = vio_copy_begin(h, h->lid_slot); if (rcq) return rcq; }
-        const int g = (n_records + 255) / 256;
-        size_t t1 = 0, t2 = 0, t3 = 0, t4 = 0, t5 = 0;
-        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t1, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted, n_records,
-                                                    0, 8, cs));
-        FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t2, d_take, d_pos, n_records, cs));
-        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p, h->lid_sorted.p,
-                                                    n_records, 0, 32, cs));
-        FLB_CUDA(h, cub::DeviceScan::InclusiveScan(nullptr, t4, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
-        FLB_CUDA(h, cub::DeviceScan::InclusiveScan(nullptr, t5, d_seed, d_rs, FeatMaxOp(), n_records, cs));
-        size_t t6 = 0;
-        FLB_CUDA(h, cub::DeviceScan::ExclusiveScan(nullptr, t6, d_seed, d_pv, FeatMaxOp(), -1, n_records, cs));
-        FLB_CUDA(h, h->lid_cub.reserve(std::max(std::max(std::max(t1, t2), std::max(t3, t4)), std::max(t5, t6))));
-        // the records into line order
-        k_feat_keys<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, h->lid_keys.p, d_idx);
-        FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t1, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted,
-                                                    n_records, 0, 8, cs));
-        if (yaw) {
-            k_velo_maps<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, ns, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p);
-            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t4, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
-            h->launches += 2;
-        }
-        k_feat_take<<<g, 256, 0, cs>>>(h->lid_keys_sorted.p, n_records, ns, yaw ? 1 : 0, d_take);
-        FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t2, d_take, d_pos, n_records, cs));
-        k_feat_gather<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, yaw ? 1 : 0, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p,
-                                         d_take, d_pos, h->feat_pts.p, d_lkey, d_count);
-        FLB_CUDA(h, cudaGetLastError());
-        h->launches += 6;
-        int M = 0;
-        FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_count, sizeof(int), cudaMemcpyDeviceToHost, cs));
-        FLB_CUDA(h, cudaStreamSynchronize(cs));
-        std::memcpy(&M, h->pin_lidar.p, sizeof(int));
-        FLB_CUDA(h, cudaMemsetAsync(d_rec, 0, sizeof(LidarRecord), cs));
-        if (M > 0) {
-            const int gm = (M + 255) / 256;
-            int lv = 1;
-            while (lv < levels && (1 << lv) <= M) ++lv;
-            FLB_CUDA(h, cudaMemsetAsync(d_lbeg, 0, 2 * ns * sizeof(int), cs));
-            FLB_CUDA(h, cudaMemsetAsync(d_lhead, 0x7f, ns * sizeof(int), cs));      // 0x7f7f7f7f: no head
-            k_feat_range<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_lkey, M, c.avia, c.blind, d_rng, d_dista, d_lbeg, d_lend, d_lhead);
-            k_feat_steps<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_rng, d_dista, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, c,
-                                             h->feat_st.p, d_J, d_vis);
-            for (int l = 0; l + 1 < lv; ++l) k_feat_jump<<<gm, 256, 0, cs>>>(d_J + (size_t)l * n1, M, d_J + (size_t)(l + 1) * n1);
-            for (int l = lv - 1; l >= 0; --l) k_feat_mark<<<gm, 256, 0, cs>>>(d_J + (size_t)l * n1, M, d_vis);
-            k_feat_vis_index<<<gm, 256, 0, cs>>>(d_vis, M, d_seed);
-            FLB_CUDA(h, cub::DeviceScan::ExclusiveScan(h->lid_cub.p, t6, d_seed, d_pv, FeatMaxOp(), -1, M, cs));
-            k_feat_types<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_rng, d_dista, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, c,
-                                             h->feat_st.p, d_vis, d_pv, d_ft, d_isect);
-            k_feat_small<<<gm, 256, 0, cs>>>(d_rng, d_dista, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, c, d_ft, d_isect, d_small);
-            k_feat_small_seed<<<gm, 256, 0, cs>>>(d_small, M, d_seed);
-            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t5, d_seed, d_rs, FeatMaxOp(), M, cs));
-            k_feat_final<<<gm, 256, 0, cs>>>(d_ft, d_small, d_rs, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, d_fin, d_seed);
-            FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t5, d_seed, d_rs2, FeatMaxOp(), M, cs));
-            k_feat_emit<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_fin, d_rs2, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, f.filter_num,
-                                            h->lid_dec.p, d_kept);
-            // flb_lidar_upload's compaction and time sort
-            FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t2, d_kept, d_pos, M, cs));
-            k_lidar_scatter<<<gm, 256, 0, cs>>>(h->lid_dec.p, d_kept, d_pos, M, h->lid_cloud_alt.p, h->lid_keys.p, d_rec);
-            k_lidar_order<<<gm, 256, 0, cs>>>(h->lid_cloud_alt.p, h->lid_keys.p, M, d_rec);
-            FLB_CUDA(h, cudaGetLastError());
-            h->launches += 15 + 2 * lv;
-        }
-        FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
-        FLB_CUDA(h, cudaStreamSynchronize(cs));
-        std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
-        if (rec.bad) return fail(h, FLB_ERR_INVALID, "%s: a point of pl_surf or its time is not finite", who);
-        if (rec.unsorted) {
-            // stable: equal times keep pl_surf's line-major order
-            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p,
-                                                        h->lid_sorted.p, rec.n_kept, 0, 32, cs));
-            FLB_CUDA(h, cudaMemcpyAsync(h->lid_cloud_alt.p, h->lid_sorted.p, (size_t)rec.n_kept * sizeof(float4), cudaMemcpyDeviceToDevice, cs));
-            k_lidar_last<<<1, 1, 0, cs>>>(h->lid_cloud_alt.p, d_rec);
-            FLB_CUDA(h, cudaGetLastError());
-            h->launches += 3;
-            FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
-            FLB_CUDA(h, cudaStreamSynchronize(cs));
-            std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
-        }
-    } else {
-        int rcq = vio_copy_begin(h, h->lid_slot);
-        if (rcq) return rcq;
+    const int g = (n_records + 255) / 256;
+    size_t t1 = 0, t2 = 0, t3 = 0, t4 = 0, t5 = 0;
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t1, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted, n_records,
+                                                0, 8, cs));
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, t2, d_take, lf.pos, n_records, cs));
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t3, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_cloud_alt.p, h->lid_sorted.p,
+                                                n_records, 0, 32, cs));
+    FLB_CUDA(h, cub::DeviceScan::InclusiveScan(nullptr, t4, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
+    FLB_CUDA(h, cub::DeviceScan::InclusiveScan(nullptr, t5, d_seed, d_rs, FeatMaxOp(), n_records, cs));
+    size_t t6 = 0;
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveScan(nullptr, t6, d_seed, d_pv, FeatMaxOp(), -1, n_records, cs));
+    FLB_CUDA(h, h->lid_cub.reserve(std::max(std::max(std::max(t1, t2), std::max(t3, t4)), std::max(t5, t6))));
+    // the records into line order
+    k_feat_keys<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, h->lid_keys.p, d_idx);
+    FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t1, h->lid_keys.p, h->lid_keys_sorted.p, d_idx, d_idx_sorted,
+                                                n_records, 0, 8, cs));
+    if (yaw) {
+        k_velo_maps<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, ns, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p);
+        FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t4, h->lid_map.p, h->lid_map.p, VeloComposeOp(), n_records, cs));
+        h->launches += 2;
     }
-    std::swap(h->lid_cloud, h->lid_cloud_alt);
-    h->lid_slot.slot ^= 1;
-    h->lid_n = rec.n_kept;
-    h->lid_cursor = 0;
-    if (n_points) *n_points = rec.n_kept;
-    if (last_offset_ms) *last_offset_ms = rec.n_kept > 0 ? rec.last : 0.f;
-    return FLB_OK;
+    k_feat_take<<<g, 256, 0, cs>>>(h->lid_keys_sorted.p, n_records, ns, yaw ? 1 : 0, d_take);
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t2, d_take, lf.pos, n_records, cs));
+    k_feat_gather<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, yaw ? 1 : 0, h->lid_keys_sorted.p, d_idx_sorted, h->lid_map.p,
+                                     d_take, lf.pos, h->feat_pts.p, d_lkey, d_count);
+    FLB_CUDA(h, cudaGetLastError());
+    h->launches += 6;
+    int M = 0;
+    FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_count, sizeof(int), cudaMemcpyDeviceToHost, cs));
+    FLB_CUDA(h, cudaStreamSynchronize(cs));
+    std::memcpy(&M, h->pin_lidar.p, sizeof(int));
+    if (M == 0) return lidar_publish(h, LidarRecord{}, n_points, last_offset_ms);
+    const int gm = (M + 255) / 256;
+    int lv = 1;
+    while (lv < levels && (1 << lv) <= M) ++lv;
+    FLB_CUDA(h, cudaMemsetAsync(d_lbeg, 0, 2 * ns * sizeof(int), cs));
+    FLB_CUDA(h, cudaMemsetAsync(d_lhead, 0x7f, ns * sizeof(int), cs));      // 0x7f7f7f7f: no head
+    k_feat_range<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_lkey, M, c.avia, c.blind, d_rng, d_dista, d_lbeg, d_lend, d_lhead);
+    k_feat_steps<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_rng, d_dista, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, c,
+                                     h->feat_st.p, d_J, d_vis);
+    for (int l = 0; l + 1 < lv; ++l) k_feat_jump<<<gm, 256, 0, cs>>>(d_J + (size_t)l * n1, M, d_J + (size_t)(l + 1) * n1);
+    for (int l = lv - 1; l >= 0; --l) k_feat_mark<<<gm, 256, 0, cs>>>(d_J + (size_t)l * n1, M, d_vis);
+    k_feat_vis_index<<<gm, 256, 0, cs>>>(d_vis, M, d_seed);
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveScan(h->lid_cub.p, t6, d_seed, d_pv, FeatMaxOp(), -1, M, cs));
+    k_feat_types<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_rng, d_dista, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, c,
+                                     h->feat_st.p, d_vis, d_pv, d_ft, d_isect);
+    k_feat_small<<<gm, 256, 0, cs>>>(d_rng, d_dista, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, c, d_ft, d_isect, d_small);
+    k_feat_small_seed<<<gm, 256, 0, cs>>>(d_small, M, d_seed);
+    FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t5, d_seed, d_rs, FeatMaxOp(), M, cs));
+    k_feat_final<<<gm, 256, 0, cs>>>(d_ft, d_small, d_rs, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, d_fin, d_seed);
+    FLB_CUDA(h, cub::DeviceScan::InclusiveScan(h->lid_cub.p, t5, d_seed, d_rs2, FeatMaxOp(), M, cs));
+    k_feat_emit<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_fin, d_rs2, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, f.filter_num,
+                                    h->lid_dec.p, lf.kept);
+    h->launches += 12 + 2 * lv;
+    return lidar_tail(h, who, "a point of pl_surf or its time", lf, M, t2, t3, nullptr, records, f.step, n_points, last_offset_ms);
 }
 
 }  // namespace
@@ -2469,25 +2464,8 @@ int flb_lidar_upload_features(flb_handle* h, const flb_lidar_format* fmt, double
                               int* n_points, float* last_offset_ms) {
     FLB_CHECK_H(h);
     const char* who = "flb_lidar_upload_features";
-    if (n_records < 0 || !fmt || (n_records > 0 && !records) || !std::isfinite(dis_b))
-        return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
-    if (fmt->kind == kLidarVelodyne || fmt->kind == kLidarXt32)
-        return fail(h, FLB_ERR_INVALID, "%s: kind %d: a Velodyne cloud goes to flb_lidar_upload_velodyne_features; the XT32 "
-                    "has no feature branch (src/preprocess.cpp:432-464), so flb_lidar_upload serves it", who, fmt->kind);
-    if (fmt->kind != kLidarLivox && fmt->kind != kLidarOuster) return fail(h, FLB_ERR_INVALID, "%s: unknown kind %d", who, fmt->kind);
-    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || fmt->n_scans > 128 || !std::isfinite(fmt->blind))
-        return fail(h, FLB_ERR_INVALID, "%s: point_filter_num %d, n_scans %d (1..128: pl_buff[128]), blind %g", who,
-                    fmt->point_filter_num, fmt->n_scans, fmt->blind);
-    const int step = fmt->point_step;
-    const bool livox = fmt->kind == kLidarLivox;
-    if (step < 1 || !lidar_field_ok(fmt->off_x, 4, step) || !lidar_field_ok(fmt->off_y, 4, step) || !lidar_field_ok(fmt->off_z, 4, step) ||
-        !lidar_field_ok(fmt->off_time, 4, step) || !lidar_field_ok(fmt->off_line, 1, step) ||
-        (livox && !lidar_field_ok(fmt->off_tag, 1, step)))
-        return fail(h, FLB_ERR_INVALID, "%s: a field does not fit in point_step %d or is not aligned to its type", who, step);
-    LidarFmt f{};
-    f.kind = fmt->kind, f.step = step, f.off_x = fmt->off_x, f.off_y = fmt->off_y, f.off_z = fmt->off_z, f.off_time = fmt->off_time;
-    f.off_tag = livox ? fmt->off_tag : 0, f.off_line = fmt->off_line;
-    f.n_scans = fmt->n_scans, f.filter_num = fmt->point_filter_num, f.blind = fmt->blind;
+    LidarFmt f;
+    { int rcq = lidar_format(h, who, fmt, records, n_records, true, dis_b, &f); if (rcq) return rcq; }
     return lidar_features_core(h, who, f, dis_b, records, n_records, false, n_points, last_offset_ms);
 }
 
@@ -2495,25 +2473,9 @@ int flb_lidar_upload_velodyne_features(flb_handle* h, const flb_velodyne_format*
                                        int n_records, int* n_points, float* last_offset_ms, int* yaw_times) {
     FLB_CHECK_H(h);
     const char* who = "flb_lidar_upload_velodyne_features";
-    if (n_records < 0 || !fmt || (n_records > 0 && !records) || !std::isfinite(dis_b))
-        return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
-    if (fmt->point_filter_num < 1 || fmt->n_scans < 1 || fmt->n_scans > 128 || !std::isfinite(fmt->blind))
-        return fail(h, FLB_ERR_INVALID, "%s: point_filter_num %d, n_scans %d (1..128: pl_buff[128]), blind %g", who,
-                    fmt->point_filter_num, fmt->n_scans, fmt->blind);
-    const int step = fmt->point_step;
-    if (step < 1 || !velo_field_ok(fmt->off_x, 4, step) || !velo_field_ok(fmt->off_y, 4, step) || !velo_field_ok(fmt->off_z, 4, step) ||
-        !velo_field_ok(fmt->off_ring, 2, step) || (fmt->off_time != -1 && !velo_field_ok(fmt->off_time, 4, step)))
-        return fail(h, FLB_ERR_INVALID, "%s: a field does not fit in point_step %d", who, step);
-    LidarFmt f{};
-    f.kind = kLidarVelodyne, f.step = step, f.off_x = fmt->off_x, f.off_y = fmt->off_y, f.off_z = fmt->off_z;
-    f.off_time = fmt->off_time >= 0 ? fmt->off_time : 0, f.off_line = fmt->off_ring;
-    f.n_scans = fmt->n_scans, f.filter_num = fmt->point_filter_num, f.blind = fmt->blind;
-    bool given = n_records == 0;                                                  // given_offset_time (:279)
-    if (n_records > 0 && fmt->off_time >= 0) {
-        float t_last;
-        std::memcpy(&t_last, static_cast<const unsigned char*>(records) + (size_t)(n_records - 1) * step + fmt->off_time, sizeof(t_last));
-        given = t_last > 0;
-    }
+    LidarFmt f;
+    bool given = false;
+    { int rcq = velo_format(h, who, fmt, records, n_records, true, dis_b, &f, &given); if (rcq) return rcq; }
     const int rc = lidar_features_core(h, who, f, dis_b, records, n_records, !given, n_points, last_offset_ms);
     if (rc) return rc;
     if (yaw_times) *yaw_times = given ? 0 : 1;
