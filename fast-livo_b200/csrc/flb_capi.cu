@@ -541,37 +541,130 @@ size_t index_bytes(const flb_handle* h) {
     return h->sparse ? ((size_t)(unsigned)h->grid.nx + 1) * sizeof(SparseCell) : ((size_t)h->ncell + 1) * sizeof(int);
 }
 
-LioArgs make_lio_args(flb_handle* h, const LioParamsDev& prm, bool exports, int width) {
+// The device buffers of one frame that the update kernels read and write: the handle's own (handle_frame), or frame i's
+// slice of the batch buffers (flb_batch_update_enqueue).
+struct FrameBufs {
+    const float4* scan;
+    int N;
+    State18* states;             // x, x_prop, old_state (VIO), saved x, saved x_prop
+    LioCtrl* lio_ctrl;
+    VioCtrl* vio_ctrl;
+    PriorBlock* prior;
+    unsigned char* sel;
+    float4* plane;
+    unsigned char* plane_ok;
+    double* partials;
+    float* errors;
+    int err_stride;
+    double* G_last;
+};
+
+FrameBufs handle_frame(flb_handle* h) {
+    return {h->scan.p, h->N, h->states.p, h->lio_ctrl.p, h->vio_ctrl.p, h->prior.p, h->sel.p, h->plane.p, h->plane_ok.p,
+            h->partials.p, h->errors.p, h->err_stride, h->G_last.p};
+}
+
+// The argument blocks of the update kernels.  Each builder sets the fields every caller sets alike; a field that one
+// path alone sets is set at its call site.
+LioArgs make_lio_args(flb_handle* h, const LioParamsDev& prm, const FrameBufs& fb) {
     LioArgs a{};
-    a.scan = h->scan.p;
-    a.N = h->N;
+    a.scan = fb.scan;
+    a.N = fb.N;
     a.grid = h->grid;
     a.cell_start = cell_index(h);
     a.map_pts = h->map_pts.p;
-    a.state = &h->states.p[0];
+    a.state = fb.states;
     a.prm = prm;
     a.plane_thr = (float)h->cfg.plane_threshold;
-    a.ctrl = h->lio_ctrl.p;
+    a.ctrl = fb.lio_ctrl;
     a.force_rematch = -1;
-    a.pose_override = nullptr;
-    a.sel = h->sel.p;
-    a.plane = h->plane.p;
-    a.plane_ok = h->plane_ok.p;
-    a.partials = h->partials.p;
+    a.sel = fb.sel;
+    a.plane = fb.plane;
+    a.plane_ok = fb.plane_ok;
+    a.partials = fb.partials;
     a.M = h->M;
-    a.prefetch = 0;
-    if (exports) {
-        a.x_world = h->x_world.p;
-        a.x_nn_idx = h->x_nn_idx.p;
-        a.x_nn_d2 = h->x_nn_d2.p;
-        a.x_pabcd = h->x_pabcd.p;
-        a.x_pd2 = h->x_pd2.p;
-        a.x_rowmask = h->x_rowmask.p;
-        a.x_rows = h->x_rows.p;
-        a.x_meas = h->x_meas.p;
-    }
-    (void)width;
     return a;
+}
+
+LioSolveArgs make_lio_solve_args(flb_handle* h, const LioParamsDev& prm, const FrameBufs& fb) {
+    LioSolveArgs s{};
+    s.state = fb.states;
+    s.state_prop = fb.states + 1;
+    s.ctrl = fb.lio_ctrl;
+    s.prior = fb.prior;
+    s.partials = fb.partials;
+    s.nblocks = (fb.N + kLioBlock - 1) / kLioBlock;
+    s.prm = prm;
+    s.timeout_flag = &h->barrier.p->timeout;
+    return s;
+}
+
+VioArgs make_vio_args(flb_handle* h, const VioParamsDev& prm, const FrameBufs& fb) {
+    VioArgs a{};
+    a.img = h->img.p;
+    a.cam = h->cam;
+    a.pos = h->patch_pos.p;
+    a.patch = h->patch_ref.p;
+    a.search_level = h->patch_level.p;
+    a.Pn = h->Pn;
+    a.state = fb.states;
+    a.prm = prm;
+    a.ctrl = fb.vio_ctrl;
+    a.force_level = -1;
+    a.errors = fb.errors;
+    a.err_stride = fb.err_stride;
+    a.partials = fb.partials;
+    return a;
+}
+
+VioSolveArgs make_vio_solve_args(flb_handle* h, const VioParamsDev& prm, const FrameBufs& fb) {
+    VioSolveArgs s{};
+    s.state = fb.states;
+    s.state_prop = fb.states + 1;
+    s.old_state = fb.states + 2;
+    s.ctrl = fb.vio_ctrl;
+    s.prior = fb.prior;
+    s.G_last = fb.G_last;
+    s.partials = fb.partials;
+    s.nblocks = vio_nblocks(h);
+    s.errors = fb.errors;
+    s.err_stride = fb.err_stride;
+    s.Pn_total = h->Pn;
+    s.prm = prm;
+    s.timeout_flag = &h->barrier.p->timeout;
+    return s;
+}
+
+// (R, p) as 12 doubles at `dst` on the device, through the misc staging area in stream order
+int upload_pose(flb_handle* h, double* dst, const double* R, const double* p) {
+    void* stv = nullptr;
+    FLB_CUDA(h, h->st_misc.acquire(12 * sizeof(double), &stv));
+    double* st = static_cast<double*>(stv);
+    std::memcpy(st, R, 9 * sizeof(double));
+    std::memcpy(st + 9, p, 3 * sizeof(double));
+    FLB_CUDA(h, cudaMemcpyAsync(dst, st, 12 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    FLB_CUDA(h, h->st_misc.mark(h->stream));
+    return FLB_OK;
+}
+
+// The packed sums of one pass: HTH's upper triangle row by row (written out symmetric, width x width), then the
+// right-hand side (width)
+void unpack_normal_eq(const double* po, int width, double* HTH, double* rhs) {
+    int k = 0;
+    for (int r = 0; r < width; ++r)
+        for (int c = r; c < width; ++c) {
+            HTH[r * width + c] = po[k];
+            HTH[c * width + r] = po[k];
+            ++k;
+        }
+    for (int r = 0; r < width; ++r) rhs[r] = po[k + r];
+}
+
+// Every caller that reads the image needs a camera and an image of the camera's size.
+int vio_image_check(flb_handle* h, const char* who) {
+    if (!h->cam_set || h->img_w <= 0) return fail(h, FLB_ERR_STATE, "%s: camera and image must be set first", who);
+    if (h->cam.width != h->img_w || h->cam.height != h->img_h) return fail(h, FLB_ERR_STATE, "camera / image size mismatch");
+    return FLB_OK;
 }
 
 int launch_lio_pass(flb_handle* h, const LioArgs& a, int width, bool knn_family) {
@@ -599,6 +692,36 @@ int allreduce_packed(flb_handle* h, const double* partials, int nblocks, int K) 
     int r = g_nccl.AllReduce(h->packed.p, h->packed.p, (size_t)K, kNcclFloat64, kNcclSum, h->comm, h->stream);
     if (r != 0) return fail(h, FLB_ERR_COMM, "ncclAllReduce: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
     h->launches++;
+    return FLB_OK;
+}
+
+// The kernel-per-pass VIO update: up to `passes` rounds of k_vio_pass then k_vio_finalize; the kernels return at once
+// when the update (or the level) has ended.
+int vio_pass_loop(flb_handle* h, const VioArgs& a, VioSolveArgs s, int passes) {
+    const int nb = vio_nblocks(h);
+    for (int it = 0; it < passes && h->Pn > 0; ++it) {
+        {
+            LaunchScope ls(h, FAM_VIO);
+            k_vio_pass<kVioBlock><<<nb, kVioBlock, 0, h->stream>>>(a);
+            FLB_CUDA(h, cudaGetLastError());
+        }
+        if (h->comm) {
+            int rc = allreduce_packed(h, h->partials.p, nb, kVioPacked);
+            if (rc) return rc;
+            s.partials = h->packed.p;
+            s.nblocks = 1;
+            // gather every rank's per-patch errors in patch order (shards padded to errors.cap/world)
+            const size_t shard = (size_t)h->err_shard;
+            int r = g_nccl.AllGather(h->errors.p, h->errors_all.p, shard, kNcclFloat32, h->comm, h->stream);
+            if (r != 0) return fail(h, FLB_ERR_COMM, "ncclAllGather failed");
+            h->launches++;
+            s.errors = h->errors_all.p;
+            s.Pn_total = (int)(shard * (size_t)h->world);
+        }
+        LaunchScope ls(h, FAM_SOLVE);
+        k_vio_finalize<<<1, kLeaderBlock, 0, h->stream>>>(s);
+        FLB_CUDA(h, cudaGetLastError());
+    }
     return FLB_OK;
 }
 
@@ -706,7 +829,6 @@ int image_upload_frame(flb_handle* h, const uint8_t* src, int width, int height,
     h->last_vio_valid = false;
     return FLB_OK;
 }
-int vio_inputs_release(flb_handle*) { return FLB_OK; }   // (readers are fenced per slot at the next upload: vio_copy_begin)
 
 // Perform the deferred device-side state moves with plain copies (every consumer other than the persistent kernels).
 int flush_state_ops(flb_handle* h) {
@@ -770,17 +892,10 @@ int enqueue_lio_update(flb_handle* h, const flb_lio_params* prm) {
         return fail(h, FLB_ERR_STATE, "the fused NVLink exchange lives in the persistent kernels (flb_config.persistent = 1)");
     LioParamsDev d;
     to_dev_params(prm, d);
-    LioSolveArgs s{};
-    s.state = &h->states.p[0];
-    s.state_prop = &h->states.p[1];
-    s.ctrl = h->lio_ctrl.p;
-    s.prior = h->prior.p;
-    s.partials = h->partials.p;
-    s.nblocks = lio_nblocks(h);
-    s.prm = d;
+    const FrameBufs fb = handle_frame(h);
+    LioSolveArgs s = make_lio_solve_args(h, d, fb);
     s.p2p = h->p2p;
-    s.timeout_flag = &h->barrier.p->timeout;
-    LioArgs a = make_lio_args(h, d, false, 6);
+    LioArgs a = make_lio_args(h, d, fb);
     const bool lio_persistent = h->cfg.persistent && (!h->comm || h->p2p.world > 1);
     if (h->prior_pending || (h->reset_pending && !lio_persistent)) { int rcf = flush_state_ops(h); if (rcf) return rcf; }
     if (h->reset_pending) {              // the kernel starts from the saved pair and restores state / state_prop itself
@@ -882,8 +997,7 @@ int resolve_pn(flb_handle* h) {
 }
 
 int enqueue_vio_update(flb_handle* h, const flb_vio_params* prm) {
-    if (!h->cam_set || h->img_w <= 0) return fail(h, FLB_ERR_STATE, "flb_vio_update: camera and image must be set first");
-    if (h->cam.width != h->img_w || h->cam.height != h->img_h) return fail(h, FLB_ERR_STATE, "camera / image size mismatch");
+    { int rc = vio_image_check(h, "flb_vio_update"); if (rc) return rc; }
     if (!h->state_valid) return fail(h, FLB_ERR_STATE, "flb_vio_update: no device state (flb_state_upload)");
     if (prm->max_iteration > 1000) return fail(h, FLB_ERR_INVALID, "max_iteration outside [0, 1000]");
     if (h->pn_on_device && !(h->cfg.persistent && h->p2p.world <= 1 && !h->comm && prm->max_iteration > 0)) {
@@ -892,21 +1006,9 @@ int enqueue_vio_update(flb_handle* h, const flb_vio_params* prm) {
     }
     VioParamsDev d;
     to_dev_params(prm, d);
-    VioSolveArgs s{};
-    s.state = &h->states.p[0];
-    s.state_prop = &h->states.p[1];
-    s.old_state = &h->states.p[2];
-    s.ctrl = h->vio_ctrl.p;
-    s.prior = h->prior.p;
-    s.G_last = h->G_last.p;
-    s.partials = h->partials.p;
-    s.nblocks = vio_nblocks(h);
-    s.errors = h->errors.p;
-    s.err_stride = h->err_stride;
-    s.Pn_total = h->Pn;
-    s.prm = d;
+    const FrameBufs fb = handle_frame(h);
+    VioSolveArgs s = make_vio_solve_args(h, d, fb);
     s.p2p = h->p2p;
-    s.timeout_flag = &h->barrier.p->timeout;
     { int rcq = vio_inputs_acquire(h); if (rcq) return rcq; }
     const bool fused = h->p2p.world > 1;
     if (fused && !h->cfg.persistent)
@@ -924,29 +1026,13 @@ int enqueue_vio_update(flb_handle* h, const flb_vio_params* prm) {
         FLB_CUDA(h, cudaGetLastError());
     }
     if (prm->max_iteration > 0) h->err_from_sel = false;        // the passes below write sub_sparse_map->errors (:851)
-    VioArgs a{};
-    a.img = h->img.p;
-    a.cam = h->cam;
-    a.pos = h->patch_pos.p;
-    a.patch = h->patch_ref.p;
-    a.search_level = h->patch_level.p;
-    a.Pn = h->Pn;
-    a.state = &h->states.p[0];
-    a.pose_override = nullptr;
-    a.prm = d;
-    a.ctrl = h->vio_ctrl.p;
-    a.force_level = -1;
-    a.errors = h->errors.p;
-    a.err_stride = h->err_stride;
-    a.partials = h->partials.p;
+    VioArgs a = make_vio_args(h, d, fb);
     a.p2p = h->p2p;
-    a.Pn_dev = nullptr;
     if (h->pn_on_device) {                   // capacity = one patch per grid cell; the kernel reads the real count
         a.Pn = h->vm.prm.length;
         a.Pn_dev = h->vm.counters.p + VM_N_SEL;
         s.Pn_total = a.Pn;
     }
-    const int nb = vio_nblocks(h);
     static const int env_defer = [] { const char* e = getenv("FLB_DEFER"); return e ? atoi(e) : 1; }();
     if (persistent && !fused && env_defer) {
         // per-patch errors as self-validating units (zeroed once per allocation: a tag always has its top bit set)
@@ -1003,34 +1089,11 @@ int enqueue_vio_update(flb_handle* h, const flb_vio_params* prm) {
         FLB_CUDA(h, cudaLaunchCooperativeKernel((void*)k_vio_update_persistent<kVioPersBlock>, dim3(grid), dim3(kVioPersBlock), args, dyn,
                                                 h->stream));
         h->last_vio_valid = false;
-        return vio_inputs_release(h);
+        return FLB_OK;
     }
-    const int total = 3 * std::max(prm->max_iteration, 0);
-    for (int it = 0; it < total && h->Pn > 0; ++it) {
-        {
-            LaunchScope ls(h, FAM_VIO);
-            k_vio_pass<kVioBlock><<<nb, kVioBlock, 0, h->stream>>>(a);
-            FLB_CUDA(h, cudaGetLastError());
-        }
-        if (h->comm) {
-            int rc = allreduce_packed(h, h->partials.p, nb, kVioPacked);
-            if (rc) return rc;
-            s.partials = h->packed.p;
-            s.nblocks = 1;
-            // gather every rank's per-patch errors in patch order (shards padded to errors.cap/world)
-            const size_t shard = (size_t)h->err_shard;
-            int r = g_nccl.AllGather(h->errors.p, h->errors_all.p, shard, kNcclFloat32, h->comm, h->stream);
-            if (r != 0) return fail(h, FLB_ERR_COMM, "ncclAllGather failed");
-            h->launches++;
-            s.errors = h->errors_all.p;
-            s.Pn_total = (int)(shard * (size_t)h->world);
-        }
-        LaunchScope ls(h, FAM_SOLVE);
-        k_vio_finalize<<<1, kLeaderBlock, 0, h->stream>>>(s);
-        FLB_CUDA(h, cudaGetLastError());
-    }
+    { int rc = vio_pass_loop(h, a, s, 3 * std::max(prm->max_iteration, 0)); if (rc) return rc; }
     h->last_vio_valid = false;
-    return vio_inputs_release(h);
+    return FLB_OK;
 }
 
 void fill_lio_report(const LioCtrl& c, flb_lio_report* rep) {
@@ -1048,6 +1111,28 @@ void fill_vio_report(const VioCtrl& c, flb_vio_report* rep) {
     rep->skipped_last = c.skipped_last;
     rep->cov_updated = c.cov_updated;
     rep->status = c.status;
+}
+
+// A persistent kernel whose grid barrier timed out has set GridBarrier::timeout.  `bar` is the barrier as read back:
+// when it is set, clear the device barrier for the next launch and report the timeout.
+int watchdog_check(flb_handle* h, const char* bar) {
+    GridBarrier b;
+    std::memcpy(&b, bar, sizeof(b));
+    if (!b.timeout) return FLB_OK;
+    cudaMemset(h->barrier.p, 0, sizeof(GridBarrier));
+    return fail(h, FLB_ERR_TIMEOUT, "device-side grid barrier watchdog tripped");
+}
+
+// The result block {State18, LioCtrl, VioCtrl, GridBarrier} as flb_state_download and k_pack_result lay it out.
+constexpr size_t kResLio = sizeof(State18), kResVio = kResLio + sizeof(LioCtrl), kResBarrier = kResVio + sizeof(VioCtrl);
+constexpr size_t kResBytes = kResBarrier + sizeof(GridBarrier);
+
+int read_result(flb_handle* h, const char* po, flb_state18* x, flb_lio_report* lio, flb_vio_report* vio) {
+    { int rc = watchdog_check(h, po + kResBarrier); if (rc) return rc; }
+    if (x) std::memcpy(x, po, sizeof(State18));
+    if (lio) { LioCtrl c; std::memcpy(&c, po + kResLio, sizeof(c)); fill_lio_report(c, lio); }
+    if (vio) { VioCtrl c; std::memcpy(&c, po + kResVio, sizeof(c)); fill_vio_report(c, vio); }
+    return FLB_OK;
 }
 
 }  // namespace
@@ -2535,8 +2620,7 @@ int flb_visual_candidates(flb_handle* h, const double Rcw[9], const double Pcw[3
     FLB_CHECK_H(h);
     if (!Rcw || !Pcw || n < 0 || (n > 0 && !world_xyz) || stride < 3 || grid_size < 1 || border < 0 || !map_value || !winner)
         return fail(h, FLB_ERR_INVALID, "flb_visual_candidates: bad arguments");
-    if (!h->cam_set || h->img_w <= 0) return fail(h, FLB_ERR_STATE, "flb_visual_candidates: camera and image must be set first");
-    if (h->cam.width != h->img_w || h->cam.height != h->img_h) return fail(h, FLB_ERR_STATE, "camera / image size mismatch");
+    { int rc = vio_image_check(h, "flb_visual_candidates"); if (rc) return rc; }
     const int gw = h->img_w / grid_size, gh = h->img_h / grid_size, ncell = gw * gh;      // :55-57
     if (ncell < 1) return fail(h, FLB_ERR_INVALID, "flb_visual_candidates: grid_size larger than the image");
     { int rcq = vio_inputs_acquire(h); if (rcq) return rcq; }                           // the image upload has landed
@@ -2581,7 +2665,7 @@ int flb_visual_candidates(flb_handle* h, const double Rcw[9], const double Pcw[3
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
     std::memcpy(map_value, po, (size_t)ncell * sizeof(float));
     std::memcpy(winner, po + (size_t)ncell * sizeof(float), (size_t)ncell * sizeof(int));
-    return vio_inputs_release(h);
+    return FLB_OK;
 }
 
 // pcl::VoxelGrid of n >= 1 finite points already on the device (xyz, packed): k_bbox -> k_vg_keys -> radix sort ->
@@ -2944,16 +3028,18 @@ int flb_lio_pass(flb_handle* h, const flb_lio_params* prm, const double R[9], co
     FLB_CUDA(h, h->x_meas.reserve(N));
     LioParamsDev d;
     to_dev_params(prm, d);
-    void* stv = nullptr;
-    FLB_CUDA(h, h->st_misc.acquire(12 * sizeof(double), &stv));
-    double* st = static_cast<double*>(stv);
-    std::memcpy(st, R, 9 * sizeof(double));
-    std::memcpy(st + 9, p, 3 * sizeof(double));
-    FLB_CUDA(h, cudaMemcpyAsync(h->pose12.p, st, 12 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    FLB_CUDA(h, h->st_misc.mark(h->stream));
-    LioArgs a = make_lio_args(h, d, true, width);
+    { int rcp = upload_pose(h, h->pose12.p, R, p); if (rcp) return rcp; }
+    LioArgs a = make_lio_args(h, d, handle_frame(h));
     a.force_rematch = rematch ? 1 : 0;
     a.pose_override = h->pose12.p;
+    a.x_world = h->x_world.p;
+    a.x_nn_idx = h->x_nn_idx.p;
+    a.x_nn_d2 = h->x_nn_d2.p;
+    a.x_pabcd = h->x_pabcd.p;
+    a.x_pd2 = h->x_pd2.p;
+    a.x_rowmask = h->x_rowmask.p;
+    a.x_rows = h->x_rows.p;
+    a.x_meas = h->x_meas.p;
     int rc = launch_lio_pass(h, a, width, rematch != 0);
     if (rc) return rc;
     note_lio_pass(h);
@@ -2971,14 +3057,7 @@ int flb_lio_pass(flb_handle* h, const flb_lio_params* prm, const double R[9], co
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
     std::memset(out, 0, sizeof(*out));
     out->width = width;
-    int k = 0;
-    for (int r = 0; r < width; ++r)
-        for (int c = r; c < width; ++c) {
-            out->HTH[r * width + c] = po[k];
-            out->HTH[c * width + r] = po[k];
-            ++k;
-        }
-    for (int r = 0; r < width; ++r) out->HTh[r] = po[k + r];
+    unpack_normal_eq(po, width, out->HTH, out->HTh);
     out->n_eff = (int)po[K - 2];
     out->sum_abs_res = po[K - 1];
     h->last_pass_width = width;
@@ -3064,32 +3143,11 @@ int flb_state_download(flb_handle* h, flb_state18* x, flb_lio_report* lio, flb_v
     { int rcf = flush_state_ops(h); if (rcf) return rcf; }
     char* po = static_cast<char*>(h->pin_out.p);
     FLB_CUDA(h, cudaMemcpyAsync(po, &h->states.p[0], sizeof(State18), cudaMemcpyDeviceToHost, h->stream));
-    FLB_CUDA(h, cudaMemcpyAsync(po + sizeof(State18), h->lio_ctrl.p, sizeof(LioCtrl), cudaMemcpyDeviceToHost, h->stream));
-    FLB_CUDA(h, cudaMemcpyAsync(po + sizeof(State18) + sizeof(LioCtrl), h->vio_ctrl.p, sizeof(VioCtrl), cudaMemcpyDeviceToHost,
-                                h->stream));
-    FLB_CUDA(h, cudaMemcpyAsync(po + sizeof(State18) + sizeof(LioCtrl) + sizeof(VioCtrl), h->barrier.p, sizeof(GridBarrier),
-                                cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaMemcpyAsync(po + kResLio, h->lio_ctrl.p, sizeof(LioCtrl), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaMemcpyAsync(po + kResVio, h->vio_ctrl.p, sizeof(VioCtrl), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaMemcpyAsync(po + kResBarrier, h->barrier.p, sizeof(GridBarrier), cudaMemcpyDeviceToHost, h->stream));
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    {
-        GridBarrier b;
-        std::memcpy(&b, po + sizeof(State18) + sizeof(LioCtrl) + sizeof(VioCtrl), sizeof(b));
-        if (b.timeout) {
-            cudaMemset(h->barrier.p, 0, sizeof(GridBarrier));
-            return fail(h, FLB_ERR_TIMEOUT, "device-side grid barrier watchdog tripped");
-        }
-    }
-    if (x) std::memcpy(x, po, sizeof(State18));
-    if (lio) {
-        LioCtrl c;
-        std::memcpy(&c, po + sizeof(State18), sizeof(c));
-        fill_lio_report(c, lio);
-    }
-    if (vio) {
-        VioCtrl c;
-        std::memcpy(&c, po + sizeof(State18) + sizeof(LioCtrl), sizeof(c));
-        fill_vio_report(c, vio);
-    }
-    return FLB_OK;
+    return read_result(h, po, x, lio, vio);
 }
 
 // Pipelined result read-back: enqueue the copy of (state, reports) of everything enqueued so far into result slot
@@ -3100,8 +3158,7 @@ int flb_state_download_enqueue(flb_handle* h, int slot) {
     if (slot < 0 || slot > 1) return fail(h, FLB_ERR_INVALID, "flb_state_download_enqueue: slot must be 0 or 1");
     if (!h->state_valid) return fail(h, FLB_ERR_STATE, "flb_state_download_enqueue: no state uploaded");
     { int rcf = flush_state_ops(h); if (rcf) return rcf; }
-    const size_t bytes = sizeof(State18) + sizeof(LioCtrl) + sizeof(VioCtrl) + sizeof(GridBarrier);
-    FLB_CUDA(h, h->pin_res[slot].reserve(bytes));
+    FLB_CUDA(h, h->pin_res[slot].reserve(kResBytes));
     if (!h->ev_res[slot]) FLB_CUDA(h, cudaEventCreateWithFlags(&h->ev_res[slot], cudaEventDisableTiming));
     char* po = static_cast<char*>(h->pin_res[slot].p);
     {
@@ -3125,17 +3182,7 @@ int flb_state_download_wait(flb_handle* h, int slot, flb_state18* x, flb_lio_rep
     if (slot < 0 || slot > 1 || !h->res_pending[slot]) return fail(h, FLB_ERR_STATE, "flb_state_download_wait: nothing enqueued in this slot");
     FLB_CUDA(h, cudaEventSynchronize(h->ev_res[slot]));
     h->res_pending[slot] = false;
-    const char* po = static_cast<const char*>(h->pin_res[slot].p);
-    GridBarrier b;
-    std::memcpy(&b, po + sizeof(State18) + sizeof(LioCtrl) + sizeof(VioCtrl), sizeof(b));
-    if (b.timeout) {
-        cudaMemset(h->barrier.p, 0, sizeof(GridBarrier));
-        return fail(h, FLB_ERR_TIMEOUT, "device-side grid barrier watchdog tripped");
-    }
-    if (x) std::memcpy(x, po, sizeof(State18));
-    if (lio) { LioCtrl c; std::memcpy(&c, po + sizeof(State18), sizeof(c)); fill_lio_report(c, lio); }
-    if (vio) { VioCtrl c; std::memcpy(&c, po + sizeof(State18) + sizeof(LioCtrl), sizeof(c)); fill_vio_report(c, vio); }
-    return FLB_OK;
+    return read_result(h, static_cast<const char*>(h->pin_res[slot].p), x, lio, vio);
 }
 
 int flb_lio_update_enqueue(flb_handle* h, const flb_lio_params* prm) {
@@ -3201,7 +3248,7 @@ int flb_lio_update_ikfom(flb_handle* h, const flb_ikfom_params* prm, flb_state_i
     FLB_CUDA(h, h->st_state.mark(h->stream));
     FLB_CUDA(h, cudaMemcpyAsync(&h->ik_states.p[1], &h->ik_states.p[0], sizeof(StateIkfom), cudaMemcpyDeviceToDevice, h->stream));
     LioParamsDev d{};            // the extrinsic comes from the state every pass; only plane_thr / grid matter here
-    LioArgs a = make_lio_args(h, d, false, 12);
+    LioArgs a = make_lio_args(h, d, handle_frame(h));
     IkfomSolveArgs s{};
     s.state = &h->ik_states.p[0];
     s.state_prop = &h->ik_states.p[1];
@@ -3234,12 +3281,7 @@ int flb_lio_update_ikfom(flb_handle* h, const flb_ikfom_params* prm, flb_state_i
     FLB_CUDA(h, cudaMemcpyAsync(po + sizeof(StateIkfom) + sizeof(IkfomCtrl), h->barrier.p, sizeof(GridBarrier), cudaMemcpyDeviceToHost,
                                 h->stream));
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    GridBarrier b;
-    std::memcpy(&b, po + sizeof(StateIkfom) + sizeof(IkfomCtrl), sizeof(b));
-    if (b.timeout) {
-        cudaMemset(h->barrier.p, 0, sizeof(GridBarrier));
-        return fail(h, FLB_ERR_TIMEOUT, "device-side grid barrier watchdog tripped");
-    }
+    { int rcw = watchdog_check(h, po + sizeof(StateIkfom) + sizeof(IkfomCtrl)); if (rcw) return rcw; }
     std::memcpy(x, po, sizeof(StateIkfom));
     IkfomCtrl c;
     std::memcpy(&c, po + sizeof(StateIkfom), sizeof(c));
@@ -3416,8 +3458,7 @@ int flb_camera_set(flb_handle* h, const flb_camera* cam) {
 int flb_vio_pass(flb_handle* h, const flb_vio_params* prm, const double R[9], const double p[3], int level, flb_vio_eq* out) {
     FLB_CHECK_H(h);
     if (!prm || !R || !p || !out || level < 0 || level > 2) return fail(h, FLB_ERR_INVALID, "flb_vio_pass: bad arguments");
-    if (!h->cam_set || h->img_w <= 0) return fail(h, FLB_ERR_STATE, "flb_vio_pass: camera and image must be set first");
-    if (h->cam.width != h->img_w || h->cam.height != h->img_h) return fail(h, FLB_ERR_STATE, "camera / image size mismatch");
+    { int rc = vio_image_check(h, "flb_vio_pass"); if (rc) return rc; }
     std::memset(out, 0, sizeof(*out));
     { int rcp = resolve_pn(h); if (rcp) return rcp; }
     if (h->Pn == 0) return FLB_OK;
@@ -3427,28 +3468,10 @@ int flb_vio_pass(flb_handle* h, const flb_vio_params* prm, const double R[9], co
     FLB_CUDA(h, h->x_H.reserve(Pn * 64 * 6));
     VioParamsDev d;
     to_dev_params(prm, d);
-    void* stv = nullptr;
-    FLB_CUDA(h, h->st_misc.acquire(12 * sizeof(double), &stv));
-    double* st = static_cast<double*>(stv);
-    std::memcpy(st, R, 9 * sizeof(double));
-    std::memcpy(st + 9, p, 3 * sizeof(double));
-    FLB_CUDA(h, cudaMemcpyAsync(h->pose12.p, st, 12 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    FLB_CUDA(h, h->st_misc.mark(h->stream));
-    VioArgs a{};
-    a.img = h->img.p;
-    a.cam = h->cam;
-    a.pos = h->patch_pos.p;
-    a.patch = h->patch_ref.p;
-    a.search_level = h->patch_level.p;
-    a.Pn = h->Pn;
-    a.state = &h->states.p[0];
+    { int rcp = upload_pose(h, h->pose12.p, R, p); if (rcp) return rcp; }
+    VioArgs a = make_vio_args(h, d, handle_frame(h));
     a.pose_override = h->pose12.p;
-    a.prm = d;
-    a.ctrl = h->vio_ctrl.p;
     a.force_level = level;
-    a.errors = h->errors.p;
-    a.err_stride = h->err_stride;
-    a.partials = h->partials.p;
     a.x_z = h->x_z.p;
     a.x_H = h->x_H.p;
     const int nb = vio_nblocks(h);
@@ -3462,21 +3485,13 @@ int flb_vio_pass(flb_handle* h, const flb_vio_params* prm, const double R[9], co
         k_reduce_only<<<1, 32, 0, h->stream>>>(h->partials.p, nb, kVioPacked, h->packed.p);
         FLB_CUDA(h, cudaGetLastError());
     }
-    { int rcq = vio_inputs_release(h); if (rcq) return rcq; }
     FLB_CUDA(h, h->pin_out.reserve(kVioPacked * sizeof(double) + Pn * sizeof(float)));
     double* po = static_cast<double*>(h->pin_out.p);
     float* pe = reinterpret_cast<float*>(po + kVioPacked);
     FLB_CUDA(h, cudaMemcpyAsync(po, h->packed.p, kVioPacked * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     FLB_CUDA(h, cudaMemcpyAsync(pe, h->errors.p, Pn * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    int k = 0;
-    for (int r = 0; r < 6; ++r)
-        for (int c = r; c < 6; ++c) {
-            out->HTH[r * 6 + c] = po[k];
-            out->HTH[c * 6 + r] = po[k];
-            ++k;
-        }
-    for (int r = 0; r < 6; ++r) out->HTz[r] = po[21 + r];
+    unpack_normal_eq(po, 6, out->HTH, out->HTz);
     out->n_meas = (int64_t)po[27];
     out->skipped = (int)po[28];
     // error = sum_i errors[i] (float, patch order) / n_meas  (src/lidar_selection.cpp:852,857)
@@ -3519,8 +3534,7 @@ int flb_vio_update_level(flb_handle* h, const flb_vio_params* prm, int level, fl
                          const flb_state18* x_prop, float* last_error, double* G18x6, flb_vio_report* rep) {
     FLB_CHECK_H(h);
     if (!prm || !x || !x_prop || level < 0 || level > 2) return fail(h, FLB_ERR_INVALID, "flb_vio_update_level: bad arguments");
-    if (!h->cam_set || h->img_w <= 0) return fail(h, FLB_ERR_STATE, "flb_vio_update_level: camera and image must be set first");
-    if (h->cam.width != h->img_w || h->cam.height != h->img_h) return fail(h, FLB_ERR_STATE, "camera / image size mismatch");
+    { int rcc = vio_image_check(h, "flb_vio_update_level"); if (rcc) return rcc; }
     if (h->comm || h->p2p.world > 1) return fail(h, FLB_ERR_STATE, "flb_vio_update_level: single GPU");
     { int rcp = resolve_pn(h); if (rcp) return rcp; }
     if (last_error) *last_error = 0.f;                               // :746 (total_points == 0 returns 0.)
@@ -3532,58 +3546,23 @@ int flb_vio_update_level(flb_handle* h, const flb_vio_params* prm, int level, fl
     to_dev_params(prm, d);
     d.single_level = 1;
     { int rcq = vio_inputs_acquire(h); if (rcq) return rcq; }
-    VioSolveArgs s{};
-    s.state = &h->states.p[0];
-    s.state_prop = &h->states.p[1];
-    s.old_state = &h->states.p[2];
-    s.ctrl = h->vio_ctrl.p;
-    s.prior = h->prior.p;
-    s.G_last = h->G_last.p;
-    s.partials = h->partials.p;
-    s.nblocks = vio_nblocks(h);
-    s.errors = h->errors.p;
-    s.err_stride = h->err_stride;
-    s.Pn_total = h->Pn;
-    s.prm = d;
-    s.timeout_flag = &h->barrier.p->timeout;
-    VioArgs a{};
-    a.img = h->img.p;
-    a.cam = h->cam;
-    a.pos = h->patch_pos.p;
-    a.patch = h->patch_ref.p;
-    a.search_level = h->patch_level.p;
-    a.Pn = h->Pn;
-    a.state = &h->states.p[0];
-    a.prm = d;
-    a.ctrl = h->vio_ctrl.p;
-    a.force_level = -1;
-    a.errors = h->errors.p;
-    a.err_stride = h->err_stride;
-    a.partials = h->partials.p;
+    const FrameBufs fb = handle_frame(h);
+    const VioSolveArgs s = make_vio_solve_args(h, d, fb);
+    const VioArgs a = make_vio_args(h, d, fb);
     {
         LaunchScope ls(h, FAM_SOLVE);
         k_vio_begin_level<<<1, 32, 0, h->stream>>>(h->vio_ctrl.p, h->Pn, level, total_residual);
         FLB_CUDA(h, cudaGetLastError());
     }
     if (prm->max_iteration > 0) h->err_from_sel = false;
-    const int nb = vio_nblocks(h);
-    for (int it = 0; it < std::max(prm->max_iteration, 0); ++it) {      // later launches return at once when the level has ended
-        {
-            LaunchScope ls(h, FAM_VIO);
-            k_vio_pass<kVioBlock><<<nb, kVioBlock, 0, h->stream>>>(a);
-            FLB_CUDA(h, cudaGetLastError());
-        }
-        LaunchScope ls(h, FAM_SOLVE);
-        k_vio_finalize<<<1, kLeaderBlock, 0, h->stream>>>(s);
-        FLB_CUDA(h, cudaGetLastError());
-    }
+    // later passes return at once when the level has ended
+    { int rcl = vio_pass_loop(h, a, s, std::max(prm->max_iteration, 0)); if (rcl) return rcl; }
     if (G18x6) {
         LaunchScope ls(h, FAM_SOLVE);
         k_vio_export_gain<<<1, kLeaderBlock, 0, h->stream>>>(s, h->packed.p);
         FLB_CUDA(h, cudaGetLastError());
         FLB_CUDA(h, cudaMemcpyAsync(G18x6, h->packed.p, 108 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     }
-    { int rcq = vio_inputs_release(h); if (rcq) return rcq; }
     h->last_vio_valid = false;
     rc = flb_state_download(h, x, nullptr, &r);
     if (rc) return rc;
@@ -3884,8 +3863,7 @@ int flb_batch_update_enqueue(flb_handle* h, const flb_lio_params* lprm, const fl
     const int B = b.B;
     const bool vio = vprm != nullptr && h->Pn > 0 && vprm->max_iteration > 0;
     if (vio) {
-        if (!h->cam_set || h->img_w <= 0) return fail(h, FLB_ERR_STATE, "flb_batch_update_enqueue: camera and image must be set first");
-        if (h->cam.width != h->img_w || h->cam.height != h->img_h) return fail(h, FLB_ERR_STATE, "camera / image size mismatch");
+        { int rc = vio_image_check(h, "flb_batch_update_enqueue"); if (rc) return rc; }
         if (h->pn_on_device) { int rc = resolve_pn(h); if (rc) return rc; }
     }
     const int nb_lio = (b.n_max + kLioBlock - 1) / kLioBlock;
@@ -3894,39 +3872,20 @@ int flb_batch_update_enqueue(flb_handle* h, const flb_lio_params* lprm, const fl
     FLB_CUDA(h, b.partials.reserve((size_t)B * b.partials_per));
     const int estride = std::max(h->Pn, 1);
     FLB_CUDA(h, b.errors.reserve((size_t)B * 2 * estride));
+    // frame i's slice of the batch buffers
+    auto frame = [&](int i) -> FrameBufs {
+        const size_t off = (size_t)i * b.n_cap;
+        return {b.scan.p + off, b.N[i], b.states.p + (size_t)i * 5, b.lio_ctrl.p + i, b.vio_ctrl.p + i, b.prior.p + i, b.sel.p + off,
+                b.plane.p + off, b.plane_ok.p + off, b.partials.p + (size_t)i * b.partials_per, b.errors.p + (size_t)i * 2 * estride,
+                estride, b.G_last.p + (size_t)i * 108};
+    };
     LioParamsDev ld;
     to_dev_params(lprm, ld);
     std::vector<LioArgs> la(B);
     std::vector<LioSolveArgs> ls(B);
     for (int i = 0; i < B; ++i) {
-        const size_t off = (size_t)i * b.n_cap;
-        LioArgs a{};
-        a.scan = b.scan.p + off;
-        a.N = b.N[i];
-        a.grid = h->grid;
-        a.cell_start = cell_index(h);
-        a.map_pts = h->map_pts.p;
-        a.state = b.states.p + (size_t)i * 5;
-        a.prm = ld;
-        a.plane_thr = (float)h->cfg.plane_threshold;
-        a.ctrl = b.lio_ctrl.p + i;
-        a.force_rematch = -1;
-        a.sel = b.sel.p + off;
-        a.plane = b.plane.p + off;
-        a.plane_ok = b.plane_ok.p + off;
-        a.partials = b.partials.p + (size_t)i * b.partials_per;
-        a.M = h->M;
-        la[i] = a;
-        LioSolveArgs s{};
-        s.state = b.states.p + (size_t)i * 5;
-        s.state_prop = s.state + 1;
-        s.ctrl = b.lio_ctrl.p + i;
-        s.prior = b.prior.p + i;
-        s.partials = a.partials;
-        s.nblocks = (b.N[i] + kLioBlock - 1) / kLioBlock;
-        s.prm = ld;
-        s.timeout_flag = &h->barrier.p->timeout;
-        ls[i] = s;
+        la[i] = make_lio_args(h, ld, frame(i));
+        ls[i] = make_lio_solve_args(h, ld, frame(i));
     }
     // argument tables: pageable -> device through the stream (small; ordered before the launches that read them)
     FLB_CUDA(h, cudaMemcpyAsync(b.lio_args.p, la.data(), B * sizeof(LioArgs), cudaMemcpyHostToDevice, h->stream));
@@ -3960,36 +3919,8 @@ int flb_batch_update_enqueue(flb_handle* h, const flb_lio_params* lprm, const fl
     std::vector<VioArgs> va(B);
     std::vector<VioSolveArgs> vs(B);
     for (int i = 0; i < B; ++i) {
-        VioArgs a{};
-        a.img = h->img.p;
-        a.cam = h->cam;
-        a.pos = h->patch_pos.p;
-        a.patch = h->patch_ref.p;
-        a.search_level = h->patch_level.p;
-        a.Pn = h->Pn;
-        a.state = b.states.p + (size_t)i * 5;
-        a.prm = vd;
-        a.ctrl = b.vio_ctrl.p + i;
-        a.force_level = -1;
-        a.errors = b.errors.p + (size_t)i * 2 * estride;
-        a.err_stride = estride;
-        a.partials = b.partials.p + (size_t)i * b.partials_per;
-        va[i] = a;
-        VioSolveArgs s{};
-        s.state = b.states.p + (size_t)i * 5;
-        s.state_prop = s.state + 1;
-        s.old_state = s.state + 2;
-        s.ctrl = b.vio_ctrl.p + i;
-        s.prior = b.prior.p + i;
-        s.G_last = b.G_last.p + (size_t)i * 108;
-        s.partials = a.partials;
-        s.nblocks = nb_vio;
-        s.errors = a.errors;
-        s.err_stride = estride;
-        s.Pn_total = h->Pn;
-        s.prm = vd;
-        s.timeout_flag = &h->barrier.p->timeout;
-        vs[i] = s;
+        va[i] = make_vio_args(h, vd, frame(i));
+        vs[i] = make_vio_solve_args(h, vd, frame(i));
     }
     FLB_CUDA(h, cudaMemcpyAsync(b.vio_args.p, va.data(), B * sizeof(VioArgs), cudaMemcpyHostToDevice, h->stream));
     FLB_CUDA(h, cudaMemcpyAsync(b.vio_solve.p, vs.data(), B * sizeof(VioSolveArgs), cudaMemcpyHostToDevice, h->stream));
@@ -4010,7 +3941,7 @@ int flb_batch_update_enqueue(flb_handle* h, const flb_lio_params* lprm, const fl
         k_vio_finalize_batched<<<B, kLeaderBlock, 0, h->stream>>>(b.vio_solve.p);
         FLB_CUDA(h, cudaGetLastError());
     }
-    return vio_inputs_release(h);
+    return FLB_OK;
 }
 
 int flb_batch_state_download(flb_handle* h, int frame, flb_state18* x, flb_lio_report* lio, flb_vio_report* vio) {
@@ -4039,28 +3970,17 @@ namespace {
 
 int vm_check(flb_handle* h, const char* who) {
     if (!h->vm.on) return fail(h, FLB_ERR_STATE, "%s: flb_vmap_reset first", who);
-    if (!h->cam_set || h->img_w <= 0) return fail(h, FLB_ERR_STATE, "%s: camera and image must be set first", who);
-    if (h->cam.width != h->img_w || h->cam.height != h->img_h) return fail(h, FLB_ERR_STATE, "camera / image size mismatch");
-    return FLB_OK;
+    return vio_image_check(h, who);
 }
 
 // Upload (or derive from the device state) T_f_w of the current frame into vm.pose.
 int vm_set_pose(flb_handle* h, const double* Rcw, const double* Pcw) {
-    if (Rcw && Pcw) {
-        void* stv = nullptr;
-        FLB_CUDA(h, h->st_misc.acquire(12 * sizeof(double), &stv));
-        double* st = static_cast<double*>(stv);
-        std::memcpy(st, Rcw, 9 * sizeof(double));
-        std::memcpy(st + 9, Pcw, 3 * sizeof(double));
-        FLB_CUDA(h, cudaMemcpyAsync(h->vm.pose.p, st, 12 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-        FLB_CUDA(h, h->st_misc.mark(h->stream));
-    } else {
-        if (!h->state_valid) return fail(h, FLB_ERR_STATE, "visual map: no pose given and no device state");
-        { int rcf = flush_state_ops(h); if (rcf) return rcf; }
-        LaunchScope ls(h, FAM_OTHER);
-        k_vm_pose_from_state<<<1, 32, 0, h->stream>>>(&h->states.p[0], h->vm.rci.p, h->vm.pose.p);
-        FLB_CUDA(h, cudaGetLastError());
-    }
+    if (Rcw && Pcw) return upload_pose(h, h->vm.pose.p, Rcw, Pcw);
+    if (!h->state_valid) return fail(h, FLB_ERR_STATE, "visual map: no pose given and no device state");
+    { int rcf = flush_state_ops(h); if (rcf) return rcf; }
+    LaunchScope ls(h, FAM_OTHER);
+    k_vm_pose_from_state<<<1, 32, 0, h->stream>>>(&h->states.p[0], h->vm.rci.p, h->vm.pose.p);
+    FLB_CUDA(h, cudaGetLastError());
     return FLB_OK;
 }
 
@@ -4254,7 +4174,6 @@ int vm_select_dev(flb_handle* h, const float* pg_down, int n, const int* n_dev, 
         FLB_CUDA(h, cudaGetLastError());
         h->launches += 5;
     }
-    { int rcq = vio_inputs_release(h); if (rcq) return rcq; }
     h->pn_on_device = true;
     h->patches_set = true;
     h->err_from_sel = true;
@@ -4370,7 +4289,7 @@ int vm_grow_dev(flb_handle* h, const float* pg, int n, int frame_id) {
     vm.pts_ub += L;
     vm.fts_ub += L;
     vm.img_ub += 1;
-    return vio_inputs_release(h);
+    return FLB_OK;
 }
 
 }  // namespace
@@ -4420,7 +4339,7 @@ int flb_vmap_add_observations(flb_handle* h, const double Rcw[9], const double P
     }
     vm.fts_ub += L;
     vm.img_ub += 1;
-    return vio_inputs_release(h);
+    return FLB_OK;
 }
 
 }  // extern "C"
@@ -4548,7 +4467,7 @@ int flb_keypatch_image(flb_handle* h, const double Rcw[9], const double Pcw[3], 
         else *n_patches = h->Pn;
     }
     if (!is_pinned(bgr_out)) FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    return vio_inputs_release(h);
+    return FLB_OK;
 }
 
 int flb_vmap_counts(flb_handle* h, int* points, int* features, int* images, int* selected, int* last_added) {
