@@ -104,6 +104,70 @@ struct Staging {
     }
 };
 
+// The visual map's coordinate limit: 2^20 voxels of its 0.5 m key on either side of the origin.
+constexpr float kVmapCoordLimit = 5.0e5f;
+
+// n caller points of `stride` floats (x, y, z first) into dst as packed xyz.
+void pack_points(float* dst, const float* src, int n, int stride) {
+    if (stride == 3) {
+        if (n > 0) std::memcpy(dst, src, (size_t)n * 3 * sizeof(float));
+        return;
+    }
+    for (int i = 0; i < n; ++i) {
+        dst[3 * (size_t)i] = src[(size_t)i * stride];
+        dst[3 * (size_t)i + 1] = src[(size_t)i * stride + 1];
+        dst[3 * (size_t)i + 2] = src[(size_t)i * stride + 2];
+    }
+}
+
+// Bounds lo (and, HI, hi) of n packed xyz points; true when a coordinate is non-finite.  24 floats (= 8 points) at a
+// time into 24 independent accumulators: no cross-iteration dependency, so the host compiler vectorises the inner loop
+// as it stands.  A NaN updates no bound; the returned flag covers it.
+template <bool HI>
+bool fold_points(const float* xyz, int n, float lo[3], float* hi) {
+    float mn[24], mx[24];
+    for (int j = 0; j < 24; ++j) { mn[j] = INFINITY; mx[j] = -INFINITY; }
+    unsigned bad = 0;
+    const size_t n3 = (size_t)n * 3;
+    size_t i = 0;
+    for (; i + 24 <= n3; i += 24)
+        for (int j = 0; j < 24; ++j) {
+            const float v = xyz[i + j];
+            unsigned bits;
+            std::memcpy(&bits, &v, sizeof(bits));
+            bad |= ((bits & 0x7F800000u) == 0x7F800000u) ? 1u : 0u;
+            mn[j] = v < mn[j] ? v : mn[j];
+            if (HI) mx[j] = v > mx[j] ? v : mx[j];
+        }
+    for (; i < n3; ++i) {
+        const float v = xyz[i];
+        const int j = (int)(i % 24);
+        bad |= std::isfinite(v) ? 0u : 1u;
+        mn[j] = v < mn[j] ? v : mn[j];
+        if (HI) mx[j] = v > mx[j] ? v : mx[j];
+    }
+    for (int k = 0; k < 3; ++k) {
+        lo[k] = INFINITY;
+        if (HI) hi[k] = -INFINITY;
+    }
+    for (int j = 0; j < 24; ++j) {
+        lo[j % 3] = std::min(lo[j % 3], mn[j]);
+        if (HI) hi[j % 3] = std::max(hi[j % 3], mx[j]);
+    }
+    return bad != 0;
+}
+
+// The first of n packed xyz points with a coordinate that is non-finite or beyond +-limit, -1 if none: the index a
+// refusal names, rescanned only once a fold has found the input bad.
+int first_bad_point(const float* xyz, int n, float limit) {
+    for (int i = 0; i < n; ++i)
+        for (int k = 0; k < 3; ++k) {
+            const float v = xyz[3 * (size_t)i + k];
+            if (!std::isfinite(v) || std::fabs(v) > limit) return i;
+        }
+    return -1;
+}
+
 // ---- NCCL through dlopen (no link-time dependency) ----------------------------------
 typedef struct ncclComm* ncclComm_t;
 typedef struct { char internal[128]; } ncclUniqueId;
@@ -1456,16 +1520,10 @@ int flb_map_upload(flb_handle* h, const float* xyz, int M, int stride) {
     void* stv = nullptr;
     FLB_CUDA(h, h->st_map.acquire((size_t)M * 3 * sizeof(float), &stv));
     float* st = static_cast<float*>(stv);
-    float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-    for (int i = 0; i < M; ++i) {
-        for (int k = 0; k < 3; ++k) {
-            const float v = xyz[(size_t)i * stride + k];
-            if (!std::isfinite(v)) return fail(h, FLB_ERR_INVALID, "flb_map_upload: non-finite coordinate at point %d", i);
-            st[3 * (size_t)i + k] = v;
-            lo[k] = std::min(lo[k], v);
-            hi[k] = std::max(hi[k], v);
-        }
-    }
+    pack_points(st, xyz, M, stride);
+    float lo[3], hi[3];
+    if (fold_points<true>(st, M, lo, hi))
+        return fail(h, FLB_ERR_INVALID, "flb_map_upload: non-finite coordinate at point %d", first_bad_point(st, M, INFINITY));
     for (int k = 0; k < 3; ++k) { h->map_lo[k] = lo[k]; h->map_hi[k] = hi[k]; }
     FLB_CUDA(h, h->map_raw.reserve((size_t)M * 3));
     FLB_CUDA(h, cudaMemcpyAsync(h->map_raw.p, st, (size_t)M * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
@@ -1729,40 +1787,9 @@ int flb_map_add_points(flb_handle* h, const float* world_xyz, int n, int stride,
     void* stv = nullptr;
     FLB_CUDA(h, h->st_map.acquire((size_t)n * 3 * sizeof(float), &stv));
     float* st = static_cast<float*>(stv);
-    float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-    if (stride == 3) std::memcpy(st, world_xyz, (size_t)n * 3 * sizeof(float));
-    else
-        for (int i = 0; i < n; ++i) {
-            st[3 * (size_t)i] = world_xyz[(size_t)i * stride];
-            st[3 * (size_t)i + 1] = world_xyz[(size_t)i * stride + 1];
-            st[3 * (size_t)i + 2] = world_xyz[(size_t)i * stride + 2];
-        }
-    {
-        // bounds + finiteness over the packed floats, 24 (= 8 points) at a time into independent accumulators (vectorises)
-        float mn[24], mx[24];
-        for (int j = 0; j < 24; ++j) { mn[j] = INFINITY; mx[j] = -INFINITY; }
-        unsigned bad = 0;
-        const size_t n3 = (size_t)n * 3;
-        size_t i = 0;
-        for (; i + 24 <= n3; i += 24)
-            for (int j = 0; j < 24; ++j) {
-                const float v = st[i + j];
-                unsigned bits;
-                std::memcpy(&bits, &v, sizeof(bits));
-                bad |= ((bits & 0x7F800000u) == 0x7F800000u) ? 1u : 0u;
-                mn[j] = v < mn[j] ? v : mn[j];
-                mx[j] = v > mx[j] ? v : mx[j];
-            }
-        for (; i < n3; ++i) {
-            const float v = st[i];
-            const int j = (int)(i % 24);
-            bad |= std::isfinite(v) ? 0u : 1u;
-            mn[j] = v < mn[j] ? v : mn[j];
-            mx[j] = v > mx[j] ? v : mx[j];
-        }
-        if (bad) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: non-finite coordinate");
-        for (int j = 0; j < 24; ++j) { lo[j % 3] = std::min(lo[j % 3], mn[j]); hi[j % 3] = std::max(hi[j % 3], mx[j]); }
-    }
+    pack_points(st, world_xyz, n, stride);
+    float lo[3], hi[3];
+    if (fold_points<true>(st, n, lo, hi)) return fail(h, FLB_ERR_INVALID, "flb_map_add_points: non-finite coordinate");
     { int rcb = map_add_check_bounds(h, "flb_map_add_points", lo, hi, downsample_size); if (rcb) return rcb; }
     // the input is valid from here on: only now does it go to the device and the map box take it in
     FLB_CUDA(h, h->add_xyz.reserve((size_t)n * 3));
@@ -1867,9 +1894,8 @@ int flb_world_cloud(flb_handle* h, const flb_lio_params* prm, const double R[9],
         bool bad = false;
         { int rcw = scan_to_world(h, prm, R, p, src, n, source == FLB_CLOUD_SCAN, h->wc_xyz, h->wc_rec, &bad, lo, hi); if (rcw) return rcw; }
         if (bad) return fail(h, FLB_ERR_INVALID, "flb_world_cloud: non-finite coordinate");
-        // the visual map's coordinate limit (vm_upload_points: |v| <= 5e5, 2^20 voxels of its 0.5 m key)
         for (int k = 0; k < 3; ++k)
-            if (lo[k] < -5.0e5f || hi[k] > 5.0e5f) return fail(h, FLB_ERR_INVALID, "flb_world_cloud: coordinate beyond 2^20 visual-map voxels");
+            if (lo[k] < -kVmapCoordLimit || hi[k] > kVmapCoordLimit) return fail(h, FLB_ERR_INVALID, "flb_world_cloud: coordinate beyond 2^20 visual-map voxels");
     }
     std::memcpy(h->wc_lo, lo, sizeof(lo));
     std::memcpy(h->wc_hi, hi, sizeof(hi));
@@ -2639,11 +2665,7 @@ int flb_visual_candidates(flb_handle* h, const double Rcw[9], const double Pcw[3
     float* st_val = reinterpret_cast<float*>(st_pose + 12);
     std::memcpy(st_val, map_value, (size_t)ncell * sizeof(float));
     float* st_pts = st_val + ncell;
-    for (int i = 0; i < n; ++i) {
-        st_pts[3 * (size_t)i] = world_xyz[(size_t)i * stride];
-        st_pts[3 * (size_t)i + 1] = world_xyz[(size_t)i * stride + 1];
-        st_pts[3 * (size_t)i + 2] = world_xyz[(size_t)i * stride + 2];
-    }
+    pack_points(st_pts, world_xyz, n, stride);
     FLB_CUDA(h, cudaMemcpyAsync(h->vm_pose.p, st_pose, 12 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     FLB_CUDA(h, cudaMemcpyAsync(h->vm_val.p, st_val, (size_t)ncell * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     if (n > 0) FLB_CUDA(h, cudaMemcpyAsync(h->vm_pts.p, st_pts, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
@@ -2716,12 +2738,10 @@ int flb_voxel_grid(flb_handle* h, const float* xyz, int n, int stride, float lea
     void* stv = nullptr;
     FLB_CUDA(h, h->st_scan.acquire((size_t)n * 3 * sizeof(float), &stv));
     float* st = static_cast<float*>(stv);
-    for (int i = 0; i < n; ++i)
-        for (int k = 0; k < 3; ++k) {
-            const float v = xyz[(size_t)i * stride + k];
-            if (!std::isfinite(v)) return fail(h, FLB_ERR_INVALID, "flb_voxel_grid: non-finite coordinate at point %d", i);
-            st[3 * (size_t)i + k] = v;
-        }
+    pack_points(st, xyz, n, stride);
+    float lo[3];
+    if (fold_points<false>(st, n, lo, nullptr))
+        return fail(h, FLB_ERR_INVALID, "flb_voxel_grid: non-finite coordinate at point %d", first_bad_point(st, n, INFINITY));
     FLB_CUDA(h, h->scan_raw.reserve((size_t)n * 3));
     FLB_CUDA(h, h->skeys.reserve(n));
     FLB_CUDA(h, h->skeys_sorted.reserve(n));
@@ -2846,41 +2866,11 @@ int flb_scan_upload(flb_handle* h, const float* body_xyz, int N, int stride) {
     void* stv = nullptr;
     FLB_CUDA(h, h->st_scan.acquire(n1 * 3 * sizeof(float), &stv));
     float* st = static_cast<float*>(stv);
-    float lo[3] = {INFINITY, INFINITY, INFINITY};
     const bool direct = N > 0 && stride == 3 && is_pinned(body_xyz);      // page-locked packed source: no staging copy
     if (direct) st = const_cast<float*>(body_xyz);
-    else if (stride == 3) std::memcpy(st, body_xyz, (size_t)N * 3 * sizeof(float));
-    else
-        for (int i = 0; i < N; ++i) {
-            st[3 * (size_t)i] = body_xyz[(size_t)i * stride];
-            st[3 * (size_t)i + 1] = body_xyz[(size_t)i * stride + 1];
-            st[3 * (size_t)i + 2] = body_xyz[(size_t)i * stride + 2];
-        }
-    {
-        // bounds + finiteness over the packed floats, 24 (= 8 points) at a time into 24 independent accumulators:
-        // no cross-iteration dependency, so the host compiler vectorises the inner loop as it stands
-        float mn[24];
-        for (int j = 0; j < 24; ++j) mn[j] = INFINITY;
-        unsigned bad = 0;
-        const size_t n3 = (size_t)N * 3;
-        size_t i = 0;
-        for (; i + 24 <= n3; i += 24)
-            for (int j = 0; j < 24; ++j) {
-                const float v = st[i + j];
-                unsigned bits;
-                std::memcpy(&bits, &v, sizeof(bits));
-                bad |= ((bits & 0x7F800000u) == 0x7F800000u) ? 1u : 0u;
-                mn[j] = v < mn[j] ? v : mn[j];
-            }
-        for (; i < n3; ++i) {
-            const float v = st[i];
-            const int j = (int)(i % 24);
-            bad |= std::isfinite(v) ? 0u : 1u;
-            mn[j] = v < mn[j] ? v : mn[j];
-        }
-        for (int j = 0; j < 24; ++j) lo[j % 3] = std::min(lo[j % 3], mn[j]);
-        if (bad) return fail(h, FLB_ERR_INVALID, "flb_scan_upload: non-finite coordinate");
-    }
+    else pack_points(st, body_xyz, N, stride);
+    float lo[3];
+    if (fold_points<false>(st, N, lo, nullptr)) return fail(h, FLB_ERR_INVALID, "flb_scan_upload: non-finite coordinate");
     // The copy runs on `scan_stream`, ahead of the ordering that reads it (the previous upload's ordering, which read
     // scan_raw too, is earlier on the same stream).  scan_raw / skeys / svals double as flb_voxel_grid's scratch on
     // `stream`; that call ends with a stream synchronise.
@@ -3992,12 +3982,12 @@ int vm_upload_points(flb_handle* h, const float* xyz, int n, int stride) {
     void* stv = nullptr;
     FLB_CUDA(h, h->vm.st_pg.acquire(n1 * 3 * sizeof(float), &stv));
     float* st = static_cast<float*>(stv);
-    for (int i = 0; i < n; ++i)
-        for (int k = 0; k < 3; ++k) {
-            const float v = xyz[(size_t)i * stride + k];
-            if (!std::isfinite(v) || std::fabs(v) > 5.0e5f) return fail(h, FLB_ERR_INVALID, "visual map: coordinate %d non-finite or beyond 2^20 voxels", i);
-            st[3 * (size_t)i + k] = v;
-        }
+    pack_points(st, xyz, n, stride);
+    float lo[3], hi[3];
+    bool bad = fold_points<true>(st, n, lo, hi);
+    for (int k = 0; k < 3; ++k) bad = bad || lo[k] < -kVmapCoordLimit || hi[k] > kVmapCoordLimit;
+    if (bad)
+        return fail(h, FLB_ERR_INVALID, "visual map: coordinate %d non-finite or beyond 2^20 voxels", first_bad_point(st, n, kVmapCoordLimit));
     FLB_CUDA(h, cudaMemcpyAsync(h->vm.pg.p, st, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     FLB_CUDA(h, h->vm.st_pg.mark(h->stream));
     return FLB_OK;
