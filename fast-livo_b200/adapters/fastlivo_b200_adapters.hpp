@@ -21,6 +21,9 @@
 //        map_incremental()  src/laserMapping.cpp:692-706  (the uploaded scan into the map, no host transform)
 //   flb::publish_effect_world(h, lio_prm, cloud)  /  flb::publish_effect_world(h, lio_prm, R, p, cloud)   fill the cloud of
 //        publish_effect_world()  src/laserMapping.cpp:871-885  (the last LIO pass's laserCloudOri, transformed on the device)
+//   flb::publish_frame_world_rgb(h, cloud)  /  (h, Rcw, Pcw, cloud)   fill laserCloudWorldRGB of publish_frame_world_rgb()
+//        src/laserMapping.cpp:710-777 (the world cloud coloured on the device, one copy);  flb::save_rgb_map(h, cloud)
+//        fills pcl_wait_save from the device's save for the PCD written at exit (:1839-1846)
 //   flb::lasermap_fov_segment(h, cube_len, &kdtree_delete_counter)  /  (h, cube_len, pos_lid, &kdtree_delete_counter)
 //        replace lasermap_fov_segment()  src/laserMapping.cpp:363-421  (local-map cube + box delete on the device)
 //   flb::upload_camera_frame(h, bgr, gray_rule)   replaces the resize / img_rgb / cvtColor lines of
@@ -46,6 +49,7 @@
 //   StatesGroup : .rot_end .pos_end .vel_end .bias_g .bias_a .gravity .cov  (include/common_lib.h:296-381)
 #pragma once
 
+#include <cstddef>
 #include <cstdint>
 #include <cstring>
 #include <stdexcept>
@@ -193,6 +197,69 @@ inline int publish_effect_world(flb_handle* h, const flb_lio_params& lio_prm, co
     int n = 0;
     check(h, flb_effect_cloud(h, &lio_prm, Rm, pv, &n));
     return effect_cloud_fill(h, n, laserCloudWorld);
+}
+
+// ---- publish_frame_world_rgb (src/laserMapping.cpp:710-777) and the pcd_save_en map from the device ---------------
+// flb_rgb_cloud's records are pcl::PointXYZRGB's layout: x y z data[3] | b g r a | 12 zero bytes.  P (PointTypeRGB) must
+// be that type, and its default constructor must leave data[3] = 1 and a = 255 (PCL 1.8 and later), because the records
+// carry those bytes: a PCL with other defaults is refused at the first use instead of saving other bytes.
+template <class P>
+inline void rgb_point_check() {
+    static_assert(sizeof(P) == 32, "PointTypeRGB must be pcl::PointXYZRGB's 32 bytes");
+    static_assert(offsetof(P, b) == 16 && offsetof(P, g) == 17 && offsetof(P, r) == 18 && offsetof(P, a) == 19,
+                  "PointTypeRGB's colour must sit at bytes 16..19 (b, g, r, a)");
+    static const bool defaults_ok = [] {
+        const P p{};
+        return p.data[3] == 1.0f && p.a == 255;
+    }();
+    if (!defaults_ok)
+        throw Error(FLB_ERR_INVALID, "flb: PointTypeRGB() does not construct data[3] = 1 and a = 255 (flb_rgb_cloud's records do)");
+}
+template <class PointCloud>
+inline int rgb_cloud_fill(flb_handle* h, int n, PointCloud& cloud) {
+    cloud.resize((size_t)n);
+    int m = 0;
+    if (n > 0) check(h, flb_rgb_cloud_download(h, &cloud.points[0], n, &m));
+    return n;
+}
+// Fills laserCloudWorldRGB (:726-747, one copy, no host loop) from the world cloud (flb_world_cloud) coloured with the
+// current image set's colour frame (flb::upload_camera_frame / upload_camera_msg), at the device state's camera pose
+// (after flb_vmap_reset).  With pcd_save_en, flb_rgb_save_begin at start-up makes it append to the device's save too.
+template <class PointCloud>
+inline int publish_frame_world_rgb(flb_handle* h, PointCloud& laserCloudWorldRGB) {
+    rgb_point_check<typename std::decay<decltype(laserCloudWorldRGB.points[0])>::type>();
+    int n = 0;
+    check(h, flb_rgb_cloud(h, nullptr, nullptr, nullptr, 0, &n));
+    return rgb_cloud_fill(h, n, laserCloudWorldRGB);
+}
+// The same at an explicit camera pose: Rcw = new_frame_->T_f_w_.rotation_matrix(), Pcw = its translation().
+template <class Mat3, class Vec3, class PointCloud>
+inline int publish_frame_world_rgb(flb_handle* h, const Mat3& Rcw, const Vec3& Pcw, PointCloud& laserCloudWorldRGB) {
+    rgb_point_check<typename std::decay<decltype(laserCloudWorldRGB.points[0])>::type>();
+    double Rm[9], pv[3];
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) Rm[3 * i + j] = Rcw(i, j);
+        pv[i] = Pcw(i);
+    }
+    int n = 0;
+    check(h, flb_rgb_cloud(h, Rm, pv, nullptr, 0, &n));
+    return rgb_cloud_fill(h, n, laserCloudWorldRGB);
+}
+// pcl_wait_save at exit (:1839-1846): the whole device save, filled slice by slice, for pcd_writer.writeBinary.  Throws
+// flb::Error when frames were dropped at flb_rgb_save_begin's cap: a map with holes is not written silently.
+template <class PointCloud>
+inline int64_t save_rgb_map(flb_handle* h, PointCloud& pcl_wait_save) {
+    rgb_point_check<typename std::decay<decltype(pcl_wait_save.points[0])>::type>();
+    int64_t n = 0, dropped = 0;
+    check(h, flb_rgb_save_size(h, &n, &dropped, nullptr));
+    if (dropped > 0)
+        throw Error(FLB_ERR_STATE, "flb::save_rgb_map: " + std::to_string((long long)dropped) +
+                                       " points were dropped at flb_rgb_save_begin's max_points");
+    pcl_wait_save.resize((size_t)n);
+    const int64_t kSlice = (int64_t)1 << 22;
+    for (int64_t first = 0; first < n; first += kSlice)
+        check(h, flb_rgb_save_download(h, first, n - first < kSlice ? n - first : kSlice, &pcl_wait_save.points[(size_t)first]));
+    return n;
 }
 
 // ---- lasermap_fov_segment (src/laserMapping.cpp:363-421) with the cube on the device ---------------

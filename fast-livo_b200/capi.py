@@ -181,6 +181,9 @@ class FovParams(C.Structure):
 
 
 CLOUD_SCAN, CLOUD_UNDISTORTED = 0, 1       # flb_world_cloud sources (FLB_CLOUD_*)
+# flb_rgb_cloud's 32-byte record, the layout of pcl::PointXYZRGB: x y z, w = data[3] (1.0), b g r a, 12 zero bytes
+RGB_POINT = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("w", "<f4"), ("b", "u1"), ("g", "u1"), ("r", "u1"), ("a", "u1"),
+                      ("pad", "u1", 12)])
 LIDAR_LIVOX, LIDAR_VELODYNE, LIDAR_OUSTER, LIDAR_XT32 = 1, 2, 3, 4    # flb_lidar_format.kind (FLB_LIDAR_*)
 GRAY_CV4, GRAY_CV3 = 0, 1                  # flb_image_upload_bgr's cvtColor rules (FLB_GRAY_*)
 # flb_image_upload_msg's encodings (FLB_ENC_*), keyed by sensor_msgs::Image's encoding string
@@ -200,6 +203,7 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_vmap_reset", "flb_vmap_select", "flb_vmap_selected", "flb_vmap_grow", "flb_vmap_add_observations", "flb_vmap_counts",
            "flb_vmap_map_value", "flb_vmap_dump", "flb_vmap_reclaim", "flb_vmap_usage", "flb_vmap_keyframe", "flb_colorize", "flb_voxel_grid",
            "flb_world_cloud", "flb_world_cloud_download", "flb_effect_cloud", "flb_effect_cloud_download", "flb_vmap_select_cloud", "flb_vmap_grow_cloud", "flb_colorize_cloud",
+           "flb_rgb_cloud", "flb_rgb_cloud_download", "flb_rgb_save_begin", "flb_rgb_save_size", "flb_rgb_save_download", "flb_rgb_save_end",
            "flb_batch_begin", "flb_batch_set_frame", "flb_batch_state_reset_enqueue", "flb_batch_update_enqueue", "flb_batch_state_download",
            "flb_debug_set_packet_epoch", "flb_debug_block_stamps", "flb_debug_vio_stamps", "flb_debug_scan_order", "flb_debug_set_scan_sort",
            "flb_map_grid_info", "flb_debug_set_map_index", "flb_map_fov_segment", "flb_map_fov_reset",
@@ -302,6 +306,12 @@ def lib():
         L.flb_vmap_select_cloud.argtypes = [vp, vp, vp, C.c_float, vp]
         L.flb_vmap_grow_cloud.argtypes = [vp, vp, vp, C.c_int]
         L.flb_colorize_cloud.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp]
+        L.flb_rgb_cloud.argtypes = [vp, vp, vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_rgb_cloud_download.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_rgb_save_begin.argtypes = [vp, C.c_int64]
+        L.flb_rgb_save_size.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.flb_rgb_save_download.argtypes = [vp, C.c_int64, C.c_int64, vp]
+        L.flb_rgb_save_end.argtypes = [vp]
         L.flb_vmap_reset.argtypes = [vp, C.POINTER(VmapParams)]
         L.flb_vmap_select.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, vp]
         L.flb_vmap_selected.argtypes = [vp, C.c_int, C.POINTER(C.c_int)] + [vp] * 6
@@ -383,6 +393,7 @@ class Handle:
         self.N = self.M = self.Pn = 0
         self._wc_n = 0                  # points of the world cloud flb_world_cloud last built
         self._ef_n = 0                  # points of the effect cloud flb_effect_cloud last built
+        self._rc_n = 0                  # records of the coloured cloud flb_rgb_cloud last built
 
     def close(self):
         if getattr(self, "h", None):
@@ -791,6 +802,45 @@ class Handle:
         val = np.zeros(self._wc_n, np.uint8)
         self._ck(self.L.flb_colorize_cloud(self.h, pr, pp, _p(img), 0 if img is None else img.shape[1] * 3, _p(rgb), _p(val)))
         return rgb, val.astype(bool)
+
+    # ---- publish_frame_world_rgb's laserCloudWorldRGB and the run's pcl_wait_save on the device
+    def rgb_cloud(self, Rcw=None, Pcw=None, bgr=None):
+        """flb_rgb_cloud: the coloured points of the world cloud as records; returns their number.  bgr None: the
+        current image set's colour frame; Rcw / Pcw None: the pose from the device state."""
+        R, P, pr, pp = self._pose(Rcw, Pcw)
+        img = None if bgr is None else np.ascontiguousarray(bgr, np.uint8)
+        n = C.c_int()
+        self._rc_n = 0
+        self._ck(self.L.flb_rgb_cloud(self.h, pr, pp, _p(img), 0 if img is None else img.shape[1] * 3, C.byref(n)))
+        self._rc_n = n.value
+        return n.value
+
+    def rgb_cloud_download(self):
+        """flb_rgb_cloud_download: the coloured cloud, (n,) RGB_POINT records."""
+        out = np.zeros(self._rc_n, RGB_POINT)
+        n = C.c_int()
+        self._ck(self.L.flb_rgb_cloud_download(self.h, _p(out), len(out), C.byref(n)))
+        return out[:n.value]
+
+    def rgb_save_begin(self, max_points):
+        self._ck(self.L.flb_rgb_save_begin(self.h, int(max_points)))
+
+    def rgb_save_size(self):
+        """flb_rgb_save_size: dict(n, dropped, device_bytes)."""
+        n, d, b = C.c_int64(), C.c_int64(), C.c_int64()
+        self._ck(self.L.flb_rgb_save_size(self.h, C.byref(n), C.byref(d), C.byref(b)))
+        return dict(n=n.value, dropped=d.value, device_bytes=b.value)
+
+    def rgb_save_download(self, first=0, count=None):
+        """flb_rgb_save_download: records first .. first + count - 1 of the save (count None: to its end), RGB_POINT."""
+        if count is None:
+            count = self.rgb_save_size()["n"] - first
+        out = np.zeros(max(int(count), 0), RGB_POINT)
+        self._ck(self.L.flb_rgb_save_download(self.h, int(first), int(count), _p(out)))
+        return out
+
+    def rgb_save_end(self):
+        self._ck(self.L.flb_rgb_save_end(self.h))
 
     def keypatch_image(self, Rcw=None, Pcw=None, out=None):
         """flb_keypatch_image: (frame (H, W, 3) uint8, patch count) -- the current colour frame with display_keypatch's

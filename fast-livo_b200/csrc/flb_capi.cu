@@ -355,6 +355,22 @@ struct flb_handle {
     DevBuf<int> ef_count;
     DevBuf<float> ef_xyz;
     DevBuf<unsigned> ef_rec;
+    // flb_rgb_cloud: laserCloudWorldRGB as 32-byte records (rc_out, rc_n of them; rc_n < 0: none held), the per-point
+    // colour words, keep flags and their exclusive sum (n + 1 each), and the caller's colour frame when it passes one.
+    // Buffers of its own: the LIO export's row mask (x_rowmask) stays valid.
+    DevBuf<uint4> rc_out;
+    DevBuf<unsigned> rc_bgra;
+    DevBuf<int> rc_flag, rc_pos;
+    DevBuf<unsigned char> rc_img;
+    int rc_n = -1;
+    // flb_rgb_save_*: pcl_wait_save as 16-byte records in chunks of 2^kRgbChunkLog2 (rs_chunks), rs_table their pointers
+    // on the device (rs_table_n entries uploaded), rs_pack the download's staging.
+    bool rs_on = false;
+    long long rs_max = 0, rs_n = 0, rs_dropped = 0;
+    std::vector<uint4*> rs_chunks;
+    size_t rs_table_n = 0;
+    DevBuf<uint4*> rs_table;
+    DevBuf<uint4> rs_pack;
     // flb_vmap_select_cloud: downSizeFilter of the world cloud and its scratch (the scan slot's stays untouched)
     DevBuf<float> wc_down;
     DevBuf<unsigned> wc_keys, wc_keys_sorted;
@@ -914,6 +930,17 @@ void note_lio_pass(flb_handle* h) {
     h->ef_N = h->N;
 }
 
+// flb_rgb_save_end / flb_destroy: the save's chunks, table and staging (cudaFree waits for the kernels that use them).
+void rgb_save_free(flb_handle* h) {
+    for (uint4* c : h->rs_chunks) cudaFree(c);
+    h->rs_chunks.clear();
+    h->rs_table_n = 0;
+    h->rs_table.release();
+    h->rs_pack.release();
+    h->rs_on = false;
+    h->rs_max = h->rs_n = h->rs_dropped = 0;
+}
+
 // Flag base for one persistent launch: flags epoch+1 .. epoch+4095 belong to it alone.  On wrap-around the
 // packet and the arrival lines are cleared (stream-ordered) so that no stale unit can ever match.
 int next_epoch(flb_handle* h, unsigned* epoch) {
@@ -1301,6 +1328,8 @@ int flb_destroy(flb_handle* h) {
     h->wc_xyz.release(); h->wc_rec.release(); h->wc_down.release(); h->wc_keys.release(); h->wc_keys_sorted.release();
     h->wc_vals.release(); h->wc_vals_sorted.release(); h->wc_heads.release(); h->wc_box.release();
     h->ef_scatter.release(); h->ef_body.release(); h->ef_flag.release(); h->ef_count.release(); h->ef_xyz.release(); h->ef_rec.release();
+    h->rc_out.release(); h->rc_bgra.release(); h->rc_flag.release(); h->rc_pos.release(); h->rc_img.release();
+    rgb_save_free(h);
     h->sf_keys.release(); h->sf_keys_sorted.release(); h->sf_rec.release(); h->sf_vals.release(); h->sf_vals_sorted.release();
     h->sf_heads.release(); h->sf_xyz.release();
     h->cell_table.release(); h->cell_keys.release(); h->cell_keys_alt.release();
@@ -4344,29 +4373,37 @@ int colorize_pose(flb_handle* h, const char* who, const double* Rcw, const doubl
     return vm_set_pose(h, Rcw, Pcw);
 }
 
-// The per-point kernel and the download of rgb / valid for n >= 1 device points xyz.  The colour image: the caller's
-// bgr, uploaded ahead of rgb / valid; bgr == NULL: the current image set's colour frame (flb_image_upload_bgr), read in
-// place once its upload has landed.
+// The colour frame the colouring reads, into *d_img: the caller's bgr, packed and uploaded on `stream` into dst
+// (W x H x 3 bytes); bgr == NULL: the current image set's colour frame (flb_image_upload_bgr), read in place once its
+// upload has landed.
+int colorize_image(flb_handle* h, const uint8_t* bgr, int stride_bytes, unsigned char* dst, const unsigned char** d_img) {
+    if (!bgr) {
+        *d_img = h->img_bgr.p;
+        return vio_inputs_acquire(h);
+    }
+    const int W = h->cam.width, H = h->cam.height;
+    const size_t img_bytes = (size_t)W * H * 3;
+    void* stv = nullptr;
+    FLB_CUDA(h, h->st_img.acquire(img_bytes, &stv));
+    unsigned char* st = static_cast<unsigned char*>(stv);
+    for (int r = 0; r < H; ++r) std::memcpy(st + (size_t)r * W * 3, bgr + (size_t)r * stride_bytes, (size_t)W * 3);
+    FLB_CUDA(h, cudaMemcpyAsync(dst, st, img_bytes, cudaMemcpyHostToDevice, h->stream));
+    FLB_CUDA(h, h->st_img.mark(h->stream));
+    *d_img = dst;
+    return FLB_OK;
+}
+
+// The per-point kernel and the download of rgb / valid for n >= 1 device points xyz, the colour image (colorize_image)
+// uploaded ahead of rgb / valid.
 int colorize_dev(flb_handle* h, const uint8_t* bgr, int stride_bytes, const float* xyz, int n, uint8_t* rgb, uint8_t* valid) {
     auto& vm = h->vm;
     const int W = h->cam.width, H = h->cam.height;
     const size_t img_bytes = bgr ? (size_t)W * H * 3 : 0;
     FLB_CUDA(h, h->x_rowmask.reserve(img_bytes + (size_t)n * 4));     // [colour image |] rgb | valid
-    const unsigned char* d_img = h->img_bgr.p;
+    const unsigned char* d_img = nullptr;
     unsigned char* d_rgb = h->x_rowmask.p + img_bytes;
     unsigned char* d_val = d_rgb + (size_t)n * 3;
-    if (bgr) {
-        d_img = h->x_rowmask.p;
-        void* stv = nullptr;
-        FLB_CUDA(h, h->st_img.acquire(img_bytes, &stv));
-        unsigned char* st = static_cast<unsigned char*>(stv);
-        for (int r = 0; r < H; ++r) std::memcpy(st + (size_t)r * W * 3, bgr + (size_t)r * stride_bytes, (size_t)W * 3);
-        FLB_CUDA(h, cudaMemcpyAsync(h->x_rowmask.p, st, img_bytes, cudaMemcpyHostToDevice, h->stream));
-        FLB_CUDA(h, h->st_img.mark(h->stream));
-    } else {
-        int rcq = vio_inputs_acquire(h);
-        if (rcq) return rcq;
-    }
+    { int rci = colorize_image(h, bgr, stride_bytes, h->x_rowmask.p, &d_img); if (rci) return rci; }
     {
         LaunchScope ls(h, FAM_OTHER);
         k_vm_colorize<<<(n + 255) / 256, 256, 0, h->stream>>>(h->cam, vm.pose.p, d_img, xyz, n, d_rgb, d_val);
@@ -4385,6 +4422,29 @@ int colorize_dev(flb_handle* h, const uint8_t* bgr, int stride_bytes, const floa
 int colorize_frame_check(flb_handle* h, const char* who, const uint8_t* bgr) {
     if (!bgr && !(h->img_bgr_valid && h->img_w == h->cam.width && h->img_h == h->cam.height))
         return fail(h, FLB_ERR_STATE, "%s: bgr == NULL needs the current image from flb_image_upload_bgr at the camera's size", who);
+    return FLB_OK;
+}
+
+// Chunks for `need` save records, their pointers uploaded to rs_table on `stream` (a table that grows is reallocated:
+// cudaFree waits for the scatters reading the old one).  *ok = false when the device has no memory for one more chunk:
+// the frame is then dropped like one beyond the cap; the chunks that were allocated stay for later frames.
+int rgb_save_reserve(flb_handle* h, long long need, bool* ok) {
+    const size_t want = (size_t)((need + (1LL << kRgbChunkLog2) - 1) >> kRgbChunkLog2);
+    while (h->rs_chunks.size() < want) {
+        uint4* c = nullptr;
+        if (cudaMalloc(&c, ((size_t)1 << kRgbChunkLog2) * sizeof(uint4)) != cudaSuccess) {
+            cudaGetLastError();                       // an allocation failure is not sticky: clear it
+            break;
+        }
+        h->rs_chunks.push_back(c);
+    }
+    if (h->rs_chunks.size() > h->rs_table_n) {
+        FLB_CUDA(h, h->rs_table.reserve(h->rs_chunks.size()));
+        FLB_CUDA(h, cudaMemcpyAsync(h->rs_table.p, h->rs_chunks.data(), h->rs_chunks.size() * sizeof(uint4*), cudaMemcpyHostToDevice,
+                                    h->stream));
+        h->rs_table_n = h->rs_chunks.size();
+    }
+    *ok = h->rs_chunks.size() >= want;
     return FLB_OK;
 }
 
@@ -4418,6 +4478,131 @@ int flb_colorize_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], 
     if (n == 0) return FLB_OK;
     { int rc = colorize_pose(h, "flb_colorize_cloud", Rcw, Pcw); if (rc) return rc; }
     return colorize_dev(h, bgr, stride_bytes, h->wc_xyz.p, n, rgb, valid);
+}
+
+// publish_frame_world_rgb's laserCloudWorldRGB (src/laserMapping.cpp:726-747) as 32-byte records on the device:
+// k_rgb_flags colours every world point, cub's exclusive sum ranks the kept ones, the count is read back, and
+// k_rgb_scatter writes each kept point's record (and, with the save on and room under its cap, its save record).
+int flb_rgb_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, int* n_out) {
+    FLB_CHECK_H(h);
+    h->rc_n = -1;                                     // on any error below, no cloud is held
+    if (n_out) *n_out = 0;
+    if (!h->cam_set) return fail(h, FLB_ERR_STATE, "flb_rgb_cloud: flb_camera_set first");
+    { int rc = wc_check(h, "flb_rgb_cloud"); if (rc) return rc; }
+    const int n = h->wc_n;
+    if (bgr && stride_bytes < 3 * h->cam.width) return fail(h, FLB_ERR_INVALID, "flb_rgb_cloud: bad arguments");
+    { int rc = colorize_frame_check(h, "flb_rgb_cloud", bgr); if (rc) return rc; }
+    if (n == 0) {
+        h->rc_n = 0;
+        return FLB_OK;
+    }
+    { int rc = colorize_pose(h, "flb_rgb_cloud", Rcw, Pcw); if (rc) return rc; }
+    if (bgr) FLB_CUDA(h, h->rc_img.reserve((size_t)h->cam.width * h->cam.height * 3));
+    FLB_CUDA(h, h->rc_bgra.reserve(n));
+    FLB_CUDA(h, h->rc_flag.reserve((size_t)n + 1));
+    FLB_CUDA(h, h->rc_pos.reserve((size_t)n + 1));
+    const unsigned char* d_img = nullptr;
+    { int rci = colorize_image(h, bgr, stride_bytes, h->rc_img.p, &d_img); if (rci) return rci; }
+    {
+        LaunchScope ls(h, FAM_OTHER);
+        k_rgb_flags<<<(n + 1 + 255) / 256, 256, 0, h->stream>>>(h->cam, h->vm.pose.p, d_img, h->wc_xyz.p, n, h->rc_bgra.p, h->rc_flag.p);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    size_t tmp_bytes = 0;
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, h->rc_flag.p, h->rc_pos.p, n + 1, h->stream));
+    FLB_CUDA(h, h->cub_tmp.reserve(tmp_bytes));
+    FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->cub_tmp.p, tmp_bytes, h->rc_flag.p, h->rc_pos.p, n + 1, h->stream));
+    h->launches++;
+    FLB_CUDA(h, h->pin_out.reserve(sizeof(int)));
+    int* cnt = static_cast<int*>(h->pin_out.p);
+    FLB_CUDA(h, cudaMemcpyAsync(cnt, h->rc_pos.p + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    const int m = *cnt;
+    uint4* const* table = nullptr;
+    if (h->rs_on && m > 0) {
+        bool ok = m <= h->rs_max - h->rs_n;
+        if (ok) { int rcs = rgb_save_reserve(h, h->rs_n + m, &ok); if (rcs) return rcs; }
+        if (ok) table = h->rs_table.p;
+        else h->rs_dropped += m;                      // the frame's cloud is still built: saving never stops publishing
+    }
+    if (m > 0) {
+        FLB_CUDA(h, h->rc_out.reserve(2 * (size_t)m));
+        LaunchScope ls(h, FAM_OTHER);
+        k_rgb_scatter<<<(n + 255) / 256, 256, 0, h->stream>>>(h->wc_xyz.p, h->rc_bgra.p, h->rc_flag.p, h->rc_pos.p, n, h->rc_out.p, table,
+                                                              h->rs_n);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    if (table) h->rs_n += m;
+    h->rc_n = m;
+    if (n_out) *n_out = m;
+    return FLB_OK;
+}
+
+int flb_rgb_cloud_download(flb_handle* h, void* points32, int capacity, int* n_out) {
+    FLB_CHECK_H(h);
+    if (capacity < 0 || (capacity > 0 && !points32)) return fail(h, FLB_ERR_INVALID, "flb_rgb_cloud_download: bad arguments");
+    if (h->rc_n < 0) return fail(h, FLB_ERR_STATE, "flb_rgb_cloud_download: no coloured cloud (flb_rgb_cloud first, or it failed)");
+    if (n_out) *n_out = h->rc_n;
+    const int m = std::min(capacity, h->rc_n);
+    if (m > 0) {
+        FLB_CUDA(h, cudaMemcpyAsync(points32, h->rc_out.p, (size_t)m * 2 * sizeof(uint4), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    }
+    return FLB_OK;
+}
+
+int flb_rgb_save_begin(flb_handle* h, int64_t max_points) {
+    FLB_CHECK_H(h);
+    if (max_points < 1) return fail(h, FLB_ERR_INVALID, "flb_rgb_save_begin: max_points %lld < 1", (long long)max_points);
+    if (h->rs_on) return fail(h, FLB_ERR_STATE, "flb_rgb_save_begin: a save is open (flb_rgb_save_end first)");
+    h->rs_on = true;
+    h->rs_max = max_points;
+    h->rs_n = h->rs_dropped = 0;
+    return FLB_OK;
+}
+
+int flb_rgb_save_size(flb_handle* h, int64_t* n, int64_t* dropped, int64_t* device_bytes) {
+    FLB_CHECK_H(h);
+    if (!h->rs_on) return fail(h, FLB_ERR_STATE, "flb_rgb_save_size: no save open (flb_rgb_save_begin first)");
+    if (n) *n = h->rs_n;
+    if (dropped) *dropped = h->rs_dropped;
+    if (device_bytes)
+        *device_bytes = (int64_t)(h->rs_chunks.size() * ((size_t)1 << kRgbChunkLog2) * sizeof(uint4) + h->rs_table.cap * sizeof(uint4*) +
+                                  h->rs_pack.cap * sizeof(uint4));
+    return FLB_OK;
+}
+
+int flb_rgb_save_download(flb_handle* h, int64_t first, int64_t count, void* points32) {
+    FLB_CHECK_H(h);
+    if (!h->rs_on) return fail(h, FLB_ERR_STATE, "flb_rgb_save_download: no save open (flb_rgb_save_begin first)");
+    if (first < 0 || count < 0 || count > h->rs_n - first || (count > 0 && !points32))
+        return fail(h, FLB_ERR_INVALID, "flb_rgb_save_download: bad arguments (records %lld + %lld of %lld)", (long long)first,
+                    (long long)count, h->rs_n);
+    if (count == 0) return FLB_OK;
+    // One bounded slice at a time: k_rgb_save_pack expands it into rs_pack, the copy takes it out; stream order keeps
+    // the next slice's pack behind the copy.
+    constexpr long long kSlice = 1LL << 18;
+    FLB_CUDA(h, h->rs_pack.reserve(2 * (size_t)std::min<long long>(count, kSlice)));
+    char* dst = static_cast<char*>(points32);
+    for (long long done = 0; done < count; done += kSlice) {
+        const int k = (int)std::min<long long>(count - done, kSlice);
+        {
+            LaunchScope ls(h, FAM_OTHER);
+            k_rgb_save_pack<<<(k + 255) / 256, 256, 0, h->stream>>>(h->rs_table.p, first + done, k, h->rs_pack.p);
+            FLB_CUDA(h, cudaGetLastError());
+        }
+        FLB_CUDA(h, cudaMemcpyAsync(dst + done * 2 * (long long)sizeof(uint4), h->rs_pack.p, (size_t)k * 2 * sizeof(uint4),
+                                    cudaMemcpyDeviceToHost, h->stream));
+    }
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    return FLB_OK;
+}
+
+int flb_rgb_save_end(flb_handle* h) {
+    FLB_CHECK_H(h);
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    rgb_save_free(h);
+    return FLB_OK;
 }
 
 // LidarSelector::display_keypatch (src/lidar_selection.cpp:985-1005) without its text, into a copy of the current colour

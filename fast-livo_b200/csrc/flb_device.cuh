@@ -1209,6 +1209,53 @@ FLB_HD bool vm_colorize_point(const CamModel& cam, const double* Rcw, const doub
     return true;
 }
 
+// ---- flb_rgb_cloud: laserCloudWorldRGB (src/laserMapping.cpp:726-747) as records, and its run-long save (pcl_wait_save,
+// :777).  Words, not floats, so that no colour word is ever moved through a float register (r >= 128 makes it a NaN).
+#if defined(__CUDACC__)
+typedef uint4 rgb_word4;
+#else
+struct rgb_word4 { unsigned x, y, z, w; };
+#endif
+// The colour word of a kept point: pcl::PointXYZRGB's b, g, r, a bytes (offsets 16..19), a = 255 as PCL 1.8+ constructs it.
+FLB_HD unsigned rgb_bgra_word(const unsigned char* rgb) {
+    return (unsigned)rgb[2] | ((unsigned)rgb[1] << 8) | ((unsigned)rgb[0] << 16) | 0xFF000000u;
+}
+// k_rgb_flags, one world point: vm_colorize_point's verdict as the 0/1 keep flag, its colour word (0 when not kept).
+FLB_HD int rgb_flag_point(const CamModel& cam, const double* Rcw, const double* Pcw, const unsigned char* bgr, const float* p,
+                          unsigned* bgra) {
+    unsigned char c[3] = {0, 0, 0};
+    const bool ok = vm_colorize_point(cam, Rcw, Pcw, bgr, p, c);
+    *bgra = ok ? rgb_bgra_word(c) : 0u;
+    return ok ? 1 : 0;
+}
+// The save lives in chunks of 2^kRgbChunkLog2 16-byte records {x, y, z, bgra}; record i is entry i & mask of chunk i >> log2.
+constexpr int kRgbChunkLog2 = 20;
+FLB_HD rgb_word4* rgb_save_slot(rgb_word4* const* chunks, long long i, int chunk_log2) {
+    return chunks[i >> chunk_log2] + (i & ((1LL << chunk_log2) - 1));
+}
+// The ABI's 32-byte record (pcl::PointXYZRGB): x, y, z, data[3] = 1.0f | bgra, three zero words; two 16-byte halves.
+FLB_HD void rgb_record32(unsigned x, unsigned y, unsigned z, unsigned bgra, rgb_word4* rec) {
+    rgb_word4 a, b;
+    a.x = x; a.y = y; a.z = z; a.w = 0x3F800000u;
+    b.x = bgra; b.y = 0u; b.z = 0u; b.w = 0u;
+    rec[0] = a;
+    rec[1] = b;
+}
+// k_rgb_scatter, one kept point p at its rank `slot`: its record in the frame's cloud and, chunks != NULL, its save record
+// at save_base + slot.
+FLB_HD void rgb_scatter_point(const float* p, unsigned bgra, int slot, rgb_word4* out, rgb_word4* const* chunks, long long save_base,
+                              int chunk_log2) {
+    const unsigned x = float_as_u32(p[0]), y = float_as_u32(p[1]), z = float_as_u32(p[2]);
+    rgb_record32(x, y, z, bgra, out + 2 * (size_t)slot);
+    if (chunks) {
+        rgb_word4 s;
+        s.x = x; s.y = y; s.z = z; s.w = bgra;
+        *rgb_save_slot(chunks, save_base + slot, chunk_log2) = s;
+    }
+}
+// k_rgb_save_pack, one save record expanded to the 32-byte record.
+FLB_HD void rgb_save_expand(const rgb_word4& s, rgb_word4* rec) { rgb_record32(s.x, s.y, s.z, s.w, rec); }
+
 // The device-resident visual map: Point (include/point.h) and Feature (include/feature.h) flattened.
 constexpr int kVmMaxObs = 20;            // addObservation keeps obs_.size() < 20 before adding one (:946-952)
 struct VmFeature {

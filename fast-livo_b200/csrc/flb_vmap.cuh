@@ -448,6 +448,43 @@ __global__ void k_vm_colorize(CamModel cam, const double* __restrict__ pose12, c
     valid[i] = ok ? 1 : 0;
 }
 
+// flb_rgb_cloud, stage 1: one thread per world point writes its keep flag and colour word (rgb_flag_point); thread n
+// writes flag[n] = 0, so that entry n of the exclusive sum over n + 1 flags is the record count.
+__global__ void __launch_bounds__(256) k_rgb_flags(CamModel cam, const double* __restrict__ pose12, const unsigned char* __restrict__ bgr,
+                                                   const float* __restrict__ xyz, int n, unsigned* __restrict__ bgra, int* __restrict__ flag) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > n) return;
+    if (i == n) {
+        flag[n] = 0;
+        return;
+    }
+    double Rcw[9], Pcw[3];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) Rcw[k] = pose12[k];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) Pcw[k] = pose12[9 + k];
+    const float p[3] = {xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2]};
+    flag[i] = rgb_flag_point(cam, Rcw, Pcw, bgr, p, &bgra[i]);
+}
+
+// flb_rgb_cloud, stage 3: one thread per world point; a kept one writes its record at its rank pos[i] (two 16-byte
+// stores) and, chunks != NULL, its save record at save_base + pos[i] (rgb_scatter_point).
+__global__ void __launch_bounds__(256) k_rgb_scatter(const float* __restrict__ xyz, const unsigned* __restrict__ bgra, const int* __restrict__ flag,
+                                                     const int* __restrict__ pos, int n, uint4* __restrict__ out, uint4* const* __restrict__ chunks,
+                                                     long long save_base) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !flag[i]) return;
+    const float p[3] = {xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2]};
+    rgb_scatter_point(p, bgra[i], pos[i], out, chunks, save_base, kRgbChunkLog2);
+}
+
+// flb_rgb_save_download: save records first .. first + count - 1 expanded to 32-byte records in out.
+__global__ void __launch_bounds__(256) k_rgb_save_pack(uint4* const* __restrict__ chunks, long long first, int count, uint4* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    rgb_save_expand(*rgb_save_slot(chunks, first + i, kRgbChunkLog2), out + 2 * (size_t)i);
+}
+
 // display_keypatch (src/lidar_selection.cpp:985-1005), step 1: one warp per patch (n patches, or *n_dev of at most n)
 // stamps its index into owner (W x H, all -1 before) over its clipped disk.  atomicMax leaves the highest index where
 // disks overlap, which is what drawing in list order leaves, without ordering the warps.

@@ -647,6 +647,36 @@ int flb_vmap_select_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3
 int flb_vmap_grow_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], int frame_id);
 int flb_colorize_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, uint8_t* rgb,
                        uint8_t* valid);
+/* publish_frame_world_rgb's laserCloudWorldRGB (src/laserMapping.cpp:726-747) built on the device as records: the world
+ * cloud's points that flb_colorize_cloud marks valid, in world-cloud order, with its r, g, b bytes (its clamp for pc in
+ * (-1, 0) and for the last row and column included).  Pose, bgr and stride rules, and the FLB_ERR_STATE cases (no
+ * camera, no world cloud, bgr == NULL without a colour frame of the camera's size, no pose and no flb_vmap_reset), are
+ * flb_colorize_cloud's; a world cloud of 0 points gives 0 records (and needs no pose).  One 32-byte record per point, the
+ * layout of pcl::PointXYZRGB:
+ *   float x, y, z at bytes 0 / 4 / 8; float 1.0f at 12 (data[3]); uint8 b, g, r, a at 16..19 with a = 255; bytes 20..31 zero.
+ * Blocking: reading the record count back (4 bytes) is its one synchronise.  *n_out (may be NULL) = records.  The LIO
+ * export (flb_lio_export) stays valid.  With a save open (flb_rgb_save_begin) the records are appended to it as well.
+ * On any error no coloured cloud is held.  FLB_ERR_INVALID: bgr with stride_bytes < 3 * width. */
+int flb_rgb_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], const uint8_t* bgr, int stride_bytes, int* n_out);
+/* Up to `capacity` records of the last flb_rgb_cloud, 32 bytes each, into points32 (blocking); *n_out = records held.
+ * FLB_ERR_INVALID for a bad capacity or buffer, FLB_ERR_STATE when no coloured cloud is held. */
+int flb_rgb_cloud_download(flb_handle* h, void* points32, int capacity, int* n_out);
+/* pcl_wait_save with pcd_save_en (`*pcl_wait_save += *laserCloudWorldRGB`, :777; written as rgb_scan_all.pcd at exit,
+ * :1839-1846) on the device.  After flb_rgb_save_begin every successful flb_rgb_cloud appends its records, so the save
+ * is the frames' clouds concatenated in call order.  It is held as 16-byte records {x, y, z, bgra} in device chunks of
+ * 2^20 records, allocated as frames need them and never copied.  max_points (>= 1) caps it: a frame whose records would
+ * pass the cap is not appended at all and its record count is added to `dropped` (so is a frame for which no chunk can be
+ * allocated); its own cloud is still built and flb_rgb_cloud returns FLB_OK.  One save per handle.
+ *   flb_rgb_save_begin: FLB_ERR_INVALID for max_points < 1, FLB_ERR_STATE when a save is open.
+ *   flb_rgb_save_size: records held, records dropped, device bytes the save holds (any pointer may be NULL).
+ *   flb_rgb_save_download: records first .. first + count - 1 as 32-byte records (flb_rgb_cloud's layout), expanded on
+ *   the device through a bounded staging buffer (blocking); FLB_ERR_INVALID for a range outside the save.
+ *   flb_rgb_save_end: frees the save (no save open: nothing to do).
+ *   Size and download return FLB_ERR_STATE when no save is open. */
+int flb_rgb_save_begin(flb_handle* h, int64_t max_points);
+int flb_rgb_save_size(flb_handle* h, int64_t* n, int64_t* dropped, int64_t* device_bytes);
+int flb_rgb_save_download(flb_handle* h, int64_t first, int64_t count, void* points32);
+int flb_rgb_save_end(flb_handle* h);
 /* LidarSelector::display_keypatch (src/lidar_selection.cpp:985-1005) without its putText: the current image set's
  * camera-size colour frame (img_cp = img_rgb, :1035-1036) with one filled circle per patch of the current patch list,
  * written to bgr_out (W x H x 3 BGR8, stride_bytes a row).  The image set's colour frame itself is not modified, so
