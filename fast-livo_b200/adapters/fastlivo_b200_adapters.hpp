@@ -21,6 +21,8 @@
 //        map_incremental()  src/laserMapping.cpp:692-706  (the uploaded scan into the map, no host transform)
 //   flb::publish_effect_world(h, lio_prm, cloud)  /  flb::publish_effect_world(h, lio_prm, R, p, cloud)   fill the cloud of
 //        publish_effect_world()  src/laserMapping.cpp:871-885  (the last LIO pass's laserCloudOri, transformed on the device)
+//   flb::publish_frame_world(h, cloud)   fill pcl_wait_pub of publish_frame_world() src/laserMapping.cpp:780-813 (img_enable:
+//        0; the world cloud with its intensities, one copy);  flb::save_intensity_map(h, cloud)   pcl_wait_save_lidar
 //   flb::publish_frame_world_rgb(h, cloud)  /  (h, Rcw, Pcw, cloud)   fill laserCloudWorldRGB of publish_frame_world_rgb()
 //        src/laserMapping.cpp:710-777 (the world cloud coloured on the device, one copy);  flb::save_rgb_map(h, cloud)
 //        fills pcl_wait_save from the device's save for the PCD written at exit (:1839-1846)
@@ -164,18 +166,27 @@ inline void map_incremental(flb_handle* h, const flb_lio_params& lio_prm, const 
 
 // ---- publish_effect_world (src/laserMapping.cpp:871-885) from the last LIO pass on the device -----------------
 // Fills `laserCloudWorld` (a PCL cloud: resize(n) and .points with x, y, z) with laserCloudOri of the last LIO pass
-// (:1588-1600) transformed by RGBpointBodyToWorld; the caller converts and publishes it as before.  Only x, y, z are
-// written: the device holds no intensity.  18-DoF path: at the device state the LIO update left.
+// (:1588-1600) transformed by RGBpointBodyToWorld; the caller converts and publishes it as before.  x, y, z are written,
+// and the intensity too when the scan carries one (flb::preprocess -> undistort_pcl_on_device -> downsample_scan);
+// with a host-uploaded scan the points' other fields are left as they were.  18-DoF path: at the device state the LIO
+// update left.
 template <class PointCloud>
 inline int effect_cloud_fill(flb_handle* h, int n, PointCloud& cloud) {
-    std::vector<float> xyz((size_t)n * 3);
+    std::vector<float> rec((size_t)n * 12);
     int m = 0;
-    check(h, flb_effect_cloud_download(h, xyz.data(), n, &m));
+    const int rc = flb_effect_cloud_download_points(h, rec.data(), n, &m);
+    const bool with_intensity = rc == FLB_OK;
+    if (!with_intensity) {
+        if (rc != FLB_ERR_STATE) check(h, rc);
+        check(h, flb_effect_cloud_download(h, rec.data(), n, &m));   // no intensity: packed x, y, z
+    }
     cloud.resize((size_t)n);
+    const size_t w = with_intensity ? 12 : 3;
     for (int i = 0; i < n; ++i) {
-        cloud.points[i].x = xyz[3 * (size_t)i];
-        cloud.points[i].y = xyz[3 * (size_t)i + 1];
-        cloud.points[i].z = xyz[3 * (size_t)i + 2];
+        cloud.points[i].x = rec[w * (size_t)i];
+        cloud.points[i].y = rec[w * (size_t)i + 1];
+        cloud.points[i].z = rec[w * (size_t)i + 2];
+        if (with_intensity) cloud.points[i].intensity = rec[w * (size_t)i + 8];
     }
     return n;
 }
@@ -197,6 +208,53 @@ inline int publish_effect_world(flb_handle* h, const flb_lio_params& lio_prm, co
     int n = 0;
     check(h, flb_effect_cloud(h, &lio_prm, Rm, pv, &n));
     return effect_cloud_fill(h, n, laserCloudWorld);
+}
+
+// ---- publish_frame_world (src/laserMapping.cpp:780-813, img_enable: 0) and its pcd_save_en map from the device --------
+// The intensity records are pcl::PointXYZINormal's layout: x y z data[3] | normal data_n | intensity curvature 0 0.  P
+// (PointType) must be that type, and its default constructor must leave data[3] = 1 and the rest zero, because the
+// records carry those bytes (RGBpointBodyToWorld writes into a fresh PointCloudXYZI(size, 1)).
+template <class P>
+inline void xyzi_point_check() {
+    static_assert(sizeof(P) == 48, "PointType must be pcl::PointXYZINormal's 48 bytes");
+    static_assert(offsetof(P, intensity) == 32 && offsetof(P, curvature) == 36,
+                  "PointType's intensity and curvature must sit at bytes 32 and 36");
+    static const bool defaults_ok = [] {
+        const P p{};
+        return p.data[3] == 1.0f && p.normal_x == 0.f && p.normal_y == 0.f && p.normal_z == 0.f && p.intensity == 0.f &&
+               p.curvature == 0.f;
+    }();
+    if (!defaults_ok)
+        throw Error(FLB_ERR_INVALID, "flb: PointType() does not construct data[3] = 1 and zero normal / intensity / curvature "
+                                     "(the intensity records do)");
+}
+// Fills the published cloud of publish_frame_world (pcl_wait_pub) from the world cloud (flb_world_cloud of a source that
+// carries intensity: flb::preprocess, undistort_pcl_on_device and, for dense_map_en = 0, downsample_scan), one copy and
+// no host loop.  With pcd_save_en, flb_lidar_save_begin at start-up makes it append to the device's save too (:812).
+template <class PointCloud>
+inline int publish_frame_world(flb_handle* h, PointCloud& pcl_wait_pub) {
+    xyzi_point_check<typename std::decay<decltype(pcl_wait_pub.points[0])>::type>();
+    int n = 0;
+    check(h, flb_world_cloud_download(h, nullptr, 0, &n));       // the count only
+    pcl_wait_pub.resize((size_t)n);
+    check(h, flb_world_cloud_points(h, n > 0 ? &pcl_wait_pub.points[0] : nullptr, n, &n));   // one copy, and the save's append
+    return n;
+}
+// pcl_wait_save_lidar at exit (intensity_sacn_all.pcd, :1848-1853): the whole device save, filled slice by slice.
+// Throws flb::Error when frames were dropped at flb_lidar_save_begin's cap: a map with holes is not written silently.
+template <class PointCloud>
+inline int64_t save_intensity_map(flb_handle* h, PointCloud& pcl_wait_save_lidar) {
+    xyzi_point_check<typename std::decay<decltype(pcl_wait_save_lidar.points[0])>::type>();
+    int64_t n = 0, dropped = 0;
+    check(h, flb_lidar_save_size(h, &n, &dropped, nullptr));
+    if (dropped > 0)
+        throw Error(FLB_ERR_STATE, "flb::save_intensity_map: " + std::to_string((long long)dropped) +
+                                       " points were dropped at flb_lidar_save_begin's max_points");
+    pcl_wait_save_lidar.resize((size_t)n);
+    const int64_t kSlice = (int64_t)1 << 22;
+    for (int64_t first = 0; first < n; first += kSlice)
+        check(h, flb_lidar_save_download(h, first, n - first < kSlice ? n - first : kSlice, &pcl_wait_save_lidar.points[(size_t)first]));
+    return n;
 }
 
 // ---- publish_frame_world_rgb (src/laserMapping.cpp:710-777) and the pcd_save_en map from the device ---------------
@@ -579,16 +637,27 @@ inline LidarInfo preprocess(flb_handle* h, const LivoxMsg& msg, int n_scans, dou
     } else {
         f.off_x = 4, f.off_y = 8, f.off_z = 12, f.off_tag = 17, f.off_line = 18;
     }
+    const int off_intensity = (int)offsetof(typename std::decay<decltype(msg.points[0])>::type, reflectivity);
     f.n_scans = n_scans;
     f.point_filter_num = point_filter_num;
     f.blind = blind;
-    check(h, flb_lidar_upload(h, &f, n > 0 ? &msg.points[0] : nullptr, n, &r.n_points, &r.last_offset_ms));
+    check(h, flb_lidar_upload_intensity(h, &f, off_intensity, n > 0 ? &msg.points[0] : nullptr, n, &r.n_points, &r.last_offset_ms));
     return r;
+}
+
+// The PointCloud2's `intensity` field when it is FLOAT32, else -1: pcl::fromROSMsg maps a field into the typed cloud only
+// when name and datatype match, so any other intensity leaves every point's at 0.
+template <class PointCloud2>
+inline int intensity_field(const PointCloud2& msg) {
+    enum { kFloat32 = 7 };                               // sensor_msgs::PointField::FLOAT32
+    for (const auto& fld : msg.fields)
+        if (fld.name == "intensity" && (int)fld.datatype == kFloat32) return (int)fld.offset;
+    return -1;
 }
 
 // sensor_msgs::PointCloud2 (.fields[].name / .offset, .point_step, .width, .height, .data): oust64_handler,
 // velodyne_handler (clouds with per-point times) or xt32_handler by `kind` (FLB_LIDAR_*).  The time field is the one
-// the handler's point type names: t (Ouster), time (Velodyne), timestamp (XT32).
+// the handler's point type names: t (Ouster), time (Velodyne), timestamp (XT32).  The intensity is kept (intensity_field).
 template <class PointCloud2>
 inline LidarInfo preprocess(flb_handle* h, const PointCloud2& msg, int kind, int n_scans, double blind, int point_filter_num) {
     flb_lidar_format f{};
@@ -607,13 +676,14 @@ inline LidarInfo preprocess(flb_handle* h, const PointCloud2& msg, int kind, int
     f.blind = blind;
     LidarInfo r{};
     const int n = (int)((size_t)msg.width * msg.height);
-    check(h, flb_lidar_upload(h, &f, n > 0 ? msg.data.data() : nullptr, n, &r.n_points, &r.last_offset_ms));
+    check(h, flb_lidar_upload_intensity(h, &f, intensity_field(msg), n > 0 ? msg.data.data() : nullptr, n, &r.n_points,
+                                        &r.last_offset_ms));
     return r;
 }
 
 // sensor_msgs::PointCloud2 of any Velodyne driver: velodyne_handler with or without per-point times, fields at any
 // offset.  x, y, z (FLOAT32) and ring (UINT16) are looked up by name, time (FLOAT32) when the cloud has one; a missing
-// field or another datatype throws.  yaw_times = the times came from the yaw angle (!given_offset_time, src/preprocess.cpp:279).
+// field or another datatype throws.  The intensity is kept (intensity_field).  yaw_times = the times came from the yaw angle (!given_offset_time, src/preprocess.cpp:279).
 struct VelodyneInfo : LidarInfo {
     bool yaw_times;
 };
@@ -639,7 +709,8 @@ inline VelodyneInfo preprocess_velodyne(flb_handle* h, const PointCloud2& msg, i
     VelodyneInfo r{};
     int yaw = 0;
     const int n = (int)((size_t)msg.width * msg.height);
-    check(h, flb_lidar_upload_velodyne(h, &f, n > 0 ? msg.data.data() : nullptr, n, &r.n_points, &r.last_offset_ms, &yaw));
+    check(h, flb_lidar_upload_velodyne_intensity(h, &f, intensity_field(msg), n > 0 ? msg.data.data() : nullptr, n, &r.n_points,
+                                                 &r.last_offset_ms, &yaw));
     r.yaw_times = yaw != 0;
     return r;
 }

@@ -184,6 +184,11 @@ CLOUD_SCAN, CLOUD_UNDISTORTED = 0, 1       # flb_world_cloud sources (FLB_CLOUD_
 # flb_rgb_cloud's 32-byte record, the layout of pcl::PointXYZRGB: x y z, w = data[3] (1.0), b g r a, 12 zero bytes
 RGB_POINT = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("w", "<f4"), ("b", "u1"), ("g", "u1"), ("r", "u1"), ("a", "u1"),
                       ("pad", "u1", 12)])
+# the 48-byte record of the intensity outputs (flb_lidar_download_points, flb_world_cloud_points,
+# flb_effect_cloud_download_points, flb_lidar_save_download), the layout of pcl::PointXYZINormal: x y z, w = data[3] (1.0),
+# normal and data_n (zero), intensity, curvature, 8 zero bytes
+XYZINORMAL_POINT = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("w", "<f4"), ("normal", "<f4", 4), ("intensity", "<f4"),
+                             ("curvature", "<f4"), ("pad", "<f4", 2)])
 LIDAR_LIVOX, LIDAR_VELODYNE, LIDAR_OUSTER, LIDAR_XT32 = 1, 2, 3, 4    # flb_lidar_format.kind (FLB_LIDAR_*)
 GRAY_CV4, GRAY_CV3 = 0, 1                  # flb_image_upload_bgr's cvtColor rules (FLB_GRAY_*)
 # flb_image_upload_msg's encodings (FLB_ENC_*), keyed by sensor_msgs::Image's encoding string
@@ -210,7 +215,9 @@ SYMBOLS = ["flb_abi_version", "flb_create", "flb_destroy", "flb_last_error", "fl
            "flb_image_upload_bgr", "flb_image_download",
            "flb_lidar_upload", "flb_lidar_download", "flb_imu_undistort_lidar", "flb_lidar_upload_velodyne",
            "flb_lidar_upload_features", "flb_lidar_upload_velodyne_features", "flb_image_upload_msg",
-           "flb_keypatch_image"]
+           "flb_keypatch_image", "flb_lidar_upload_intensity", "flb_lidar_upload_velodyne_intensity", "flb_lidar_download_points",
+           "flb_world_cloud_points", "flb_effect_cloud_download_points", "flb_lidar_save_begin", "flb_lidar_save_size",
+           "flb_lidar_save_download", "flb_lidar_save_end"]
 
 
 def lib_path() -> str:
@@ -273,6 +280,16 @@ def lib():
                                                 C.POINTER(C.c_float)]
         L.flb_lidar_upload_velodyne_features.argtypes = [vp, C.POINTER(VelodyneFormat), C.c_double, vp, C.c_int, C.POINTER(C.c_int),
                                                          C.POINTER(C.c_float), C.POINTER(C.c_int)]
+        L.flb_lidar_upload_intensity.argtypes = [vp, C.POINTER(LidarFormat), C.c_int, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_float)]
+        L.flb_lidar_upload_velodyne_intensity.argtypes = [vp, C.POINTER(VelodyneFormat), C.c_int, vp, C.c_int, C.POINTER(C.c_int),
+                                                          C.POINTER(C.c_float), C.POINTER(C.c_int)]
+        L.flb_lidar_download_points.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_world_cloud_points.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_effect_cloud_download_points.argtypes = [vp, vp, C.c_int, C.POINTER(C.c_int)]
+        L.flb_lidar_save_begin.argtypes = [vp, C.c_int64]
+        L.flb_lidar_save_size.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.flb_lidar_save_download.argtypes = [vp, C.c_int64, C.c_int64, vp]
+        L.flb_lidar_save_end.argtypes = [vp]
         L.flb_imu_undistort_lidar.argtypes = [vp, C.POINTER(ImuParams), C.POINTER(ImuCarry), vp, C.c_int, C.c_double, C.c_double,
                                               C.c_double, C.c_int, C.POINTER(C.c_int), vp, C.c_int, vp, C.POINTER(C.c_int)]
         L.flb_visual_candidates.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
@@ -760,6 +777,38 @@ class Handle:
         self._ck(self.L.flb_world_cloud_download(self.h, _p(out), len(out), C.byref(n)))
         return out[:n.value]
 
+    def world_cloud_points(self, download=True):
+        """flb_world_cloud_points: publish_frame_world's pcl_wait_pub, (n,) XYZINORMAL_POINT records (appended to an open
+        LiDAR save).  download=False: points48 = NULL (only the save append); returns the point count."""
+        n = C.c_int()
+        if not download:
+            self._ck(self.L.flb_world_cloud_points(self.h, None, 0, C.byref(n)))
+            return n.value
+        out = np.zeros(self._wc_n, XYZINORMAL_POINT)
+        self._ck(self.L.flb_world_cloud_points(self.h, _p(out), len(out), C.byref(n)))
+        return out[:n.value]
+
+    def lidar_save_begin(self, max_points):
+        self._ck(self.L.flb_lidar_save_begin(self.h, int(max_points)))
+
+    def lidar_save_size(self):
+        """flb_lidar_save_size: dict(n, dropped, device_bytes)."""
+        n, d, b = C.c_int64(), C.c_int64(), C.c_int64()
+        self._ck(self.L.flb_lidar_save_size(self.h, C.byref(n), C.byref(d), C.byref(b)))
+        return dict(n=n.value, dropped=d.value, device_bytes=b.value)
+
+    def lidar_save_download(self, first=0, count=None):
+        """flb_lidar_save_download: records first .. first + count - 1 of the save (count None: to its end),
+        XYZINORMAL_POINT."""
+        if count is None:
+            count = self.lidar_save_size()["n"] - first
+        out = np.zeros(max(int(count), 0), XYZINORMAL_POINT)
+        self._ck(self.L.flb_lidar_save_download(self.h, int(first), int(count), _p(out)))
+        return out
+
+    def lidar_save_end(self):
+        self._ck(self.L.flb_lidar_save_end(self.h))
+
     # ---- the last LIO pass's effective points (publish_effect_world) on the device
     def effect_cloud(self, prm, R=None, p=None):
         """flb_effect_cloud: laserCloudOri of the last LIO pass at pose (R, p), or at the device state x when both are
@@ -777,6 +826,13 @@ class Handle:
         out = np.zeros((self._ef_n, 3), np.float32)
         n = C.c_int()
         self._ck(self.L.flb_effect_cloud_download(self.h, _p(out), len(out), C.byref(n)))
+        return out[:n.value]
+
+    def effect_cloud_download_points(self):
+        """flb_effect_cloud_download_points: the effect cloud with its intensities, (n,) XYZINORMAL_POINT records."""
+        out = np.zeros(self._ef_n, XYZINORMAL_POINT)
+        n = C.c_int()
+        self._ck(self.L.flb_effect_cloud_download_points(self.h, _p(out), len(out), C.byref(n)))
         return out[:n.value]
 
     def vmap_select_cloud(self, Rcw, Pcw, leaf=0.2, blocking=True):
@@ -945,6 +1001,24 @@ class Handle:
         """flb_lidar_upload_velodyne_features (feature_extract_enable: 1).  Returns (pl_surf.size(),
         points.back().curvature after the sort, whether the times came from the yaw)."""
         return self._lidar_upload(self.L.flb_lidar_upload_velodyne_features, fmt, records, n_records, float(dis_b), yaw=True)
+
+    def lidar_upload_intensity(self, fmt: LidarFormat, records, off_intensity, n_records=None):
+        """flb_lidar_upload_intensity: lidar_upload keeping each point's intensity; off_intensity = the field's byte offset
+        (Livox reflectivity u8, others float32), or -1 (every point 0)."""
+        return self._lidar_upload(self.L.flb_lidar_upload_intensity, fmt, records, n_records, int(off_intensity))
+
+    def lidar_upload_velodyne_intensity(self, fmt: VelodyneFormat, records, off_intensity, n_records=None):
+        """flb_lidar_upload_velodyne_intensity: lidar_upload_velodyne keeping each point's float32 intensity (any offset;
+        -1: every point 0)."""
+        return self._lidar_upload(self.L.flb_lidar_upload_velodyne_intensity, fmt, records, n_records, int(off_intensity), yaw=True)
+
+    def lidar_download_points(self):
+        """flb_lidar_download_points: the current cloud as pl_surf holds it, (n,) XYZINORMAL_POINT records."""
+        n = C.c_int()
+        self._ck(self.L.flb_lidar_download_points(self.h, None, 0, C.byref(n)))
+        out = np.zeros(n.value, XYZINORMAL_POINT)
+        self._ck(self.L.flb_lidar_download_points(self.h, _p(out), n.value, None))
+        return out
 
     def lidar_download(self):
         """flb_lidar_download: the decoded, time-sorted cloud, (n, 4) float32 x, y, z, curvature."""

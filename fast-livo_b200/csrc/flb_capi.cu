@@ -70,6 +70,18 @@ struct PinBuf {
     }
 };
 
+// A run-long save of 16-byte records (flb_rgb_save_*, flb_lidar_save_*): chunks of 2^kSaveChunkLog2 records, `table`
+// their pointers on the device (table_n entries uploaded), `pack` the download's staging.  The save_* functions below
+// are its one implementation; each save brings its own expansion kernel.
+struct SaveStore {
+    bool on = false;
+    long long max = 0, n = 0, dropped = 0;
+    std::vector<uint4*> chunks;
+    size_t table_n = 0;
+    DevBuf<uint4*> table;
+    DevBuf<uint4> pack;
+};
+
 // Pinned staging area for host->device uploads.  An upload packs the caller's data into it and
 // enqueues the copy; `done` marks that copy, and the next user of the same area waits on it (normally
 // long complete), so uploads never block on the stream and the caller's buffer is free on return.
@@ -270,6 +282,10 @@ struct flb_handle {
     // updates already enqueued on `stream` still read this one, then swaps the two and makes `stream` wait for it
     DevBuf<float4> scan_alt, plane_alt;
     DevBuf<unsigned char> sel_alt, plane_ok_alt;
+    // each scan set's intensities in the caller's order (flb_scan_from_undistorted of an undistortion that carries them),
+    // swapped with the set; scan_has_int[_alt]: the set carries them
+    DevBuf<float> scan_int, scan_int_alt;
+    bool scan_has_int = false, scan_has_int_alt = false;
     cudaStream_t scan_stream = nullptr;
     cudaEvent_t ev_scan_ready = nullptr;
     cudaEvent_t ev_scan_free[2] = {nullptr, nullptr};   // [slot]: everything on `stream` that reads that slot has been enqueued before it
@@ -315,11 +331,20 @@ struct flb_handle {
     // count.  undist_n < 0: none (no call yet, or the last one failed)
     const float4* undist_pts = nullptr;
     int undist_n = -1;
+    // its intensities (flb_imu_undistort_lidar of a cloud that carries them: a copy, so a later upload does not change them)
+    DevBuf<float> undist_int;
+    bool undist_has_int = false;
     // flb_lidar_upload: the decoded, time-sorted cloud of the current driver message (meas.lidar) as {x, y, z, curvature}.
     // Double-buffered like the image: an upload decodes into lid_cloud_alt on copy_stream and swaps once it has
     // succeeded.  lid_n < 0: no cloud; lid_cursor: lidar_scan_index_now.  The scratch below belongs to copy_stream,
     // whose order fences its reuse.
     DevBuf<float4> lid_cloud, lid_cloud_alt;
+    // the intensity calls: each set's intensities (one float per point, swapped with it); lid_has_int: the current cloud
+    // carries them; lid_int_zero: they are all 0 and not stored (off_intensity -1, the feature calls).  lid_int_sorted:
+    // the radix sort's output; lid_pack: flb_lidar_download_points' records.
+    DevBuf<float> lid_int, lid_int_alt, lid_int_sorted;
+    bool lid_has_int = false, lid_int_zero = false;
+    DevBuf<uint4> lid_pack;
     InSlot lid_slot;
     int lid_n = -1, lid_cursor = 0;
     DevBuf<unsigned char> lid_raw, lid_cub;    // the raw records; cub's scratch
@@ -343,6 +368,10 @@ struct flb_handle {
     DevBuf<unsigned> wc_rec;           // bounds + non-finite record of the transform (kScanRec*)
     int wc_n = -1;
     float wc_lo[3] = {0, 0, 0}, wc_hi[3] = {0, 0, 0};
+    // its intensities, when its source carries them (wc_has_int), and flb_world_cloud_points' records
+    DevBuf<float> wc_int;
+    bool wc_has_int = false;
+    DevBuf<uint4> wc_pack;
     // flb_effect_cloud: laserCloudOri of the last LIO pass.  scan_gen counts scan installs; a pass records the generation
     // and point count of the set it ran on (ef_gen, ef_N) and is pending until captured.  The set survives one more
     // install (it becomes scan_alt), not two, nor flb_voxel_grid: then the pass is lost.  The capture keeps the rows'
@@ -355,6 +384,10 @@ struct flb_handle {
     DevBuf<int> ef_count;
     DevBuf<float> ef_xyz;
     DevBuf<unsigned> ef_rec;
+    // the captured rows' intensities when their scan set carries them (ef_has_int), and their records
+    DevBuf<float> ef_int;
+    bool ef_has_int = false;
+    DevBuf<uint4> ef_pack;
     // flb_rgb_cloud: laserCloudWorldRGB as 32-byte records (rc_out, rc_n of them; rc_n < 0: none held), the per-point
     // colour words, keep flags and their exclusive sum (n + 1 each), and the caller's colour frame when it passes one.
     // Buffers of its own: the LIO export's row mask (x_rowmask) stays valid.
@@ -363,14 +396,8 @@ struct flb_handle {
     DevBuf<int> rc_flag, rc_pos;
     DevBuf<unsigned char> rc_img;
     int rc_n = -1;
-    // flb_rgb_save_*: pcl_wait_save as 16-byte records in chunks of 2^kRgbChunkLog2 (rs_chunks), rs_table their pointers
-    // on the device (rs_table_n entries uploaded), rs_pack the download's staging.
-    bool rs_on = false;
-    long long rs_max = 0, rs_n = 0, rs_dropped = 0;
-    std::vector<uint4*> rs_chunks;
-    size_t rs_table_n = 0;
-    DevBuf<uint4*> rs_table;
-    DevBuf<uint4> rs_pack;
+    // flb_rgb_save_*: pcl_wait_save; flb_lidar_save_*: pcl_wait_save_lidar
+    SaveStore rgb_save, lidar_save;
     // flb_vmap_select_cloud: downSizeFilter of the world cloud and its scratch (the scan slot's stays untouched)
     DevBuf<float> wc_down;
     DevBuf<unsigned> wc_keys, wc_keys_sorted;
@@ -930,15 +957,103 @@ void note_lio_pass(flb_handle* h) {
     h->ef_N = h->N;
 }
 
-// flb_rgb_save_end / flb_destroy: the save's chunks, table and staging (cudaFree waits for the kernels that use them).
-void rgb_save_free(flb_handle* h) {
-    for (uint4* c : h->rs_chunks) cudaFree(c);
-    h->rs_chunks.clear();
-    h->rs_table_n = 0;
-    h->rs_table.release();
-    h->rs_pack.release();
-    h->rs_on = false;
-    h->rs_max = h->rs_n = h->rs_dropped = 0;
+// flb_*_save_end / flb_destroy: the save's chunks, table and staging (cudaFree waits for the kernels that use them).
+void save_free(SaveStore& s) {
+    for (uint4* c : s.chunks) cudaFree(c);
+    s.chunks.clear();
+    s.table_n = 0;
+    s.table.release();
+    s.pack.release();
+    s.on = false;
+    s.max = s.n = s.dropped = 0;
+}
+
+// Chunks for `need` save records, their pointers uploaded to the save's table on `stream` (a table that grows is
+// reallocated: cudaFree waits for the scatters reading the old one).  *ok = false when the device has no memory for one
+// more chunk: the frame is then dropped like one beyond the cap; the chunks that were allocated stay for later frames.
+int save_reserve(flb_handle* h, SaveStore& s, long long need, bool* ok) {
+    const size_t want = (size_t)((need + (1LL << kSaveChunkLog2) - 1) >> kSaveChunkLog2);
+    while (s.chunks.size() < want) {
+        uint4* c = nullptr;
+        if (cudaMalloc(&c, ((size_t)1 << kSaveChunkLog2) * sizeof(uint4)) != cudaSuccess) {
+            cudaGetLastError();                       // an allocation failure is not sticky: clear it
+            break;
+        }
+        s.chunks.push_back(c);
+    }
+    if (s.chunks.size() > s.table_n) {
+        FLB_CUDA(h, s.table.reserve(s.chunks.size()));
+        FLB_CUDA(h, cudaMemcpyAsync(s.table.p, s.chunks.data(), s.chunks.size() * sizeof(uint4*), cudaMemcpyHostToDevice, h->stream));
+        s.table_n = s.chunks.size();
+    }
+    *ok = s.chunks.size() >= want;
+    return FLB_OK;
+}
+
+// A frame of m records for the save: *table = the chunk table to scatter into from s.n on, or nullptr when the save is
+// closed, m is 0, or the frame is dropped (past the cap, or no memory for a chunk: counted in `dropped`).  The caller
+// adds m to s.n once it has enqueued the scatter into the table.
+int save_frame(flb_handle* h, SaveStore& s, int m, uint4* const** table) {
+    *table = nullptr;
+    if (!s.on || m <= 0) return FLB_OK;
+    bool ok = m <= s.max - s.n;
+    if (ok) { int rcs = save_reserve(h, s, s.n + m, &ok); if (rcs) return rcs; }
+    if (ok) *table = s.table.p;
+    else s.dropped += m;                              // the frame's cloud is still built: saving never stops publishing
+    return FLB_OK;
+}
+
+int save_begin(flb_handle* h, SaveStore& s, const char* who, int64_t max_points) {
+    if (max_points < 1) return fail(h, FLB_ERR_INVALID, "%s_begin: max_points %lld < 1", who, (long long)max_points);
+    if (s.on) return fail(h, FLB_ERR_STATE, "%s_begin: a save is open (%s_end first)", who, who);
+    s.on = true;
+    s.max = max_points;
+    s.n = s.dropped = 0;
+    return FLB_OK;
+}
+
+int save_size(flb_handle* h, const SaveStore& s, const char* who, int64_t* n, int64_t* dropped, int64_t* device_bytes) {
+    if (!s.on) return fail(h, FLB_ERR_STATE, "%s_size: no save open (%s_begin first)", who, who);
+    if (n) *n = s.n;
+    if (dropped) *dropped = s.dropped;
+    if (device_bytes)
+        *device_bytes = (int64_t)(s.chunks.size() * ((size_t)1 << kSaveChunkLog2) * sizeof(uint4) + s.table.cap * sizeof(uint4*) +
+                                  s.pack.cap * sizeof(uint4));
+    return FLB_OK;
+}
+
+// Records first .. first + count - 1, expanded by the save's kernel `expand` to `words` 16-byte words each, into dst.
+// One bounded slice at a time: `expand` writes it to the staging, the copy takes it out; stream order keeps the next
+// slice's expansion behind the copy.
+typedef void (*SaveExpandKernel)(uint4* const*, long long, int, uint4*);
+int save_download(flb_handle* h, SaveStore& s, const char* who, int64_t first, int64_t count, void* out, int words,
+                  SaveExpandKernel expand) {
+    if (!s.on) return fail(h, FLB_ERR_STATE, "%s_download: no save open (%s_begin first)", who, who);
+    if (first < 0 || count < 0 || count > s.n - first || (count > 0 && !out))
+        return fail(h, FLB_ERR_INVALID, "%s_download: bad arguments (records %lld + %lld of %lld)", who, (long long)first,
+                    (long long)count, s.n);
+    if (count == 0) return FLB_OK;
+    constexpr long long kSlice = 1LL << 18;
+    FLB_CUDA(h, s.pack.reserve((size_t)words * (size_t)std::min<long long>(count, kSlice)));
+    char* dst = static_cast<char*>(out);
+    for (long long done = 0; done < count; done += kSlice) {
+        const int k = (int)std::min<long long>(count - done, kSlice);
+        {
+            LaunchScope ls(h, FAM_OTHER);
+            expand<<<(k + 255) / 256, 256, 0, h->stream>>>(s.table.p, first + done, k, s.pack.p);
+            FLB_CUDA(h, cudaGetLastError());
+        }
+        FLB_CUDA(h, cudaMemcpyAsync(dst + done * words * (long long)sizeof(uint4), s.pack.p, (size_t)k * words * sizeof(uint4),
+                                    cudaMemcpyDeviceToHost, h->stream));
+    }
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    return FLB_OK;
+}
+
+int save_end(flb_handle* h, SaveStore& s) {
+    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    save_free(s);
+    return FLB_OK;
 }
 
 // Flag base for one persistent launch: flags epoch+1 .. epoch+4095 belong to it alone.  On wrap-around the
@@ -1329,7 +1444,10 @@ int flb_destroy(flb_handle* h) {
     h->wc_vals.release(); h->wc_vals_sorted.release(); h->wc_heads.release(); h->wc_box.release();
     h->ef_scatter.release(); h->ef_body.release(); h->ef_flag.release(); h->ef_count.release(); h->ef_xyz.release(); h->ef_rec.release();
     h->rc_out.release(); h->rc_bgra.release(); h->rc_flag.release(); h->rc_pos.release(); h->rc_img.release();
-    rgb_save_free(h);
+    save_free(h->rgb_save);
+    save_free(h->lidar_save);
+    h->lid_int.release(); h->lid_int_alt.release(); h->lid_int_sorted.release(); h->lid_pack.release(); h->undist_int.release();
+    h->scan_int.release(); h->scan_int_alt.release(); h->wc_int.release(); h->wc_pack.release(); h->ef_int.release(); h->ef_pack.release();
     h->sf_keys.release(); h->sf_keys_sorted.release(); h->sf_rec.release(); h->sf_vals.release(); h->sf_vals_sorted.release();
     h->sf_heads.release(); h->sf_xyz.release();
     h->cell_table.release(); h->cell_keys.release(); h->cell_keys_alt.release();
@@ -1899,20 +2017,24 @@ int flb_map_add_scan(flb_handle* h, const flb_lio_params* prm, const double R[9]
 int flb_world_cloud(flb_handle* h, const flb_lio_params* prm, const double R[9], const double p[3], int source, int* n_out) {
     FLB_CHECK_H(h);
     h->wc_n = -1;                                     // on any error below, no cloud is held
+    h->wc_has_int = false;
     if (n_out) *n_out = 0;
     if (!prm || (R == nullptr) != (p == nullptr) || (source != FLB_CLOUD_SCAN && source != FLB_CLOUD_UNDISTORTED))
         return fail(h, FLB_ERR_INVALID, "flb_world_cloud: bad arguments (prm, R and p both or neither, source)");
     const float4* src = nullptr;
+    const float* src_int = nullptr;                   // the source's intensities in the caller's order, when it carries them
     int n = 0;
     if (source == FLB_CLOUD_SCAN) {
         if (h->comm || h->p2p.world > 0)
             return fail(h, FLB_ERR_STATE, "flb_world_cloud: FLB_CLOUD_SCAN is single GPU only (each rank holds only its shard of the scan)");
         if (!h->scan_valid) return fail(h, FLB_ERR_STATE, "flb_world_cloud: no scan uploaded since the last flb_voxel_grid (or ever)");
         src = h->scan.p;
+        src_int = h->scan_has_int ? h->scan_int.p : nullptr;
         n = h->N;
     } else {
         if (h->undist_n < 0) return fail(h, FLB_ERR_STATE, "flb_world_cloud: no flb_imu_undistort output (none yet, or the last call failed)");
         src = h->undist_pts;
+        src_int = h->undist_has_int ? h->undist_int.p : nullptr;
         n = h->undist_n;
     }
     if (!R && !h->state_valid) return fail(h, FLB_ERR_STATE, "flb_world_cloud: no pose given and no device state");
@@ -1926,8 +2048,13 @@ int flb_world_cloud(flb_handle* h, const flb_lio_params* prm, const double R[9],
         for (int k = 0; k < 3; ++k)
             if (lo[k] < -kVmapCoordLimit || hi[k] > kVmapCoordLimit) return fail(h, FLB_ERR_INVALID, "flb_world_cloud: coordinate beyond 2^20 visual-map voxels");
     }
+    if (src_int && n > 0) {
+        FLB_CUDA(h, h->wc_int.reserve(n));
+        FLB_CUDA(h, cudaMemcpyAsync(h->wc_int.p, src_int, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+    }
     std::memcpy(h->wc_lo, lo, sizeof(lo));
     std::memcpy(h->wc_hi, hi, sizeof(hi));
+    h->wc_has_int = src_int != nullptr;
     h->wc_n = n;
     if (n_out) *n_out = n;
     return FLB_OK;
@@ -1946,14 +2073,45 @@ int flb_world_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out
     return FLB_OK;
 }
 
+// publish_frame_world's pcl_wait_pub (src/laserMapping.cpp:780-813): the world cloud with its intensities as 48-byte
+// records, packed by one kernel into wc_pack and copied out once; with a LiDAR save open the same kernel appends the
+// frame's save records (`*pcl_wait_save_lidar += *pcl_wait_pub`, :812).
+int flb_world_cloud_points(flb_handle* h, void* points48, int capacity, int* n_out) {
+    FLB_CHECK_H(h);
+    const char* who = "flb_world_cloud_points";
+    if (capacity < 0 || (capacity > 0 && !points48)) return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
+    if (h->wc_n < 0) return fail(h, FLB_ERR_STATE, "%s: no world cloud (flb_world_cloud first, or it failed)", who);
+    if (!h->wc_has_int) return fail(h, FLB_ERR_STATE, "%s: the world cloud's source carries no intensity", who);
+    const int n = h->wc_n;
+    if (n_out) *n_out = n;
+    uint4* const* table = nullptr;
+    { int rcs = save_frame(h, h->lidar_save, n, &table); if (rcs) return rcs; }
+    const int m = points48 ? std::min(capacity, n) : 0;
+    if (table || m > 0) {
+        FLB_CUDA(h, h->wc_pack.reserve(3 * (size_t)n));
+        LaunchScope ls(h, FAM_OTHER);
+        k_xyzi_scatter<<<(n + 255) / 256, 256, 0, h->stream>>>(h->wc_xyz.p, h->wc_int.p, n, h->wc_pack.p, table, h->lidar_save.n);
+        FLB_CUDA(h, cudaGetLastError());
+    }
+    if (table) h->lidar_save.n += n;
+    if (m > 0) {
+        FLB_CUDA(h, cudaMemcpyAsync(points48, h->wc_pack.p, (size_t)m * 3 * sizeof(uint4), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    }
+    return FLB_OK;
+}
+
 // laserCloudOri of the pending pass into ef_body: the rows of the scan set it ran on (the current one, or scan_alt after
 // one more install), scattered to their caller's index by k_effect_scatter and compacted in that order by cub's select.
 // Runs on `stream` after the pass; the count read ends with a stream synchronise, so a later install cannot overwrite
 // the set under it.
+// With an intensity on the set, the same select compacts the set's intensities (caller order) into ef_int.
 static int effect_capture(flb_handle* h) {
     const bool cur = h->scan_gen == h->ef_gen;
     const float4* scan = cur ? h->scan.p : h->scan_alt.p;
     const unsigned char* sel = cur ? h->sel.p : h->sel_alt.p;
+    const bool carry = cur ? h->scan_has_int : h->scan_has_int_alt;
+    const float* scan_int = cur ? h->scan_int.p : h->scan_int_alt.p;
     const int N = h->ef_N;
     int n = 0;
     if (N > 0) {
@@ -1971,12 +2129,20 @@ static int effect_capture(flb_handle* h) {
         FLB_CUDA(h, h->cub_tmp.reserve(tmp_bytes));
         FLB_CUDA(h, cub::DeviceSelect::Flagged(h->cub_tmp.p, tmp_bytes, h->ef_scatter.p, h->ef_flag.p, h->ef_body.p, h->ef_count.p, N, h->stream));
         h->launches++;
+        if (carry) {
+            FLB_CUDA(h, h->ef_int.reserve(N));
+            FLB_CUDA(h, cub::DeviceSelect::Flagged(nullptr, tmp_bytes, scan_int, h->ef_flag.p, h->ef_int.p, h->ef_count.p, N, h->stream));
+            FLB_CUDA(h, h->cub_tmp.reserve(tmp_bytes));
+            FLB_CUDA(h, cub::DeviceSelect::Flagged(h->cub_tmp.p, tmp_bytes, scan_int, h->ef_flag.p, h->ef_int.p, h->ef_count.p, N, h->stream));
+            h->launches++;
+        }
         int* cnt = static_cast<int*>(h->pin_out.p);
         FLB_CUDA(h, cudaMemcpyAsync(cnt, h->ef_count.p, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
         FLB_CUDA(h, cudaStreamSynchronize(h->stream));
         n = *cnt;
     }
     h->ef_n = n;
+    h->ef_has_int = carry;
     h->ef_state = flb_handle::kEfNone;
     return FLB_OK;
 }
@@ -2019,6 +2185,47 @@ int flb_effect_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_ou
         FLB_CUDA(h, cudaStreamSynchronize(h->stream));
     }
     return FLB_OK;
+}
+
+int flb_effect_cloud_download_points(flb_handle* h, void* points48, int capacity, int* n_out) {
+    FLB_CHECK_H(h);
+    const char* who = "flb_effect_cloud_download_points";
+    if (capacity < 0 || (capacity > 0 && !points48)) return fail(h, FLB_ERR_INVALID, "%s: bad arguments", who);
+    if (h->ef_wn < 0) return fail(h, FLB_ERR_STATE, "%s: no effect cloud (flb_effect_cloud first, or it failed)", who);
+    if (!h->ef_has_int) return fail(h, FLB_ERR_STATE, "%s: the effect cloud's scan carries no intensity", who);
+    if (n_out) *n_out = h->ef_wn;
+    const int m = std::min(capacity, h->ef_wn);
+    if (m > 0) {
+        FLB_CUDA(h, h->ef_pack.reserve(3 * (size_t)m));
+        {
+            LaunchScope ls(h, FAM_OTHER);
+            k_xyzi_scatter<<<(m + 255) / 256, 256, 0, h->stream>>>(h->ef_xyz.p, h->ef_int.p, m, h->ef_pack.p, nullptr, 0);
+            FLB_CUDA(h, cudaGetLastError());
+        }
+        FLB_CUDA(h, cudaMemcpyAsync(points48, h->ef_pack.p, (size_t)m * 3 * sizeof(uint4), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    }
+    return FLB_OK;
+}
+
+int flb_lidar_save_begin(flb_handle* h, int64_t max_points) {
+    FLB_CHECK_H(h);
+    return save_begin(h, h->lidar_save, "flb_lidar_save", max_points);
+}
+
+int flb_lidar_save_size(flb_handle* h, int64_t* n, int64_t* dropped, int64_t* device_bytes) {
+    FLB_CHECK_H(h);
+    return save_size(h, h->lidar_save, "flb_lidar_save", n, dropped, device_bytes);
+}
+
+int flb_lidar_save_download(flb_handle* h, int64_t first, int64_t count, void* points48) {
+    FLB_CHECK_H(h);
+    return save_download(h, h->lidar_save, "flb_lidar_save", first, count, points48, 3, k_xyzi_save_pack);
+}
+
+int flb_lidar_save_end(flb_handle* h) {
+    FLB_CHECK_H(h);
+    return save_end(h, h->lidar_save);
 }
 
 int flb_map_delete_boxes(flb_handle* h, const float* boxes, int nb) {
@@ -2226,6 +2433,7 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
                       float* out_xyz, double* poses_out, int* n_poses_out) {
     FLB_CHECK_H(h);
     h->undist_n = -1;                 // flb_world_cloud's FLB_CLOUD_UNDISTORTED source is this call's output, or none
+    h->undist_has_int = false;
     if (!prm || !carry || !v_imu || n_imu < 1 || n_points < 0 || (n_points > 0 && !pts) || stride < 4 ||
         offset_index < 3 || offset_index >= stride)
         return fail(h, FLB_ERR_INVALID, "flb_imu_undistort: bad arguments");
@@ -2267,6 +2475,7 @@ int lidar_format(flb_handle* h, const char* who, const flb_lidar_format* fmt, co
     f->kind = fmt->kind, f->step = step, f->off_x = fmt->off_x, f->off_y = fmt->off_y, f->off_z = fmt->off_z, f->off_time = fmt->off_time;
     f->off_tag = livox ? fmt->off_tag : 0, f->off_line = line ? fmt->off_line : 0;
     f->n_scans = fmt->n_scans, f->filter_num = fmt->point_filter_num, f->blind = fmt->blind;
+    f->off_int = kLidarIntNone;
     return FLB_OK;
 }
 
@@ -2288,6 +2497,7 @@ int velo_format(flb_handle* h, const char* who, const flb_velodyne_format* fmt, 
     f->kind = kLidarVelodyne, f->step = step, f->off_x = fmt->off_x, f->off_y = fmt->off_y, f->off_z = fmt->off_z;
     f->off_time = fmt->off_time >= 0 ? fmt->off_time : 0, f->off_line = features ? fmt->off_ring : 0;
     f->n_scans = fmt->n_scans, f->filter_num = fmt->point_filter_num, f->blind = fmt->blind;
+    f->off_int = kLidarIntNone;
     *given = n_records == 0;
     if (n_records > 0 && fmt->off_time >= 0) {
         float t_last;
@@ -2337,9 +2547,13 @@ int lidar_begin(flb_handle* h, const void* records, int n_records, int step) {
     return vio_copy_begin(h, h->lid_slot);
 }
 
-// the idle cloud set, holding rec.n_kept points, becomes the current cloud with its cursor at the start
-int lidar_publish(flb_handle* h, const LidarRecord& rec, int* n_points, float* last_offset_ms) {
+// the idle cloud set, holding rec.n_kept points (and their intensities when f carries them), becomes the current cloud
+// with its cursor at the start
+int lidar_publish(flb_handle* h, const LidarFmt& f, const LidarRecord& rec, int* n_points, float* last_offset_ms) {
     std::swap(h->lid_cloud, h->lid_cloud_alt);
+    std::swap(h->lid_int, h->lid_int_alt);
+    h->lid_has_int = f.off_int != kLidarIntNone;
+    h->lid_int_zero = f.off_int == kLidarIntZero;
     h->lid_slot.slot ^= 1;
     h->lid_n = rec.n_kept;
     h->lid_cursor = 0;
@@ -2351,17 +2565,26 @@ int lidar_publish(flb_handle* h, const LidarRecord& rec, int* n_points, float* l
 // Every route's end, from n > 0 candidates (lid_dec, lf.kept): compact them into the idle cloud set, refuse (yaw: a ring
 // >= n_scans, named from the host records; then a kept value that is not finite, in the caller's words `what`), re-sort
 // the times when they are out of order, and publish.  t_sum, t_sort: lid_cub's sizes for the ExclusiveSum and the 32-bit
-// SortPairs over n items.  A refusal publishes nothing.
+// SortPairs over n items.  A refusal publishes nothing.  With an intensity field (f.off_int >= 0) the intensities are
+// compacted beside the points and re-sorted by a second stable sort on the same keys, which applies the same
+// permutation; an all-zero intensity (kLidarIntZero) is a flag, so the feature calls keep their launches.
 int lidar_tail(flb_handle* h, const char* who, const char* what, const LidarFlags& lf, int n, size_t t_sum, size_t t_sort,
-               const VeloYaw* yaw, const void* records, int step, int* n_points, float* last_offset_ms) {
+               const VeloYaw* yaw, const void* records, const LidarFmt& f, int* n_points, float* last_offset_ms) {
     cudaStream_t cs = h->copy_stream;
     const int g = (n + 255) / 256;
+    const bool carry = f.off_int >= 0;
     FLB_CUDA(h, cudaMemsetAsync(lf.rec, 0, sizeof(LidarRecord), cs));
     FLB_CUDA(h, cub::DeviceScan::ExclusiveSum(h->lid_cub.p, t_sum, lf.kept, lf.pos, n, cs));
     k_lidar_scatter<<<g, 256, 0, cs>>>(h->lid_dec.p, lf.kept, lf.pos, n, h->lid_cloud_alt.p, h->lid_keys.p, lf.rec);
     k_lidar_order<<<g, 256, 0, cs>>>(h->lid_cloud_alt.p, h->lid_keys.p, n, lf.rec);
     FLB_CUDA(h, cudaGetLastError());
     h->launches += 3;
+    if (carry) {
+        FLB_CUDA(h, h->lid_int_alt.reserve(n));
+        k_lidar_intensity<<<g, 256, 0, cs>>>(h->lid_raw.p, n, f, lf.kept, lf.pos, h->lid_int_alt.p);
+        FLB_CUDA(h, cudaGetLastError());
+        h->launches += 1;
+    }
     LidarRecord rec{};
     int bad_ring = INT_MAX;
     FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, lf.rec, sizeof(rec) + (yaw ? sizeof(int) : 0), cudaMemcpyDeviceToHost, cs));
@@ -2370,7 +2593,7 @@ int lidar_tail(flb_handle* h, const char* who, const char* what, const LidarFlag
     if (yaw) std::memcpy(&bad_ring, static_cast<const char*>(h->pin_lidar.p) + sizeof(rec), sizeof(int));
     if (bad_ring < n) {
         uint16_t ring;
-        std::memcpy(&ring, static_cast<const unsigned char*>(records) + (size_t)bad_ring * step + yaw->off_ring, sizeof(ring));
+        std::memcpy(&ring, static_cast<const unsigned char*>(records) + (size_t)bad_ring * f.step + yaw->off_ring, sizeof(ring));
         return fail(h, FLB_ERR_INVALID, "%s: record %d has ring %u >= n_scans %d (the per-ring yaw state has no such ring)", who,
                     bad_ring, (unsigned)ring, yaw->n_scans);
     }
@@ -2384,11 +2607,22 @@ int lidar_tail(flb_handle* h, const char* who, const char* what, const LidarFlag
         k_lidar_last<<<1, 1, 0, cs>>>(h->lid_cloud_alt.p, lf.rec);
         FLB_CUDA(h, cudaGetLastError());
         h->launches += 3;
+        if (carry) {
+            size_t t_int = 0;
+            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(nullptr, t_int, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_int_alt.p,
+                                                        h->lid_int_sorted.p, rec.n_kept, 0, 32, cs));
+            FLB_CUDA(h, h->lid_cub.reserve(t_int));
+            FLB_CUDA(h, h->lid_int_sorted.reserve(rec.n_kept));
+            FLB_CUDA(h, cub::DeviceRadixSort::SortPairs(h->lid_cub.p, t_int, h->lid_keys.p, h->lid_keys_sorted.p, h->lid_int_alt.p,
+                                                        h->lid_int_sorted.p, rec.n_kept, 0, 32, cs));
+            FLB_CUDA(h, cudaMemcpyAsync(h->lid_int_alt.p, h->lid_int_sorted.p, (size_t)rec.n_kept * sizeof(float), cudaMemcpyDeviceToDevice, cs));
+            h->launches += 2;
+        }
         FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, lf.rec, sizeof(rec), cudaMemcpyDeviceToHost, cs));
         FLB_CUDA(h, cudaStreamSynchronize(cs));
         std::memcpy(&rec, h->pin_lidar.p, sizeof(rec));
     }
-    return lidar_publish(h, rec, n_points, last_offset_ms);
+    return lidar_publish(h, f, rec, n_points, last_offset_ms);
 }
 
 // flb_lidar_upload and flb_lidar_upload_velodyne from the argument checks on: decode and filter the records into
@@ -2400,7 +2634,7 @@ int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const v
     const bool livox = f.kind == kLidarLivox;
     const size_t n1 = std::max(n_records, 1);
     { int rcq = lidar_begin(h, records, n_records, step); if (rcq) return rcq; }
-    if (n_records == 0) return lidar_publish(h, LidarRecord{}, n_points, last_offset_ms);
+    if (n_records == 0) return lidar_publish(h, f, LidarRecord{}, n_points, last_offset_ms);
     cudaStream_t cs = h->copy_stream;
     const LidarFlags lf(h->lid_flags.p, n1);
     int* d_vnum = lf.own;
@@ -2446,17 +2680,28 @@ int lidar_upload_core(flb_handle* h, const char* who, const LidarFmt& f, const v
         k_lidar_flags<<<g, 256, 0, cs>>>(h->lid_raw.p, n_records, f, d_vnum, h->lid_dec.p, lf.kept);
         h->launches += 1;
     }
-    return lidar_tail(h, who, "a kept point or time", lf, n_records, t2, t3, yaw, records, step, n_points, last_offset_ms);
+    return lidar_tail(h, who, "a kept point or time", lf, n_records, t2, t3, yaw, records, f, n_points, last_offset_ms);
 }
 
-}  // namespace
+// The intensity field of the intensity calls: -1 (every point reads 0) or a field within the record, aligned to its type
+// when `aligned` (flb_lidar_upload_intensity: Livox u8, others float32; the Velodyne call takes any offset).
+int lidar_int_field(flb_handle* h, const char* who, int off_intensity, int bytes, int step, bool aligned, LidarFmt* f) {
+    if (off_intensity != -1 && !(aligned ? lidar_field_ok(off_intensity, bytes, step) : velo_field_ok(off_intensity, bytes, step)))
+        return fail(h, FLB_ERR_INVALID, "%s: off_intensity %d does not fit in point_step %d%s", who, off_intensity, step,
+                    aligned ? " or is not aligned to its type" : "");
+    f->off_int = off_intensity == -1 ? kLidarIntZero : off_intensity;
+    return FLB_OK;
+}
 
-int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* records, int n_records, int* n_points,
-                     float* last_offset_ms) {
-    FLB_CHECK_H(h);
-    const char* who = "flb_lidar_upload";
+// flb_lidar_upload and (intensity) flb_lidar_upload_intensity
+int lidar_upload_entry(flb_handle* h, const char* who, const flb_lidar_format* fmt, bool intensity, int off_intensity, const void* records,
+                       int n_records, int* n_points, float* last_offset_ms) {
     LidarFmt f;
     { int rcq = lidar_format(h, who, fmt, records, n_records, false, 0.0, &f); if (rcq) return rcq; }
+    if (intensity) {
+        int rci = lidar_int_field(h, who, off_intensity, f.kind == kLidarLivox ? 1 : 4, f.step, true, &f);
+        if (rci) return rci;
+    }
     const unsigned char* rec_h = static_cast<const unsigned char*>(records);
     if (n_records > 0 && f.kind == kLidarVelodyne) {
         float t_last;                                                              // given_offset_time, :279
@@ -2469,18 +2714,45 @@ int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* rec
     return lidar_upload_core(h, who, f, records, n_records, nullptr, n_points, last_offset_ms);
 }
 
-int flb_lidar_upload_velodyne(flb_handle* h, const flb_velodyne_format* fmt, const void* records, int n_records, int* n_points,
-                              float* last_offset_ms, int* yaw_times) {
-    FLB_CHECK_H(h);
-    const char* who = "flb_lidar_upload_velodyne";
+// flb_lidar_upload_velodyne and (intensity) flb_lidar_upload_velodyne_intensity
+int velo_upload_entry(flb_handle* h, const char* who, const flb_velodyne_format* fmt, bool intensity, int off_intensity,
+                      const void* records, int n_records, int* n_points, float* last_offset_ms, int* yaw_times) {
     LidarFmt f;
     bool given = false;
     { int rcq = velo_format(h, who, fmt, records, n_records, false, 0.0, &f, &given); if (rcq) return rcq; }
+    if (intensity) { int rci = lidar_int_field(h, who, off_intensity, 4, f.step, false, &f); if (rci) return rci; }
     VeloYaw yaw{fmt->off_ring, fmt->n_scans};
     const int rc = lidar_upload_core(h, who, f, records, n_records, given ? nullptr : &yaw, n_points, last_offset_ms);
     if (rc) return rc;
     if (yaw_times) *yaw_times = given ? 0 : 1;
     return FLB_OK;
+}
+
+}  // namespace
+
+int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* records, int n_records, int* n_points,
+                     float* last_offset_ms) {
+    FLB_CHECK_H(h);
+    return lidar_upload_entry(h, "flb_lidar_upload", fmt, false, 0, records, n_records, n_points, last_offset_ms);
+}
+
+int flb_lidar_upload_intensity(flb_handle* h, const flb_lidar_format* fmt, int off_intensity, const void* records, int n_records,
+                               int* n_points, float* last_offset_ms) {
+    FLB_CHECK_H(h);
+    return lidar_upload_entry(h, "flb_lidar_upload_intensity", fmt, true, off_intensity, records, n_records, n_points, last_offset_ms);
+}
+
+int flb_lidar_upload_velodyne(flb_handle* h, const flb_velodyne_format* fmt, const void* records, int n_records, int* n_points,
+                              float* last_offset_ms, int* yaw_times) {
+    FLB_CHECK_H(h);
+    return velo_upload_entry(h, "flb_lidar_upload_velodyne", fmt, false, 0, records, n_records, n_points, last_offset_ms, yaw_times);
+}
+
+int flb_lidar_upload_velodyne_intensity(flb_handle* h, const flb_velodyne_format* fmt, int off_intensity, const void* records,
+                                        int n_records, int* n_points, float* last_offset_ms, int* yaw_times) {
+    FLB_CHECK_H(h);
+    return velo_upload_entry(h, "flb_lidar_upload_velodyne_intensity", fmt, true, off_intensity, records, n_records, n_points,
+                             last_offset_ms, yaw_times);
 }
 
 // ---- the feature branches: give_feature's pl_surf ------------------------------------------------------------------
@@ -2517,7 +2789,7 @@ int lidar_features_core(flb_handle* h, const char* who, const LidarFmt& f, doubl
     FLB_CUDA(h, h->feat_st.reserve(n1));
     FLB_CUDA(h, h->feat_u8.reserve(2 * n1));
     { int rcq = lidar_begin(h, records, n_records, f.step); if (rcq) return rcq; }
-    if (n_records == 0) return lidar_publish(h, LidarRecord{}, n_points, last_offset_ms);
+    if (n_records == 0) return lidar_publish(h, f, LidarRecord{}, n_points, last_offset_ms);
     cudaStream_t cs = h->copy_stream;
     const LidarFlags lf(h->lid_flags.p, n1);
     int* d_take = lf.own;
@@ -2572,7 +2844,7 @@ int lidar_features_core(flb_handle* h, const char* who, const LidarFmt& f, doubl
     FLB_CUDA(h, cudaMemcpyAsync(h->pin_lidar.p, d_count, sizeof(int), cudaMemcpyDeviceToHost, cs));
     FLB_CUDA(h, cudaStreamSynchronize(cs));
     std::memcpy(&M, h->pin_lidar.p, sizeof(int));
-    if (M == 0) return lidar_publish(h, LidarRecord{}, n_points, last_offset_ms);
+    if (M == 0) return lidar_publish(h, f, LidarRecord{}, n_points, last_offset_ms);
     const int gm = (M + 255) / 256;
     int lv = 1;
     while (lv < levels && (1 << lv) <= M) ++lv;
@@ -2595,7 +2867,7 @@ int lidar_features_core(flb_handle* h, const char* who, const LidarFmt& f, doubl
     k_feat_emit<<<gm, 256, 0, cs>>>(h->feat_pts.p, d_fin, d_rs2, d_lkey, d_lbeg, d_lend, d_lhead, M, min_size, f.filter_num,
                                     h->lid_dec.p, lf.kept);
     h->launches += 12 + 2 * lv;
-    return lidar_tail(h, who, "a point of pl_surf or its time", lf, M, t2, t3, nullptr, records, f.step, n_points, last_offset_ms);
+    return lidar_tail(h, who, "a point of pl_surf or its time", lf, M, t2, t3, nullptr, records, f, n_points, last_offset_ms);
 }
 
 }  // namespace
@@ -2606,6 +2878,7 @@ int flb_lidar_upload_features(flb_handle* h, const flb_lidar_format* fmt, double
     const char* who = "flb_lidar_upload_features";
     LidarFmt f;
     { int rcq = lidar_format(h, who, fmt, records, n_records, true, dis_b, &f); if (rcq) return rcq; }
+    f.off_int = kLidarIntZero;                                   // give_feature's pl_surf: fresh points, intensity 0 (:738-767)
     return lidar_features_core(h, who, f, dis_b, records, n_records, false, n_points, last_offset_ms);
 }
 
@@ -2616,6 +2889,7 @@ int flb_lidar_upload_velodyne_features(flb_handle* h, const flb_velodyne_format*
     LidarFmt f;
     bool given = false;
     { int rcq = velo_format(h, who, fmt, records, n_records, true, dis_b, &f, &given); if (rcq) return rcq; }
+    f.off_int = kLidarIntZero;
     const int rc = lidar_features_core(h, who, f, dis_b, records, n_records, !given, n_points, last_offset_ms);
     if (rc) return rc;
     if (yaw_times) *yaw_times = given ? 0 : 1;
@@ -2635,11 +2909,35 @@ int flb_lidar_download(flb_handle* h, float* xyzt, int capacity_points, int* n_o
     return FLB_OK;
 }
 
+int flb_lidar_download_points(flb_handle* h, void* points48, int capacity, int* n_out) {
+    FLB_CHECK_H(h);
+    if (capacity < 0 || (capacity > 0 && !points48)) return fail(h, FLB_ERR_INVALID, "flb_lidar_download_points: bad arguments");
+    if (h->lid_n < 0) return fail(h, FLB_ERR_STATE, "flb_lidar_download_points: no cloud (flb_lidar_upload_intensity)");
+    if (!h->lid_has_int)
+        return fail(h, FLB_ERR_STATE, "flb_lidar_download_points: the cloud carries no intensity (flb_lidar_upload or "
+                    "flb_lidar_upload_velodyne; the *_intensity and *_features calls keep it)");
+    if (n_out) *n_out = h->lid_n;
+    const int m = std::min(capacity, h->lid_n);
+    if (m > 0) {
+        FLB_CUDA(h, h->lid_pack.reserve(3 * (size_t)m));
+        {
+            LaunchScope ls(h, FAM_OTHER);
+            k_lidar_points48<<<(m + 255) / 256, 256, 0, h->stream>>>(h->lid_cloud.p, h->lid_int_zero ? nullptr : h->lid_int.p, m,
+                                                                    h->lid_pack.p);
+            FLB_CUDA(h, cudaGetLastError());
+        }
+        FLB_CUDA(h, cudaMemcpyAsync(points48, h->lid_pack.p, (size_t)m * 3 * sizeof(uint4), cudaMemcpyDeviceToHost, h->stream));
+        FLB_CUDA(h, cudaStreamSynchronize(h->stream));
+    }
+    return FLB_OK;
+}
+
 int flb_imu_undistort_lidar(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* carry, const flb_imu_sample* v_imu, int n_imu,
                             double pcl_beg_time, double pcl_end_time, double pcl_offset_time, int is_lidar_end, int* n_taken,
                             float* out_xyz, int capacity_points, double* poses_out, int* n_poses_out) {
     FLB_CHECK_H(h);
     h->undist_n = -1;
+    h->undist_has_int = false;
     if (!prm || !carry || !v_imu || n_imu < 1 || std::isnan(pcl_offset_time))
         return fail(h, FLB_ERR_INVALID, "flb_imu_undistort_lidar: bad arguments");
     if (h->lid_n < 0) return fail(h, FLB_ERR_STATE, "flb_imu_undistort_lidar: no cloud (flb_lidar_upload)");
@@ -2665,6 +2963,12 @@ int flb_imu_undistort_lidar(flb_handle* h, const flb_imu_params* prm, flb_imu_ca
     const int rc = imu_undistort_core(h, "flb_imu_undistort_lidar", prm, carry, v_imu, n_imu, pcl_beg_time, pcl_end_time, nullptr, 4, 3,
                                       h->lid_cloud.p + begin, taken, out_xyz, poses_out, n_poses_out);
     if (rc) return rc;
+    if (h->lid_has_int && taken > 0) {                                             // pcl_out's intensities, a copy
+        FLB_CUDA(h, h->undist_int.reserve(taken));
+        if (h->lid_int_zero) FLB_CUDA(h, cudaMemsetAsync(h->undist_int.p, 0, (size_t)taken * sizeof(float), h->stream));
+        else FLB_CUDA(h, cudaMemcpyAsync(h->undist_int.p, h->lid_int.p + begin, (size_t)taken * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+    }
+    h->undist_has_int = h->lid_has_int;
     h->lid_cursor = is_lidar_end ? 0 : begin + taken;                             // :638, :643-646
     if (n_taken) *n_taken = taken;
     return FLB_OK;
@@ -2806,7 +3110,9 @@ int flb_voxel_grid(flb_handle* h, const float* xyz, int n, int stride, float lea
 // The ordering runs on `scan_stream` into the slot that is NOT being read: updates of the previous frame still queued or
 // running on `stream` keep their scan, and -- because the persistent kernels leave one SM free and the ordering is one
 // block (k_scan_sort_block) -- this frame's upload overlaps them instead of queueing behind them.
-static int scan_install_dev(flb_handle* h, const float* xyz, int N, const float lo[3]) {
+//   carry_int: the idle set's scan_int_alt already holds the points' intensities in the caller's order (written on `stream`,
+// which orders it after every reader of the set's previous content).
+static int scan_install_dev(flb_handle* h, const float* xyz, int N, const float lo[3], bool carry_int) {
     const size_t n1 = (size_t)std::max(N, 1);
     const int cur = h->scan_slot, alt = cur ^ 1;
     cudaStream_t ss = h->scan_stream;
@@ -2880,6 +3186,9 @@ static int scan_install_dev(flb_handle* h, const float* xyz, int N, const float 
     std::swap(h->sel, h->sel_alt);
     std::swap(h->plane_ok, h->plane_ok_alt);
     std::swap(h->plane, h->plane_alt);
+    std::swap(h->scan_int, h->scan_int_alt);
+    h->scan_has_int_alt = h->scan_has_int;
+    h->scan_has_int = carry_int;
     h->scan_slot = alt;
     h->N = N;     // enqueue-only: everything later on this handle's stream is ordered after the upload
     h->scan_valid = true;
@@ -2908,7 +3217,7 @@ int flb_scan_upload(flb_handle* h, const float* body_xyz, int N, int stride) {
         FLB_CUDA(h, cudaMemcpyAsync(h->scan_raw.p, st, (size_t)N * 3 * sizeof(float), cudaMemcpyHostToDevice, h->scan_stream));
         if (!direct) FLB_CUDA(h, h->st_scan.mark(h->scan_stream));
     }
-    return scan_install_dev(h, h->scan_raw.p, N, lo);
+    return scan_install_dev(h, h->scan_raw.p, N, lo, false);
 }
 
 // downSizeFilterSurf.setInputCloud(feats_undistort); downSizeFilterSurf.filter(*feats_down_body) (src/laserMapping.cpp:
@@ -2954,6 +3263,14 @@ int flb_scan_from_undistorted(flb_handle* h, float leaf, int* n_out) {
         }
         const VgScratch vs{h->sf_keys.p, h->sf_keys_sorted.p, h->sf_vals.p, h->sf_vals_sorted.p, h->sf_heads.p, h->sf_heads.p + n, box};
         { int rcv = voxel_grid_dev(h, h->sf_xyz.p, n, leaf, vs, h->sf_down.p); if (rcv) return rcv; }
+        if (h->undist_has_int) {
+            FLB_CUDA(h, h->scan_int_alt.reserve(n));
+            LaunchScope ls(h, FAM_OTHER);
+            k_vg_intensity<<<(n + 255) / 256, 256, 0, h->stream>>>(h->undist_int.p, vs.keys_sorted, vs.vals_sorted, vs.head, vs.rank, n,
+                                                                  h->scan_int_alt.p);
+            FLB_CUDA(h, cudaGetLastError());
+            h->launches++;
+        }
         {
             LaunchScope ls(h, FAM_OTHER);
             k_cloud_bounds<<<(n + 255) / 256, 256, 0, h->stream>>>(h->sf_down.p, n, box + 7, rec_c);
@@ -2970,7 +3287,7 @@ int flb_scan_from_undistorted(flb_handle* h, float leaf, int* n_out) {
         float hi[3];
         scan_rec_bounds(rec + kSfRecCentroids, lo, hi);
     }
-    { int rci = scan_install_dev(h, h->sf_down.p, m, lo); if (rci) return rci; }
+    { int rci = scan_install_dev(h, h->sf_down.p, m, lo, h->undist_has_int); if (rci) return rci; }
     if (n_out) *n_out = m;
     return FLB_OK;
 }
@@ -4425,29 +4742,6 @@ int colorize_frame_check(flb_handle* h, const char* who, const uint8_t* bgr) {
     return FLB_OK;
 }
 
-// Chunks for `need` save records, their pointers uploaded to rs_table on `stream` (a table that grows is reallocated:
-// cudaFree waits for the scatters reading the old one).  *ok = false when the device has no memory for one more chunk:
-// the frame is then dropped like one beyond the cap; the chunks that were allocated stay for later frames.
-int rgb_save_reserve(flb_handle* h, long long need, bool* ok) {
-    const size_t want = (size_t)((need + (1LL << kRgbChunkLog2) - 1) >> kRgbChunkLog2);
-    while (h->rs_chunks.size() < want) {
-        uint4* c = nullptr;
-        if (cudaMalloc(&c, ((size_t)1 << kRgbChunkLog2) * sizeof(uint4)) != cudaSuccess) {
-            cudaGetLastError();                       // an allocation failure is not sticky: clear it
-            break;
-        }
-        h->rs_chunks.push_back(c);
-    }
-    if (h->rs_chunks.size() > h->rs_table_n) {
-        FLB_CUDA(h, h->rs_table.reserve(h->rs_chunks.size()));
-        FLB_CUDA(h, cudaMemcpyAsync(h->rs_table.p, h->rs_chunks.data(), h->rs_chunks.size() * sizeof(uint4*), cudaMemcpyHostToDevice,
-                                    h->stream));
-        h->rs_table_n = h->rs_chunks.size();
-    }
-    *ok = h->rs_chunks.size() >= want;
-    return FLB_OK;
-}
-
 }  // namespace
 
 extern "C" {
@@ -4519,20 +4813,15 @@ int flb_rgb_cloud(flb_handle* h, const double Rcw[9], const double Pcw[3], const
     FLB_CUDA(h, cudaStreamSynchronize(h->stream));
     const int m = *cnt;
     uint4* const* table = nullptr;
-    if (h->rs_on && m > 0) {
-        bool ok = m <= h->rs_max - h->rs_n;
-        if (ok) { int rcs = rgb_save_reserve(h, h->rs_n + m, &ok); if (rcs) return rcs; }
-        if (ok) table = h->rs_table.p;
-        else h->rs_dropped += m;                      // the frame's cloud is still built: saving never stops publishing
-    }
+    { int rcs = save_frame(h, h->rgb_save, m, &table); if (rcs) return rcs; }
     if (m > 0) {
         FLB_CUDA(h, h->rc_out.reserve(2 * (size_t)m));
         LaunchScope ls(h, FAM_OTHER);
         k_rgb_scatter<<<(n + 255) / 256, 256, 0, h->stream>>>(h->wc_xyz.p, h->rc_bgra.p, h->rc_flag.p, h->rc_pos.p, n, h->rc_out.p, table,
-                                                              h->rs_n);
+                                                              h->rgb_save.n);
         FLB_CUDA(h, cudaGetLastError());
     }
-    if (table) h->rs_n += m;
+    if (table) h->rgb_save.n += m;
     h->rc_n = m;
     if (n_out) *n_out = m;
     return FLB_OK;
@@ -4553,56 +4842,22 @@ int flb_rgb_cloud_download(flb_handle* h, void* points32, int capacity, int* n_o
 
 int flb_rgb_save_begin(flb_handle* h, int64_t max_points) {
     FLB_CHECK_H(h);
-    if (max_points < 1) return fail(h, FLB_ERR_INVALID, "flb_rgb_save_begin: max_points %lld < 1", (long long)max_points);
-    if (h->rs_on) return fail(h, FLB_ERR_STATE, "flb_rgb_save_begin: a save is open (flb_rgb_save_end first)");
-    h->rs_on = true;
-    h->rs_max = max_points;
-    h->rs_n = h->rs_dropped = 0;
-    return FLB_OK;
+    return save_begin(h, h->rgb_save, "flb_rgb_save", max_points);
 }
 
 int flb_rgb_save_size(flb_handle* h, int64_t* n, int64_t* dropped, int64_t* device_bytes) {
     FLB_CHECK_H(h);
-    if (!h->rs_on) return fail(h, FLB_ERR_STATE, "flb_rgb_save_size: no save open (flb_rgb_save_begin first)");
-    if (n) *n = h->rs_n;
-    if (dropped) *dropped = h->rs_dropped;
-    if (device_bytes)
-        *device_bytes = (int64_t)(h->rs_chunks.size() * ((size_t)1 << kRgbChunkLog2) * sizeof(uint4) + h->rs_table.cap * sizeof(uint4*) +
-                                  h->rs_pack.cap * sizeof(uint4));
-    return FLB_OK;
+    return save_size(h, h->rgb_save, "flb_rgb_save", n, dropped, device_bytes);
 }
 
 int flb_rgb_save_download(flb_handle* h, int64_t first, int64_t count, void* points32) {
     FLB_CHECK_H(h);
-    if (!h->rs_on) return fail(h, FLB_ERR_STATE, "flb_rgb_save_download: no save open (flb_rgb_save_begin first)");
-    if (first < 0 || count < 0 || count > h->rs_n - first || (count > 0 && !points32))
-        return fail(h, FLB_ERR_INVALID, "flb_rgb_save_download: bad arguments (records %lld + %lld of %lld)", (long long)first,
-                    (long long)count, h->rs_n);
-    if (count == 0) return FLB_OK;
-    // One bounded slice at a time: k_rgb_save_pack expands it into rs_pack, the copy takes it out; stream order keeps
-    // the next slice's pack behind the copy.
-    constexpr long long kSlice = 1LL << 18;
-    FLB_CUDA(h, h->rs_pack.reserve(2 * (size_t)std::min<long long>(count, kSlice)));
-    char* dst = static_cast<char*>(points32);
-    for (long long done = 0; done < count; done += kSlice) {
-        const int k = (int)std::min<long long>(count - done, kSlice);
-        {
-            LaunchScope ls(h, FAM_OTHER);
-            k_rgb_save_pack<<<(k + 255) / 256, 256, 0, h->stream>>>(h->rs_table.p, first + done, k, h->rs_pack.p);
-            FLB_CUDA(h, cudaGetLastError());
-        }
-        FLB_CUDA(h, cudaMemcpyAsync(dst + done * 2 * (long long)sizeof(uint4), h->rs_pack.p, (size_t)k * 2 * sizeof(uint4),
-                                    cudaMemcpyDeviceToHost, h->stream));
-    }
-    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    return FLB_OK;
+    return save_download(h, h->rgb_save, "flb_rgb_save", first, count, points32, 2, k_rgb_save_pack);
 }
 
 int flb_rgb_save_end(flb_handle* h) {
     FLB_CHECK_H(h);
-    FLB_CUDA(h, cudaStreamSynchronize(h->stream));
-    rgb_save_free(h);
-    return FLB_OK;
+    return save_end(h, h->rgb_save);
 }
 
 // LidarSelector::display_keypatch (src/lidar_selection.cpp:985-1005) without its text, into a copy of the current colour

@@ -1228,11 +1228,14 @@ FLB_HD int rgb_flag_point(const CamModel& cam, const double* Rcw, const double* 
     *bgra = ok ? rgb_bgra_word(c) : 0u;
     return ok ? 1 : 0;
 }
-// The save lives in chunks of 2^kRgbChunkLog2 16-byte records {x, y, z, bgra}; record i is entry i & mask of chunk i >> log2.
-constexpr int kRgbChunkLog2 = 20;
-FLB_HD rgb_word4* rgb_save_slot(rgb_word4* const* chunks, long long i, int chunk_log2) {
+// A save (flb_rgb_save_*, flb_lidar_save_*) lives in chunks of 2^kSaveChunkLog2 16-byte records; record i is entry
+// i & mask of chunk i >> log2.  The RGB save's record is {x, y, z, bgra}, the LiDAR save's {x, y, z, intensity}.
+constexpr int kSaveChunkLog2 = 20;
+constexpr int kRgbChunkLog2 = kSaveChunkLog2;
+FLB_HD rgb_word4* save_slot(rgb_word4* const* chunks, long long i, int chunk_log2) {
     return chunks[i >> chunk_log2] + (i & ((1LL << chunk_log2) - 1));
 }
+FLB_HD rgb_word4* rgb_save_slot(rgb_word4* const* chunks, long long i, int chunk_log2) { return save_slot(chunks, i, chunk_log2); }
 // The ABI's 32-byte record (pcl::PointXYZRGB): x, y, z, data[3] = 1.0f | bgra, three zero words; two 16-byte halves.
 FLB_HD void rgb_record32(unsigned x, unsigned y, unsigned z, unsigned bgra, rgb_word4* rec) {
     rgb_word4 a, b;
@@ -1255,6 +1258,47 @@ FLB_HD void rgb_scatter_point(const float* p, unsigned bgra, int slot, rgb_word4
 }
 // k_rgb_save_pack, one save record expanded to the 32-byte record.
 FLB_HD void rgb_save_expand(const rgb_word4& s, rgb_word4* rec) { rgb_record32(s.x, s.y, s.z, s.w, rec); }
+
+// ---- the LiDAR clouds as pcl::PointXYZINormal records: the raw cloud (pl_surf), publish_frame_world's pcl_wait_pub
+// (src/laserMapping.cpp:780-813, written by RGBpointBodyToWorld into a fresh PointCloudXYZI), the effect cloud
+// (laserCloudOri, :871-885) and the run's pcl_wait_save_lidar (:812).  Words again: an intensity is copied, never
+// computed on, so a NaN keeps its bits.
+// The 48-byte record: x, y, z, data[3] = 1.0f | normal_x, normal_y, normal_z, data_n[3] = 0 | intensity, curvature, 0, 0.
+FLB_HD void xyzi_record48(unsigned x, unsigned y, unsigned z, unsigned intensity, unsigned curvature, rgb_word4* rec) {
+    rgb_word4 a, b, c;
+    a.x = x; a.y = y; a.z = z; a.w = 0x3F800000u;
+    b.x = 0u; b.y = 0u; b.z = 0u; b.w = 0u;
+    c.x = intensity; c.y = curvature; c.z = 0u; c.w = 0u;
+    rec[0] = a;
+    rec[1] = b;
+    rec[2] = c;
+}
+// One point of the world or effect cloud at `slot` (curvature 0: the fresh point of :1763-1772 / :875) and,
+// chunks != NULL, its LiDAR-save record {x, y, z, intensity} at save_base + slot.
+FLB_HD void xyzi_scatter_point(const float* p, const float* intensity, int slot, rgb_word4* out, rgb_word4* const* chunks,
+                               long long save_base, int chunk_log2) {
+    const unsigned x = float_as_u32(p[0]), y = float_as_u32(p[1]), z = float_as_u32(p[2]), in = float_as_u32(*intensity);
+    xyzi_record48(x, y, z, in, 0u, out + 3 * (size_t)slot);
+    if (chunks) {
+        rgb_word4 s;
+        s.x = x; s.y = y; s.z = z; s.w = in;
+        *save_slot(chunks, save_base + slot, chunk_log2) = s;
+    }
+}
+// k_xyzi_save_pack, one LiDAR-save record expanded to the 48-byte record.
+FLB_HD void xyzi_save_expand(const rgb_word4& s, rgb_word4* rec) { xyzi_record48(s.x, s.y, s.z, s.w, 0u, rec); }
+// downSizeFilterSurf's leaf mean of the intensity (pcl::VoxelGrid with downsample_all_data_, :1398-1399) for the leaf
+// whose first sorted entry is i: the float sum in sorted order over float(count), as k_vg_centroids averages x, y, z.
+FLB_HD float vg_leaf_mean(const float* v, const unsigned* keys_sorted, const int* vals_sorted, int i, int n) {
+    const unsigned k = keys_sorted[i];
+    float s = 0.f;
+    int c = 0;
+    for (int j = i; j < n && keys_sorted[j] == k; ++j) {
+        s += v[vals_sorted[j]];
+        ++c;
+    }
+    return s / (float)c;
+}
 
 // The device-resident visual map: Point (include/point.h) and Feature (include/feature.h) flattened.
 constexpr int kVmMaxObs = 20;            // addObservation keeps obs_.size() < 20 before adding one (:946-952)
@@ -1756,10 +1800,14 @@ FLB_HD unsigned linear_v(int s0, int s1, int b0, int b1) { return (unsigned)((((
 // The non-feature (`else`) branches of the four handlers of src/preprocess.cpp, one driver record at a time
 // (flb_lidar_upload).  A record is `step` bytes; its fields sit at the byte offsets of LidarFmt.
 enum { kLidarLivox = 1, kLidarVelodyne = 2, kLidarOuster = 3, kLidarXt32 = 4 };
+// off_int: the intensity field (Livox: reflectivity, u8; the others: float32), kLidarIntZero for a cloud whose points all
+// read 0 (a message without a FLOAT32 intensity, give_feature's pl_surf), kLidarIntNone when the call keeps no intensity.
+enum { kLidarIntNone = -2, kLidarIntZero = -1 };
 struct LidarFmt {
     int kind, step, off_x, off_y, off_z, off_time, off_tag, off_line, n_scans, filter_num;
     double blind;
     double time_head;      // XT32: points[0].timestamp (:441)
+    int off_int;
 };
 struct LidarPoint { float x, y, z, t; };      // t: PointType::curvature, the offset from the scan start in ms
 
@@ -1819,6 +1867,14 @@ FLB_HD unsigned lidar_time_key(float t) {
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 FLB_HD bool lidar_finite(float v) { return (float_as_u32(v) & 0x7f800000u) != 0x7f800000u; }
+// The intensity of record r (f.off_int >= 0 or kLidarIntZero): Livox reflectivity as float (:148), the others' float32
+// intensity field as pcl::fromROSMsg copies it (:170, :266, :437), 0 without one.  Not checked for finiteness: the
+// reference publishes what the driver sent.
+FLB_HD float lidar_intensity(const unsigned char* r, const LidarFmt& f) {
+    if (f.off_int < 0) return 0.f;
+    if (f.kind == kLidarLivox) return (float)r[f.off_int];
+    return u32_as_float(lidar_ld32(r + f.off_int));
+}
 
 // ------------------------------------------------------------------ Velodyne times from the yaw angle
 // velodyne_handler's non-feature branch without per-point times (src/preprocess.cpp:376-428, flb_lidar_upload_velodyne).

@@ -735,6 +735,39 @@ __global__ void k_vg_centroids(const float* __restrict__ xyz, const unsigned* __
     o[0] = sx / fc; o[1] = sy / fc; o[2] = sz / fc;
 }
 
+// flb_scan_from_undistorted with an intensity: each leaf's mean intensity at its rank, over voxel_grid_dev's sorted keys.
+__global__ void __launch_bounds__(256) k_vg_intensity(const float* __restrict__ inten, const unsigned* __restrict__ keys_sorted,
+                                                      const int* __restrict__ vals_sorted, const int* __restrict__ head,
+                                                      const int* __restrict__ rank, int n, float* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && head[i]) out[rank[i]] = vg_leaf_mean(inten, keys_sorted, vals_sorted, i, n);
+}
+
+// flb_lidar_download_points: the current cloud {x, y, z, curvature} with its intensities (inten NULL: all 0) as 48-byte
+// records.
+__global__ void __launch_bounds__(256) k_lidar_points48(const float4* __restrict__ cloud, const float* __restrict__ inten, int n,
+                                                        uint4* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 q = cloud[i];
+    xyzi_record48(__float_as_uint(q.x), __float_as_uint(q.y), __float_as_uint(q.z), inten ? __float_as_uint(inten[i]) : 0u, __float_as_uint(q.w),
+                  out + 3 * (size_t)i);
+}
+
+// flb_world_cloud_points / flb_effect_cloud_download_points: packed xyz with its intensities as 48-byte records and,
+// chunks != NULL, the LiDAR-save records at save_base + i (xyzi_scatter_point).
+__global__ void __launch_bounds__(256) k_xyzi_scatter(const float* __restrict__ xyz, const float* __restrict__ inten, int n,
+                                                      uint4* __restrict__ out, uint4* const* __restrict__ chunks, long long save_base) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) xyzi_scatter_point(xyz + 3 * (size_t)i, inten + i, i, out, chunks, save_base, kSaveChunkLog2);
+}
+
+// flb_lidar_save_download: save records first .. first + count - 1 expanded to 48-byte records in out.
+__global__ void __launch_bounds__(256) k_xyzi_save_pack(uint4* const* __restrict__ chunks, long long first, int count, uint4* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < count) xyzi_save_expand(*save_slot(chunks, first + i, kSaveChunkLog2), out + 3 * (size_t)i);
+}
+
 // ---------------------------------------------------------------------------------------
 // scan preparation: Morton order in the BODY frame.  A rigid transform preserves spatial
 // neighbourhoods, so the lanes of a warp query neighbouring map cells at every pose: similar trip
@@ -3672,6 +3705,15 @@ __global__ void __launch_bounds__(256) k_lidar_order(const float4* __restrict__ 
     if (j >= m || j >= n) return;
     if (j > 0 && keys[j] < keys[j - 1]) rec->unsorted = 1;
     if (j == m - 1) rec->last = cloud[j].w;
+}
+
+// The intensity calls with an intensity field (f.off_int >= 0): each kept record's intensity at its rank, next to
+// k_lidar_scatter's point.
+__global__ void __launch_bounds__(256) k_lidar_intensity(const unsigned char* __restrict__ raw, int n, LidarFmt f,
+                                                         const int* __restrict__ kept, const int* __restrict__ pos,
+                                                         float* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && kept[i]) out[pos[i]] = lidar_intensity(raw + (size_t)i * f.step, f);
 }
 
 // After the sort: points.back().curvature.

@@ -198,7 +198,9 @@ int flb_imu_undistort(flb_handle* h, const flb_imu_params* prm, flb_imu_carry* c
  *     (:454); i % point_filter_num == 0 (:456); kept when the float sum of squares > blind, not its square (:458).
  * The kept points are then sorted by curvature (time_list).  std::sort leaves the order of equal times unspecified; here
  * it is the stable order (equal times keep record order).  Ties are real: the lines of a Livox fire together.
- * The cloud stays on the device as {x, y, z, curvature}; intensity is not kept (no device cloud carries it).
+ * The cloud stays on the device as {x, y, z, curvature}.  flb_lidar_upload keeps no intensity; flb_lidar_upload_intensity
+ * (below) keeps one float per point beside it, which follows the point through the sort, the window, the scan filter and
+ * the world and effect clouds.
  *
  * flb_lidar_upload: records = n_records records of fmt->point_step bytes (CustomMsg::points, or PointCloud2::data).
  * *n_points = pl_surf.size(), *last_offset_ms = points.back().curvature after the sort (0 for an empty cloud); either
@@ -230,6 +232,30 @@ int flb_lidar_upload(flb_handle* h, const flb_lidar_format* fmt, const void* rec
  * be NULL) = its size; xyzt may be NULL.  Blocking.  FLB_ERR_STATE without a cloud, FLB_ERR_INVALID when
  * capacity_points is below its size. */
 int flb_lidar_download(flb_handle* h, float* xyzt, int capacity_points, int* n_out);
+/* ---- intensity (publish_frame_world, pcl_wait_save_lidar, publish_effect_world) ---------------------------------------
+ * flb_lidar_upload with the intensity of every kept point, as pl_surf holds it: Livox reflectivity (u8 -> float, :148);
+ * for the other kinds the float32 `intensity` field that pcl::fromROSMsg copies (:170, :266, :437).  off_intensity: the
+ * field's byte offset within point_step (Livox: CustomPoint::reflectivity, 16; others: aligned to 4), or -1 for a message
+ * without a FLOAT32 intensity field, whose points PCL's field mapping leaves at 0.  The intensity is not checked: a
+ * non-finite one is kept, as the reference publishes it.  Everything else -- checks, bytes of x, y, z and curvature, the
+ * swap on success, the cursor reset -- is flb_lidar_upload's; FLB_ERR_INVALID also for an off_intensity that is neither -1
+ * nor a field that fits (and is aligned).
+ *   Which clouds carry an intensity: the *_intensity and the *_features calls (give_feature's pl_surf points are fresh,
+ * so their intensity is 0, :738-767), and what flb_imu_undistort_lidar, flb_scan_from_undistorted and flb_world_cloud /
+ * flb_effect_cloud make of such a cloud.  flb_lidar_upload, flb_lidar_upload_velodyne, flb_imu_undistort and
+ * flb_scan_upload give clouds without one.  flb_imu_undistort_lidar copies the window's intensities (a later upload does
+ * not change them); flb_scan_from_undistorted averages them per leaf as downSizeFilterSurf does (downsample_all_data_:
+ * the leaf's float sum in the leaf order of its x, y, z mean, over float(count)); flb_world_cloud takes the source's, in
+ * the caller's order.
+ *   The record outputs below are 48-byte pcl::PointXYZINormal records:
+ *     float x, y, z at 0 / 4 / 8; 1.0f at 12 (data[3]); bytes 16..31 zero (normal, data_n); float intensity at 32;
+ *     float curvature at 36 (the raw cloud's time offset; 0 for the world and effect clouds); bytes 40..47 zero.
+ * Each returns FLB_ERR_STATE when its cloud carries no intensity, and FLB_ERR_INVALID for capacity < 0 or a NULL
+ * buffer with capacity > 0; *n_out (may be NULL) = the cloud's size, and up to `capacity` records are written. */
+int flb_lidar_upload_intensity(flb_handle* h, const flb_lidar_format* fmt, int off_intensity, const void* records, int n_records,
+                               int* n_points, float* last_offset_ms);
+/* The current cloud as pl_surf holds it (curvature = time offset), blocking.  FLB_ERR_STATE also without a cloud. */
+int flb_lidar_download_points(flb_handle* h, void* points48, int capacity, int* n_out);
 /* UndistortPcl from :621 on with the device cloud as lidar_meas.lidar.  The window (:634-639): the points from the
  * handle's cursor on while (double)curvature <= pcl_offset_time, read in place; *n_taken (may be NULL) = pcl_out.size().
  * Then everything flb_imu_undistort does on those points, with the same outputs (out_xyz may be NULL; its capacity is
@@ -283,6 +309,10 @@ typedef struct flb_velodyne_format {
 } flb_velodyne_format;
 int flb_lidar_upload_velodyne(flb_handle* h, const flb_velodyne_format* fmt, const void* records, int n_records, int* n_points,
                               float* last_offset_ms, int* yaw_times);
+/* flb_lidar_upload_velodyne with intensities, as flb_lidar_upload_intensity: off_intensity is the float32 `intensity`
+ * field at any byte offset within point_step (as the other fields), or -1 (every point 0). */
+int flb_lidar_upload_velodyne_intensity(flb_handle* h, const flb_velodyne_format* fmt, int off_intensity, const void* records,
+                                        int n_records, int* n_points, float* last_offset_ms, int* yaw_times);
 
 /* ---- surface features (feature_extract_enable: 1) ------------------------------------------------------------------
  * The feature branches of Preprocess: avia_handler :94-135, oust64_handler :174-227 and velodyne_handler :299-373,
@@ -612,6 +642,20 @@ int flb_colorize(flb_handle* h, const double Rcw[9], const double Pcw[3], const 
 int flb_world_cloud(flb_handle* h, const struct flb_lio_params* prm, const double R[9], const double p[3], int source, int* n_out);
 /* publish_frame_world / the PCD save: up to `capacity` points of the world cloud, xyz floats (blocking). */
 int flb_world_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out);
+/* publish_frame_world's pcl_wait_pub (src/laserMapping.cpp:780-813, img_enable: 0) as 48-byte PointXYZINormal records
+ * (flb_lidar_upload_intensity's layout; curvature 0): one kernel packs them, then one copy, or none when points48 is
+ * NULL.  With a LiDAR save open (flb_lidar_save_begin) every successful call appends the frame's records to it (:812).
+ * FLB_ERR_STATE: no world cloud, or its source carries no intensity.  Blocking when points48 is given. */
+int flb_world_cloud_points(flb_handle* h, void* points48, int capacity, int* n_out);
+/* pcl_wait_save_lidar (`*pcl_wait_save_lidar += *pcl_wait_pub`, :812; written as intensity_sacn_all.pcd at exit,
+ * :1848-1853) on the device, with exactly the rules of flb_rgb_save_* (below) and the same store: a cap with whole
+ * frames dropped and counted, 16-byte records {x, y, z, intensity} in device chunks of 2^20 records, and a download that
+ * expands a slice to 48-byte records (flb_world_cloud_points' layout) through a bounded staging buffer.  The LiDAR save
+ * and the RGB save are independent: both may be open on one handle. */
+int flb_lidar_save_begin(flb_handle* h, int64_t max_points);
+int flb_lidar_save_size(flb_handle* h, int64_t* n, int64_t* dropped, int64_t* device_bytes);
+int flb_lidar_save_download(flb_handle* h, int64_t first, int64_t count, void* points48);
+int flb_lidar_save_end(flb_handle* h);
 
 /* ---- the effective points of the last LIO pass on the device (publish_effect_world) ------------------------------
  * publish_effect_world (src/laserMapping.cpp:871-885, called at :1776) publishes laserCloudOri -- the body points of the
@@ -628,7 +672,8 @@ int flb_world_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out
  * at the new pose (the reference republishes its stale laserCloudOri when the loop does not run: before flg_EKF_inited,
  * :1506, or with lidar_en off).  No pass ever: 0 points.  The scan, its row mask and its plane cache are double-buffered
  * together, so a pass's rows can be captured until the second scan upload after it (or an flb_voxel_grid, which uses
- * the scan slot as scratch); after that the call returns FLB_ERR_STATE until the next pass.  Intensity is not carried.
+ * the scan slot as scratch); after that the call returns FLB_ERR_STATE until the next pass.  When the pass's scan set
+ * carries intensities (flb_scan_from_undistorted of an intensity cloud), the capture keeps each row's intensity too.
  * Blocking.  *n_out (may be NULL) = points.  On any error no effect cloud is held.
  *   FLB_ERR_STATE: the pass's rows were replaced before capture, no pose given and no device state, after flb_comm_init
  *   / flb_p2p_attach (each rank holds only its shard of the scan).
@@ -637,6 +682,9 @@ int flb_effect_cloud(flb_handle* h, const struct flb_lio_params* prm, const doub
 /* pubLaserCloudEffect's points: up to `capacity` points of the effect cloud, xyz floats (blocking, as
  * flb_world_cloud_download).  FLB_ERR_INVALID for a bad capacity or buffer, FLB_ERR_STATE when no effect cloud is held. */
 int flb_effect_cloud_download(flb_handle* h, float* xyz, int capacity, int* n_out);
+/* The effect cloud as 48-byte PointXYZINormal records with the rows' intensities (curvature 0), blocking.
+ * FLB_ERR_STATE: no effect cloud, or its scan carried no intensity. */
+int flb_effect_cloud_download_points(flb_handle* h, void* points48, int capacity, int* n_out);
 /* flb_vmap_select / flb_vmap_grow / flb_colorize with pg = the world cloud: the same pose, enqueue and blocking rules and
  * byte-identical results to those calls on the host-transformed cloud.  flb_vmap_select_cloud applies downSizeFilter
  * (pcl::VoxelGrid with `leaf`, 0.2 in the reference: src/lidar_selection.cpp:7, :351-353; flb_voxel_grid's result) on
